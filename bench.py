@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — query images/sec of the OnePose++ 2D-3D matcher hot path on B200.
+"""bench.py — query images/sec of the OnePose++ 2D-3D matcher hot path on H100.
 
     python bench.py --gpus 1 --steps 20 --warmup 3            # our CUDA path, one JSON line
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...   # N > 1
     python bench.py --impl reference --steps K --warmup W      # reference CPU arm (oracle port)
+    python bench.py --steps K --dump-outputs DIR               # + the last timed step's outputs as DIR/*.npy
 
 A "step" is one forward of ``OnePosePlus_model`` over a batch of 512x512 query images against a
 5000-point planted descriptor bank (BASELINE.json configs[2]: batch 64 on one GPU; with N GPUs the
@@ -40,15 +41,44 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--profile-ops", action="store_true", help="print the per-op breakdown to stderr")
     ap.add_argument("--no-c5", action="store_true", help="skip the BASELINE configs[4] block")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (rank 0)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
+
+
+DUMP_BYTES = 60 * 10**6   # stays under 64 MB (decimal or binary) with the .npy headers
+
+
+def dump_outputs(d, inputs, out_dir, budget=DUMP_BYTES):
+    """Every tensor the forward added to the data dict, as float32 (floating outputs) or float64
+    (integer ids, exact).  Each output gets the same share of the budget, which depends only on how
+    many outputs there are.  An output larger than its share is replaced by a sample of its
+    flattened elements at indices drawn from a fixed seed (sorted); the indices are written next to
+    it as <name>_idx.npy (float64), so two builds given the same arguments write comparable files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    outs = sorted((k, v) for k, v in d.items() if torch.is_tensor(v) and k not in inputs)
+    share = budget // max(len(outs), 1)
+    for k, v in outs:
+        a = v.detach()
+        a = a.float() if a.is_floating_point() else a.double()
+        if a.numel() * a.element_size() > share:
+            n = share // (a.element_size() + 8)          # values + their float64 indices
+            g = torch.Generator().manual_seed(1234)
+            idx = torch.randint(0, a.numel(), (n,), generator=g).sort().values
+            np.save(os.path.join(out_dir, f"{k}_idx.npy"), idx.double().numpy())
+            a = a.reshape(-1)[idx.to(a.device)]
+        np.save(os.path.join(out_dir, f"{k}.npy"), a.cpu().numpy())
 
 
 # ---------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md: sample nvidia-smi DURING the timed region)
+# clocks sampler: SM clock and throttle reasons sampled DURING the timed region
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
-    """SM clock + throttle reasons of the GPU while the timed region runs (B200_PROFILING.md's clocks
-    line).  Read through NVML in this process (the counters nvidia-smi prints; a poll costs tens of
+    """SM clock + throttle reasons of the GPU while the timed region runs.  Read through NVML in this process (the counters nvidia-smi prints; a poll costs tens of
     microseconds) — a looping `nvidia-smi -lms 100` child was seen to slow the eager-mode timed region
     it overlapped by 5-8 % on some boxes (driver lock held during its queries) while the later,
     unsampled regions of the same run were not affected.  Falls back to `nvidia-smi -lms 200`."""
@@ -194,7 +224,7 @@ def run_reference(args, rank):
 # our arm
 # ---------------------------------------------------------------------------------------------
 def conv_flops_table(B, h=H, w=W, head=True):
-    """Algorithmic MACs of the tcgen05 conv launches of one backbone pass (true channel counts;
+    """Algorithmic MACs of the wgmma conv launches of one backbone pass (true channel counts;
     the 7x7 conv1 — 0.41 GMAC/image — is listed separately).  head=False: without
     layer1_outconv2, which the forward evaluates on the match windows only."""
     h2, h4, h8 = (h // 2) * (w // 2), (h // 4) * (w // 4), (h // 8) * (w // 8)
@@ -207,19 +237,6 @@ def conv_flops_table(B, h=H, w=W, head=True):
     if head:
         macs += h2 * 196 * 196 * 9 + h2 * 128 * 196 * 9                                # layer1_outconv2
     return 2.0 * macs * B
-
-
-def ncu_traffic(kernel_substr, launch_index):
-    """DRAM bytes (read + write) of one launch from the committed ncu capture at the bench batch
-    (profiles/r2_ncu_b64_raw.csv: kernel name, launch index, dram__bytes_read.sum, dram__bytes_write.sum),
-    or None when no capture at this batch is committed — never a scaled constant."""
-    path = os.path.join(ROOT, "profiles", "r2_ncu_b64_traffic.json")
-    try:
-        t = json.load(open(path))
-        e = t[kernel_substr][launch_index]
-        return e["dram_read_bytes"] + e["dram_write_bytes"]
-    except (OSError, KeyError, IndexError, ValueError):
-        return None
 
 
 def cuda_time(fn, reps, warm=2):
@@ -273,7 +290,7 @@ def bench_c5(model, sd, dev, workload, peaks, steps=5, batch=8):
         alg = batch * (n + S) * pl * 256 * 2 * 2 + (batch * n * S * 4 if mode == "eager" else 0)
         res[f"sim_passes_ms_conf_{mode}"] = ms
         res[f"sim_passes_hbm_gbs_conf_{mode}"] = alg / ms / 1e6
-        res[f"sim_passes_hbm_frac_conf_{mode}"] = alg / ms / 1e6 / peaks.get("hbm_gbs", 6562.6)
+        res[f"sim_passes_hbm_frac_conf_{mode}"] = alg / ms / 1e6 / peaks.get("hbm_gbs", 3350.0)
     res["note"] = ("sim-pass bytes = tokens read once per GEMM pass (2 passes) + the fp32 conf_matrix store when "
                    "materialised; 2*2*20000*4800*256 flop per image and pass on the tensor pipe (x3 issued)")
     model.conf_matrix_mode = "eager"
@@ -329,9 +346,10 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_burst = peaks.get("bf16_tflops", 1590.0)   # for a kernel timed alone (B200_PROFILING.md)
-    peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "fallback"
+    # fallback: the H100 SXM data sheet's dense FP16/BF16 rate (at 700 W; never reached as such)
+    peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+    peak_burst = peaks.get("bf16_tflops", 989.0)   # for a kernel timed alone
+    peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)" if peaks else "H100 SXM data sheet"
 
     B = args.batch
     sd = workload.synthetic_state_dict(0)
@@ -442,6 +460,8 @@ def main():
     _lib.LAUNCHES = 0
     ms, d, t0, t1 = timed(step_resident, args.steps, per_step=True)
     clocks = sampler.stop(t0, t1) if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(d, make_data(imgs_dev, scale_dev, bank), args.dump_outputs)
     launches = _lib.LAUNCHES
     m_per_img = d["b_ids"].numel() / B
 
@@ -539,7 +559,7 @@ def main():
         except Exception as e:  # noqa: BLE001  (auxiliary number: never lose the bench line over it)
             b1 = {"error": f"{type(e).__name__}: {str(e)[:200]}"}
 
-    # dominant kernel: the tcgen05 implicit-GEMM conv engine (21 launches / forward), timed live
+    # dominant kernel: the wgmma implicit-GEMM conv engine (21 launches / forward), timed live
     # with CUDA events around the backbone on the launching stream
     conv_ms = attn_ms = l1_ms = None
     S_tok = (H // 8) * (W // 8)
@@ -570,7 +590,7 @@ def main():
         wl1, bl1 = model._plan["layer1.0.conv1"]
         l1_ms = cuda_time(lambda: ops.conv2d_nhwc(x0, wl1, bl1, y0, 3, 1, model.split, act=1), 5, warm=3)
         # coarse attention (BASELINE.json "coarse-attn tensor-pipe %"): the 6-layer linear-attention
-        # transformer on both sequences (tcgen05 GEMM launches + the KV-state kernels), one object
+        # transformer on both sequences (wgmma GEMM launches + the KV-state kernels), one object
         # per image so that nothing is served from the per-object cache
         q2, _, (hc, wc) = model._backbone(imgs_dev, defer_fine=True)
         S_tok = hc * wc
@@ -617,13 +637,13 @@ def main():
             "value": total_imgs / (ms * 1e-3), "unit": "images/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "fp16 hi+lo operand pairs, 3 tcgen05 MMAs per K-step, fp32 accumulate (fp32-grade)"
+            "dtype": "fp16 hi+lo operand pairs, 3 wgmma MMAs per K-step, fp32 accumulate (fp32-grade)"
                      if model.split else "f16",
             "data": "synthetic (seeded weights, planted descriptor bank, noisy copies of one image)",
             "config": {"workload": f"BASELINE configs[2]/[3]: batch {B} images 512x512 per GPU vs shared "
                                    f"5000-pt bank (NCCL-broadcast once when N>1)",
                        "global_batch": B * world, "matches_per_image": m_per_img,
-                       "l2": "per-step working set (activations >= 1 GB) exceeds the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set (activations >= 1 GB) exceeds the 50 MB L2; no explicit flush",
                        "settle_steps": n_settle, "step_ms": step_ms,
                        "conf_matrix": "materialised fp32 every step (reference API); see conf_lazy for the "
                                       "store-free mode"},
@@ -646,15 +666,12 @@ def main():
             "roofline": {"bound": "tensor",
                          "kernel": "gemm_kernel<A_CONV,EpiConv>: layer1 3x3 conv 128->128 @256x256 (one launch, whole batch)",
                          "achieved": l1_tf, "peak": peak_burst, "unit": "TFLOP/s", "frac": l1_tf / peak_burst,
-                         "traffic": ncu_traffic("EpiConv", 0),   # launch 0 = layer1.0.conv1, the launch timed here
                          "peak_source": peak_src.replace("bf16_tflops_sustained", "bf16_tflops (burst: kernel timed alone)"), "ms_per_launch": l1_ms,
                          "algorithmic_flops_per_launch": l1_flops, "mma_passes": passes,
                          "issued_tensor_tflops": l1_tf * passes, "issued_frac": l1_tf * passes / peak_burst,
                          "note": "achieved = algorithmic flops (2*B*256*256*128*128*9, reference fp32 math) / CUDA-event "
-                                 "time of the launch; the fp32-grade mode issues mma_passes x that on the tensor pipe; "
-                                 "traffic = dram read+write of this launch from the committed ncu --set full capture at "
-                                 "this batch (profiles/r2_ncu_b64_traffic.json), null when absent",
-                         "backbone": {"kernels": "conv1 im2col + 20 tcgen05 GEMM launches (FPN upsample-adds fused), without layer1_outconv2",
+                                 "time of the launch; the fp32-grade mode issues mma_passes x that on the tensor pipe",
+                         "backbone": {"kernels": "conv1 im2col + 20 wgmma GEMM launches (FPN upsample-adds fused), without layer1_outconv2",
                                       "ms": conv_ms, "fine_head": fine_head,
                                       "algorithmic_tflops": ach, "frac": ach / peak_tf if ach else None,
                                       "issued_frac": ach * passes / peak_tf if ach else None}},
@@ -662,8 +679,7 @@ def main():
                 "kernels": "gemm_kernel<A_ROWS,{EpiStoreF16,EpiQ,EpiLN}> x60 + kv_partial/kv_finalize x12",
                 "ms": attn_ms, "algorithmic_tflops": attn_tf, "issued_tensor_tflops": attn_tf * passes,
                 "frac_of_peak_algorithmic": attn_tf / peak_tf, "frac_of_peak_issued": attn_tf * passes / peak_tf,
-                "flops_per_image": "(4096 + 5000) tokens x 6 layers x 10*d^2 MAC + KV/QKV contractions = 72.6 GFLOP",
-                "tensor_pipe_pct_ncu": "sm__pipe_tensor_cycles_active per launch at this batch: profiles/r2_ncu_xfmr_b64.md"},
+                "flops_per_image": "(4096 + 5000) tokens x 6 layers x 10*d^2 MAC + KV/QKV contractions = 72.6 GFLOP"},
             "configs": {"c5": c5, "loftr_2d2d": loftr},
             "pose_stage": pose,
             "latency_b1": b1,

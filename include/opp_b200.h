@@ -1,4 +1,4 @@
-/* opp_b200.h — C ABI of libopp_b200.so: the B200 (sm_100a) kernels behind the OnePose++ 2D-3D
+/* opp_b200.h — C ABI of libopp_b200.so: the H100 (sm_90a) kernels behind the OnePose++ 2D-3D
  * coarse-to-fine matcher, `OnePosePlus_model.forward` (reference:
  * src/models/OnePosePlus/OnePosePlusModel.py:96-201).
  *
@@ -36,7 +36,7 @@ int opp_num_sms(void);
 
 /* ------------------------------------------------------------------------------------------
  * Backbone — ResNetFPN_8_2.forward (backbone/resnet.py:141-164), BatchNorm folded on the host;
- * every convolution runs on the tcgen05 engine, the two bilinear x2 upsample-adds of the FPN are
+ * every convolution runs on the wgmma engine, the two bilinear x2 upsample-adds of the FPN are
  * epilogues of the lateral 1x1 convolutions
  * ---------------------------------------------------------------------------------------- */
 
@@ -49,7 +49,7 @@ int opp_num_sms(void);
 int opp_conv1_im2col(const void* image, int image_u8, void* a_out, int batch, int h, int w, int split,
                      opp_stream_t stream);
 
-/* 3x3 (pad 1) or 1x1 (pad 0) convolution, stride 1 or 2, as a tcgen05 implicit GEMM
+/* 3x3 (pad 1) or 1x1 (pad 0) convolution, stride 1 or 2, as a wgmma implicit GEMM
  * (resnet.py:10-17 conv1x1/conv3x3; BasicBlock resnet.py:36-45; FPN heads resnet.py:109-124).
  *   in    NHWC fp16 [B][in_h][in_w][c_in_pad]
  *   w     fp16 [c_out_pad][planes][ksize*ksize][c_in_pad]   (BN-folded, zero in the padding)
@@ -106,7 +106,7 @@ int opp_kpt_encode(const float* kpts, const float* stats, const float* desc, con
 
 /* ------------------------------------------------------------------------------------------
  * Transformer — LoFTREncoderLayer.forward (loftr_module/transformer.py:65-94) and
- * LinearAttention.forward (loftr_module/linear_attention.py:29-61), tcgen05 GEMMs
+ * LinearAttention.forward (loftr_module/linear_attention.py:29-61), wgmma GEMMs
  * ---------------------------------------------------------------------------------------- */
 
 /* out[rows][n] = act(concat_K(a0[rows][k0], a1[rows][k1]) @ w[n][k0+k1]^T), fp16 in/out.

@@ -1,4 +1,4 @@
-"""onepose_plus_plus_b200 — B200 (sm_100a) implementation of the OnePose++ 2D-3D matcher hot path.
+"""onepose_plus_plus_b200 — H100 (sm_90a) implementation of the OnePose++ 2D-3D matcher hot path.
 
 ``OnePosePlus_model`` mirrors the reference class of the same name
 (src/models/OnePosePlus/OnePosePlusModel.py) and runs on hand-written CUDA kernels through the

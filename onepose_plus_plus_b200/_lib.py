@@ -72,7 +72,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; "
-            "g.build()'` (nvcc, sm_100a). There is no CPU/PyTorch fallback for this path.")
+            "g.build()'` (nvcc, sm_90a). There is no CPU/PyTorch fallback for this path.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, argtypes in SIGNATURES.items():
         _sig(getattr(lib, name), argtypes)

@@ -1,11 +1,11 @@
 #!/bin/bash
-# Builds libopp_b200.so (sm_100a only) next to the Python package. Usage: build.sh [extra nvcc flags]
+# Builds libopp_b200.so (sm_90a only) next to the Python package. Usage: build.sh [extra nvcc flags]
 set -e
 HERE="$(cd "$(dirname "$0")" && pwd)"
 OUT="${OPP_OUT:-$HERE/../libopp_b200.so}"
 OBJ="${OPP_OBJ:-$HERE/obj}"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-std=c++17 -O3 -lineinfo -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC -Xcompiler -Wall --expt-relaxed-constexpr"
+FLAGS="-std=c++17 -O3 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC -Xcompiler -Wall --expt-relaxed-constexpr"
 mkdir -p "$OBJ"
 pids=()
 for f in opp_gemm opp_stages opp_pnp; do
@@ -13,5 +13,5 @@ for f in opp_gemm opp_stages opp_pnp; do
   pids+=($!)
 done
 for p in "${pids[@]}"; do wait $p; done
-$NVCC -shared -gencode arch=compute_100a,code=sm_100a -o "$OUT" "$OBJ/opp_gemm.o" "$OBJ/opp_stages.o" "$OBJ/opp_pnp.o"
+$NVCC -shared -gencode arch=compute_90a,code=sm_90a -o "$OUT" "$OBJ/opp_gemm.o" "$OBJ/opp_stages.o" "$OBJ/opp_pnp.o"
 echo "built $OUT"

@@ -1,4 +1,4 @@
-// opp_gemm.cu — host launchers (C-ABI) for the tcgen05 GEMM / implicit-GEMM conv engine.
+// opp_gemm.cu — host launchers (C-ABI) for the wgmma GEMM / implicit-GEMM conv engine.
 //
 // Every entry point takes raw device pointers + sizes + a cudaStream_t, builds the TMA tensor
 // maps for the call, and launches one persistent kernel.  No allocation, no synchronisation.
@@ -48,8 +48,8 @@ int num_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 132;
   }
   return n;
 }
@@ -103,7 +103,6 @@ template <int A_MODE, class Epi, bool DYN = false>
 static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Params& ep,
                   cudaStream_t stream, const int* rows_dev = nullptr, int rows_mult = 1) {
   constexpr int kEpiBytes = epi_smem_bytes<Epi>();
-  s.stages = gemm_pick_stages(s.block_n, s.k_chunks, s.split, s.pair == 1, kEpiBytes);
   {
     static int dbg = -1;
     if (dbg < 0) {
@@ -116,9 +115,10 @@ static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Param
       const char* e = getenv("OPP_STAGES");
       cap = e ? atoi(e) : 0;
     }
-    if (cap > 1 && s.stages > cap) s.stages = cap;
+    OPP_REQUIRE(s.mma_n > 0 && gemm_pick_stages(s, kEpiBytes, cap),
+                "GEMM tile N=%d (split %d) does not fit in shared memory", s.block_n, s.split);
   }
-  const int smem = gemm_smem_bytes(s.stages, s.block_n, s.split, s.pair == 1, kEpiBytes);
+  const int smem = gemm_smem_bytes(s, kEpiBytes);
   const void* kern;
   if constexpr (DYN) kern = (const void*)gemm_kernel_dyn<A_MODE, Epi>;
   else kern = (const void*)gemm_kernel<A_MODE, Epi>;
@@ -153,9 +153,9 @@ static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Param
   cudaError_t le = cudaLaunchKernelExC(&cfg, kern, kargs);
   if (le != cudaSuccess) {
     set_last_error("cudaLaunchKernelEx failed: %s (grid %d cluster %d pair %d smem %d stages %d "
-                   "block_n %d m_tiles %d n_tiles %d batches %d)",
+                   "acc_alias %d block_n %d m_tiles %d n_tiles %d batches %d)",
                    cudaGetErrorString(le), n_clusters * s.cluster, s.cluster, s.pair, smem, s.stages,
-                   s.block_n, s.m_tiles, s.n_tiles, s.batches);
+                   s.acc_alias, s.block_n, s.m_tiles, s.n_tiles, s.batches);
     return OPP_ERR_CUDA;
   }
   return OPP_OK;
@@ -163,26 +163,10 @@ static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Param
 
 static int pick_cluster(int block_n, int m_tiles);
 
-// $OPP_PAIR=0 disables the cta_group::2 (CTA pair) mode
-static int pair_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("OPP_PAIR");
-    v = e ? atoi(e) : 1;
-  }
-  return v;
-}
-
-// decide the CTA grouping of a GEMM: a cta_group::2 pair (256 x N tiles) when there are at least
-// two M tiles, else a multicast cluster / single CTAs
+// decide the CTA grouping of a GEMM: a multicast cluster sharing the W tile, or single CTAs
 static void pick_grouping(GemmShape& s) {
-  if (pair_enabled() && s.m_tiles >= 2 && s.block_n % 16 == 0) {
-    s.pair = 1;
-    s.cluster = 2;
-  } else {
-    s.pair = 0;
-    s.cluster = pick_cluster(s.block_n, s.m_tiles);
-  }
+  s.pair = 0;
+  s.cluster = pick_cluster(s.block_n, s.m_tiles);
   s.msup = (s.m_tiles + s.cluster - 1) / s.cluster;
 }
 
@@ -193,22 +177,19 @@ static int pick_cluster(int block_n, int m_tiles) {
     const char* e = getenv("OPP_CLUSTER");
     forced = e ? atoi(e) : 0;
   }
-  // The kernel contains cta_group::2 code paths, and such kernels cannot be launched with a
-  // cluster size of 1 (cudaErrorInvalidClusterSize): the minimum is a 2-CTA multicast cluster,
-  // whose second CTA simply finds its M tile out of range when there is only one.
   int c = forced > 1 ? forced : 2;
-  while (c > 2 && (block_n % (8 * c) != 0 || m_tiles < c)) c >>= 1;
+  while (c > 1 && (block_n % (8 * c) != 0 || m_tiles < c)) c >>= 1;
   return c;
 }
 
 static int pick_block_n(int n) {
-  if (n <= 256) return (n + 15) & ~15;  // single tile (UMMA N is a multiple of 16)
+  if (n <= 256) return (n + 15) & ~15;  // single tile
   if (n % 256 == 0) return 256;
   if (n % 128 == 0) return 128;
   return 256;
 }
 
-// Latency shapes (batch 1-2: a GEMM has fewer super tiles than half the SMs, e.g. 16 CTA pairs
+// Latency shapes (batch 1-2: a GEMM has fewer super tiles than half the SMs, e.g. 16 clusters
 // for 4096 tokens): halve the N tile, down to 64 columns, so that 2-4x as many SMs share the MMAs
 // and the epilogue of the same output.  A is re-read once per N tile — a few hundred KB from L2.
 // Call after pick_grouping() and before the W map is built.  $OPP_NSPLIT=0 disables it.
@@ -245,6 +226,23 @@ static void ln_nsplit_cluster(GemmShape& s) {
   s.block_n = 128;
   s.n_tiles = 1;
 }
+
+// The fp32 accumulator tile lives in shared memory, beside the operand ring or over it: narrow the
+// N tile until ring, accumulator and epilogue scratch fit.  Sets mma_n; call before the W map is
+// built (its box is mma_n / cluster rows).
+static int fit_tile(GemmShape& s, int epi_bytes) {
+  for (;;) {
+    s.mma_n = (s.block_n + kWgmmaN - 1) / kWgmmaN * kWgmmaN;
+    GemmShape t = s;
+    if (gemm_pick_stages(t, epi_bytes)) return OPP_OK;
+    OPP_REQUIRE(s.pair == 0 && s.block_n > 16, "GEMM tile N=%d (split %d) does not fit in shared memory",
+                s.block_n, s.split);
+    s.block_n = (s.block_n / 2 + 15) & ~15;
+    s.n_tiles = (s.n_total + s.block_n - 1) / s.block_n;
+  }
+}
+// the largest epilogue scratch of the token-row GEMMs (EpiLN: DSMEM exchange slots on top)
+constexpr int kRowsEpiBytes = epi_smem_bytes<EpiLN>();
 
 // common shape / map setup for token-row GEMMs.  With split, every operand row holds two planes:
 // A_i rows are [hi(k_i) | lo(k_i)], W rows are [hi(k0+k1) | lo(k0+k1)].
@@ -288,9 +286,11 @@ static int setup_rows(TensorMaps& maps, GemmShape& s, const void* a0, int k0, co
   pick_grouping(s);
   if (nsplit_ok == 1) split_n_for_latency(s);
   if (nsplit_ok == 2) ln_nsplit_cluster(s);
+  rc = fit_tile(s, kRowsEpiBytes);
+  if (rc) return rc;
   const long long kt = (long long)planes * (k0 + k1);
   return map_rows(&maps.b, w, kt, n, w_batched ? batches : 1, kt, (long long)n * kt,
-                  s.pair == 2 ? s.block_n : s.block_n / s.cluster);
+                  s.pair == 2 ? s.mma_n : s.mma_n / s.cluster);
 }
 
 }  // namespace opp
@@ -363,6 +363,7 @@ int opp_linear_ln_dyn(const void* a0, int k0, const void* a1, int k1, const void
   OPP_REQUIRE(n == 128 || n == 256, "LayerNorm epilogue needs N in {128,256}, got %d", n);
   int rc = setup_rows(maps, s, a0, k0, a1, k1, w, 0, 1, cap_rows, n, split);
   if (rc) return rc;
+  OPP_REQUIRE(s.n_tiles == 1 && s.block_n == n, "LayerNorm row of N=%d split across tiles", n);
   OPP_REQUIRE(gamma && beta && count && rows_per_count > 0, "bad dynamic-row arguments");
   OPP_REQUIRE(out16 || out32, "no output requested");
   EpiLN::Params ep{gamma, beta, eps, (const __half*)resid, 0, (__half*)out16,
@@ -394,6 +395,9 @@ int opp_linear_ln(const void* a0, int k0, const void* a1, int k1, const void* w,
   OPP_REQUIRE(n == 128 || n == 256, "LayerNorm epilogue needs N in {128,256}, got %d", n);
   int rc = setup_rows(maps, s, a0, k0, a1, k1, w, w_batched, batches, rows, n, split, 16, 0, 2);
   if (rc) return rc;
+  // EpiLN needs whole rows in one CTA, or the two halves of the N-split cluster
+  OPP_REQUIRE(s.n_tiles == 1 && s.block_n * (s.pair == 2 ? 2 : 1) == n,
+              "LayerNorm row of N=%d split across tiles", n);
   OPP_REQUIRE(gamma && beta, "null LayerNorm parameters");
   OPP_REQUIRE(out16 || out32, "no output requested");
   EpiLN::Params ep{gamma, beta, eps, (const __half*)resid, resid_shared, (__half*)out16,
@@ -439,25 +443,27 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   s.out_w = out_w;
   s.out_h = out_h;
   s.split = split ? 1 : 0;
+  // A maps are 5-D (channel, plane, x, y, image) with channel extent c_in_pad: the last 64-channel
+  // box of a row reads zeros past c_in_pad, so every K chunk is 4 full MMA steps
   const long long C = (long long)planes * c_in_pad;  // pixel stride in elements
   const __half* base = (const __half*)in;
   int rc;
   if (stride == 1) {
-    uint64_t dims[4] = {(uint64_t)C, (uint64_t)in_w, (uint64_t)in_h, (uint64_t)batch};
-    uint64_t str[3] = {(uint64_t)C, (uint64_t)(in_w * C), (uint64_t)((long long)in_h * in_w * C)};
-    uint32_t box[4] = {64, (uint32_t)s.tile_w, (uint32_t)s.tile_h, 1};
-    rc = make_map(&maps.a[0], base, 4, dims, str, box);
+    uint64_t dims[5] = {(uint64_t)c_in_pad, (uint64_t)planes, (uint64_t)in_w, (uint64_t)in_h, (uint64_t)batch};
+    uint64_t str[4] = {(uint64_t)c_in_pad, (uint64_t)C, (uint64_t)(in_w * C), (uint64_t)((long long)in_h * in_w * C)};
+    uint32_t box[5] = {64, 1, (uint32_t)s.tile_w, (uint32_t)s.tile_h, 1};
+    rc = make_map(&maps.a[0], base, 5, dims, str, box);
     if (rc) return rc;
     maps.a[1] = maps.a[2] = maps.a[3] = maps.a[0];
   } else {
     for (int py = 0; py < 2; ++py)
       for (int px = 0; px < 2; ++px) {
-        uint64_t dims[4] = {(uint64_t)C, (uint64_t)(in_w / 2), (uint64_t)(in_h / 2),
-                            (uint64_t)batch};
-        uint64_t str[3] = {(uint64_t)(2 * C), (uint64_t)(2LL * in_w * C),
+        uint64_t dims[5] = {(uint64_t)c_in_pad, (uint64_t)planes, (uint64_t)(in_w / 2),
+                            (uint64_t)(in_h / 2), (uint64_t)batch};
+        uint64_t str[4] = {(uint64_t)c_in_pad, (uint64_t)(2 * C), (uint64_t)(2LL * in_w * C),
                            (uint64_t)((long long)in_h * in_w * C)};
-        uint32_t box[4] = {64, (uint32_t)s.tile_w, (uint32_t)s.tile_h, 1};
-        rc = make_map(&maps.a[py * 2 + px], base + ((long long)py * in_w + px) * C, 4, dims, str,
+        uint32_t box[5] = {64, 1, (uint32_t)s.tile_w, (uint32_t)s.tile_h, 1};
+        rc = make_map(&maps.a[py * 2 + px], base + ((long long)py * in_w + px) * C, 5, dims, str,
                       box);
         if (rc) return rc;
       }
@@ -466,8 +472,10 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   s.b_lo = (int)kplane;
   const long long kt = kplane * planes;
   pick_grouping(s);
-  split_n_for_latency(s);   // the 1/8-resolution layers at batch 1: 16 CTA pairs -> 64
-  rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.block_n / s.cluster);
+  split_n_for_latency(s);   // the 1/8-resolution layers at batch 1: 16 clusters -> 64
+  rc = fit_tile(s, up ? epi_smem_bytes<EpiConvUp>() : epi_smem_bytes<EpiConv>());
+  if (rc) return rc;
+  rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.mma_n / s.cluster);
   if (rc) return rc;
   OPP_REQUIRE(!up || (out_h % 2 == 0 && out_w % 2 == 0 && out_h >= 4 && out_w >= 4),
               "fused upsample-add needs even output dims >= 4 (got %d x %d)", out_h, out_w);
@@ -533,10 +541,10 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
   int rc;
   {
     const uint64_t iw = j_ids ? in_w : 8, ih = j_ids ? in_h : win + 2, ib = j_ids ? batch : matches;
-    uint64_t dims[4] = {(uint64_t)C, iw, ih, ib};
-    uint64_t str[3] = {(uint64_t)C, (uint64_t)(iw * C), (uint64_t)(ih * iw * C)};
-    uint32_t box[4] = {64, (uint32_t)pitch, (uint32_t)win, 1};
-    rc = make_map(&maps.a[0], in, 4, dims, str, box);
+    uint64_t dims[5] = {(uint64_t)c_in_pad, (uint64_t)planes, iw, ih, ib};   // 5-D: see opp_conv2d_nhwc
+    uint64_t str[4] = {(uint64_t)c_in_pad, (uint64_t)C, (uint64_t)(iw * C), (uint64_t)(ih * iw * C)};
+    uint32_t box[5] = {64, 1, (uint32_t)pitch, (uint32_t)win, 1};
+    rc = make_map(&maps.a[0], in, 5, dims, str, box);
     if (rc) return rc;
     maps.a[1] = maps.a[2] = maps.a[3] = maps.a[0];
   }
@@ -544,7 +552,9 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
   s.b_lo = (int)kplane;
   const long long kt = kplane * planes;
   pick_grouping(s);
-  rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.block_n / s.cluster);
+  rc = fit_tile(s, epi_smem_bytes<EpiWin>());
+  if (rc) return rc;
+  rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.mma_n / s.cluster);
   if (rc) return rc;
   EpiWin::Params ep{(__half*)out, (long long)c_out_pad * planes, split ? c_out_pad : 0, bias, act, slope,
                     b_ids, j_ids, wc, stride, org, in_h, in_w};

@@ -1,9 +1,8 @@
 // opp_gemm.cuh — the one tensor-core engine of the hot path.
 //
-// D[M,N] = A[M,K] * W[N,K]^T on tcgen05 (fp16 operands, fp32 accumulators in TMEM), operands
-// staged by TMA into 128B-swizzled shared memory through an mbarrier ring, persistent over
-// output tiles with a double-buffered TMEM accumulator so the epilogue of tile i overlaps the
-// MMAs of tile i+1.
+// D[M,N] = A[M,K] * W[N,K]^T on wgmma (fp16 operands, fp32 accumulators), operands staged by TMA
+// into 128B-swizzled shared memory through an mbarrier ring, persistent over output tiles.  The
+// producer warp keeps loading the next tile's operands while the epilogue of the current one runs.
 //
 // Precision: the reference computes in fp32 and the parity bar is 1e-3 on outputs whose logits
 // reach ~1e2, so single fp16 operands (2^-11) are not enough.  In `split` mode every operand is a
@@ -20,9 +19,10 @@
 // Everything after the accumulator (bias / BN / activation / residual / LayerNorm / elu+1 /
 // linear-attention normaliser / dual-softmax statistics) is a fused epilogue functor.
 //
-// Warp roles (64 + 128*groups threads): warps 0..4g-1 = epilogue (warp w owns TMEM lanes
-// 32*(w%4) .. +31, one row per thread; two groups take alternate 32-column chunks), then the TMA
-// producer warp and, with the highest id, the TMEM owner + MMA issuer warp.
+// Warp roles (32 + 256 threads): two warpgroups, then the TMA producer warp.  Warpgroup g issues
+// the wgmmas of tile rows 64g .. 64g+63 into its registers, writes them to the fp32 accumulator
+// tile in shared memory, and then runs the epilogue as epilogue group g: warp w owns accumulator
+// rows 32*(w%4) .. +31, one row per thread, and the two groups take alternate 32-column chunks.
 //
 // Reference semantics implemented by the epilogues are cited at each functor
 // (paths relative to the reference repo zju3dv/OnePose_Plus_Plus).
@@ -36,7 +36,7 @@
 #define OPP_CONV_GROUPS 2
 #endif
 #ifndef OPP_LN_GROUPS
-#define OPP_LN_GROUPS 2   // two groups + register-lean TMEM walk: no spills at the 168-register cap
+#define OPP_LN_GROUPS 2
 #endif
 #ifndef OPP_ROW_GROUPS
 #define OPP_ROW_GROUPS 2   // EpiStoreF16 / EpiQ / EpiLse / EpiConf
@@ -50,8 +50,7 @@
 #define OPP_CONF_STAGED 1
 #endif
 // BasicBlock residual of the conv epilogue through the transpose buffer (coalesced) instead of
-// row-per-thread 16 B loads.  A/B at batch 64 (profiles/r2_ab_resid_staged.md): conv2d 41.7 -> 40.8 ms,
-// kernel checks + golden + C5 parity green, no register spills (4 bytes before) -> on.
+// row-per-thread 16 B loads.
 #ifndef OPP_CONV_RESID_STAGED
 #define OPP_CONV_RESID_STAGED 1
 #endif
@@ -68,9 +67,9 @@ constexpr int kABytes = kBlockM * kBlockK * 2;
 constexpr int kMaxStages = 8;
 constexpr int kEpiParamBytes = 4096;   // bias / gamma,beta / lse vectors: 2 KB per epilogue group
 constexpr int kMaxEpiWarps = 8;
-constexpr int kEpiSmemBytes = kEpiParamBytes + kMaxEpiWarps * 2560;   // + transpose buffer per warp
-// 64 threads (producer + MMA warps) + 128 per epilogue warp group (Epi::kGroups = 1 or 2)
-constexpr int gemm_threads(int groups) { return 64 + 128 * groups; }
+// two MMA / epilogue warpgroups (Epi::kGroups must be 2) + the producer warp
+constexpr int gemm_threads(int groups) { return 32 + 128 * groups; }
+constexpr int kWgmmaN = 64;               // N of one wgmma; an N tile is 1..4 of them
 
 enum AMode : int { A_ROWS = 0, A_CONV = 1, A_WIN = 2 };
 
@@ -85,7 +84,8 @@ struct GemmShape {
   int m_tiles;      // M tiles per batch
   int n_tiles;
   int n_total;      // valid output columns
-  int block_n;      // UMMA N (multiple of 16, <= 256)
+  int block_n;      // output columns per tile (multiple of 16, <= 256)
+  int mma_n;        // block_n rounded up to kWgmmaN: W rows staged per tile and accumulator width
   int k_chunks;     // number of 64-wide K chunks per tile (per plane)
   int stages;
   int b_batched;    // W operand has a leading batch dim
@@ -94,9 +94,9 @@ struct GemmShape {
   int msup;         // ceil(m_tiles / cluster)
   int pair;         // 2: "N-split cluster" (latency shapes of the LayerNorm GEMMs): the two CTAs of the
                     // cluster work on the SAME 128-row M tile, CTA r on columns [r*block_n, +block_n),
-                    // independent pipelines, row statistics exchanged through DSMEM (EpiLN);
-                    // 1: the two CTAs of the cluster form ONE cta_group::2 MMA: 256 x N tile, each
-                    // CTA holds 128 rows of A, N/2 rows of W and 128 rows of the accumulator
+                    // independent pipelines, row statistics exchanged through DSMEM (EpiLN); else 0
+  int acc_alias;    // the accumulator tile overlays the operand ring (it does not fit beside it):
+                    // the producer starts a tile's loads only after the previous epilogue is done
   int debug_skip;   // TIMING EXPERIMENTS ONLY ($OPP_DEBUG_SKIP): 1 = skip W loads, 2 = skip A loads
   int split;        // operands are (hi|lo) plane pairs; 3 MMAs per K-step
   int b_lo;         // element offset of W's lo plane inside a row (= K total)
@@ -120,9 +120,10 @@ struct GemmShape {
 };
 
 struct EpiCtx {
-  uint32_t tmem;   // accumulator address of this thread's lane quarter, column 0 of the tile
+  uint32_t acc;    // shared-memory word address (byte address / 4) of column 0 of this thread's
+                   // accumulator row
   int b, m_tile, n_tile;
-  int q;           // TMEM lane quarter of this warp: rows 32q .. 32q+31 of the tile
+  int q;           // row quarter of this warp: rows 32q .. 32q+31 of the tile
   int a_mode;
   int row;         // row within the batch (pixel index within the image for A_CONV)
   long long grow;  // b*rows + row
@@ -202,6 +203,36 @@ __device__ __forceinline__ bool epi_row_info(const GemmShape& s, const EpiCtx& c
 }
 
 // ---------------------------------------------------------------------------------------------
+// Accumulator tile in shared memory: row r, column j at word  r * (mma_n + kAccPad) + j.
+// The pad of kAccPad = 4 words puts the 16-byte reads of 8 consecutive rows into distinct banks.
+// ---------------------------------------------------------------------------------------------
+constexpr int kAccPad = 4;
+__host__ __device__ constexpr int gemm_acc_bytes(int mma_n) { return 128 * (mma_n + kAccPad) * 4; }
+
+// 32 consecutive fp32 columns of this thread's accumulator row, starting at word address `waddr`
+__device__ __forceinline__ void acc_ld32(uint32_t waddr, float (&v)[32]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const uint4 u = lds128(waddr * 4 + 16 * i);
+    v[4 * i + 0] = __uint_as_float(u.x);
+    v[4 * i + 1] = __uint_as_float(u.y);
+    v[4 * i + 2] = __uint_as_float(u.z);
+    v[4 * i + 3] = __uint_as_float(u.w);
+  }
+}
+// Walk this thread's accumulator row in 32-column chunks: f(col, v[32]) for col = first,
+// first+step, ... < ncols (warp-uniform).  The two epilogue groups take alternate chunks
+// (first = 32*group, step = 64).
+template <class F>
+__device__ __forceinline__ void acc_foreach32(uint32_t abase, int ncols, int first, int step, F&& f) {
+  float v[32];
+  for (int col = first; col < ncols; col += step) {
+    acc_ld32(abase + col, v);
+    f(col, v);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Warp-staged, coalesced epilogue I/O.  Accumulator rows live one-per-thread, but global memory
 // wants whole 64/128-byte segments: every 32x32 chunk goes through a per-warp shared-memory
 // transpose buffer (row stride padded by 16 B so both access directions are conflict-light).
@@ -244,11 +275,9 @@ __device__ __forceinline__ void staged_store_h32(const GemmShape& s, const EpiCt
     }
     __syncwarp();
     const int seg = lane & 3;
-    // all four shared loads first, then the four global stores: paired LDS -> STG serialised ~45 clk of
-    // shared-memory latency per store (short-scoreboard stalls were 28 % of the epilogue warps' samples
-    // in the source-level ncu of the K = 256 GEMMs, which are epilogue-bound)
-    // (kBatch = false: the conv epilogues sit at the 168-register cap and are MMA-bound; the paired
-    // form there avoids spills)
+    // all four shared loads first, then the four global stores: a paired LDS -> STG waits out the
+    // shared-memory latency before every store
+    // (kBatch = false: the conv epilogues are MMA-bound; the paired form holds fewer registers)
     if constexpr (kBatch) {
       uint4 t4[4];
 #pragma unroll
@@ -370,7 +399,7 @@ struct EpiStoreF16 {
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
   __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
     const bool masked = p.row_mask && c.valid && p.row_mask[c.grow] == 0;
-    tmem_foreach32(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
       const int g0 = c.n0 + col;
       const int act = g0 < p.act_cols ? p.act : 0;
       if (act == 1) {
@@ -411,7 +440,7 @@ struct EpiQ {
       sts32f(c.smem_s + 4 * i, p.ksum[(long long)c.b * s.n_total + c.n0 + i]);
     epi_sync(c);
     const bool qmasked = p.row_mask && c.valid && p.row_mask[c.grow] == 0;
-    tmem_foreach32(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
       float dot = 0.f;
 #pragma unroll
       for (int g = 0; g < 8; ++g) {
@@ -462,10 +491,11 @@ struct EpiLN {
   // first, so both threads of a row compute bit-identical statistics), then each group
   // normalises and writes its own chunks.  Residual loads and fp16 stores go through the per-warp
   // transpose buffer (OPP_LN_STAGED): a row-per-thread 16 B access touches 32 cache lines per
-  // instruction = 32 L1 wavefronts at ~2 clk each, which made this epilogue wavefront-bound
-  // (28-34 k clk per tile against 6-12 k clk of MMA work).
+  // instruction = 32 L1 wavefronts.
   __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    if (c.it == 0) {   // gamma / beta of this CTA's columns (the same for every tile): staged once per CTA
+    // gamma / beta of this CTA's columns, staged once per CTA: a LayerNorm GEMM has one N tile, or
+    // (N-split cluster) one fixed N half per CTA; the launchers check it
+    if (c.it == 0) {
       for (int i = c.etid; i < c.ncols; i += 128) {
         sts32f(c.smem_s + 4 * i, p.gamma[c.n0 + i]);
         sts32f(c.smem_s + 4 * (256 + i), p.beta[c.n0 + i]);
@@ -474,7 +504,7 @@ struct EpiLN {
     }
     float x0 = 0.f, s1 = 0.f, s2 = 0.f;
     int cnt = 0;
-    tmem_foreach32_sel<kGroups == 1>(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
       if (cnt == 0) x0 = v[0];
       cnt += 32;
 #pragma unroll
@@ -545,7 +575,7 @@ struct EpiLN {
     // a shared residual is indexed by the row inside the batch: rebase the pointer once per tile
     const __half* resid = p.resid;
     if (resid && p.resid_shared) resid -= (long long)c.b * s.rows * p.ld;
-    tmem_foreach32_sel<kGroups == 1>(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
 #if OPP_LN_STAGED
       StagedRows pre;
       if (resid) staged_load_issue(c, resid, p.ld, p.out_lo, c.n0 + col, c.ncols - col, pre);
@@ -658,7 +688,7 @@ struct EpiConv {
     };
     if (has_res && c.col_first < c.ncols) issue(c.col_first);
 #endif
-    tmem_foreach32_sel<kGroups == 1>(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
       const int g0 = c.n0 + col;
       const int nvalid = c.ncols - col;   // >= 8, multiple of 8; columns past it are padding
 #pragma unroll
@@ -768,7 +798,7 @@ struct EpiWin {
       const int y = p.stride * cy + p.org + ly, x = p.stride * (j - cy * p.wc) + p.org + lx;
       inside = y >= 0 && y < p.in_h && x >= 0 && x < p.in_w;
     }
-    tmem_foreach32_sel<kGroups == 1>(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
       const int nvalid = c.ncols - col;
 #pragma unroll
       for (int g = 0; g < 8; ++g) {
@@ -803,9 +833,8 @@ struct EpiWin {
 // of the coarse map (15 * 0.5 < 8 columns, 1 * 0.5 < 1 row).  Per 32-channel chunk and plane the
 // warp fetches those <= 30 pixels' 64-byte segments coalesced into its transpose buffer
 // (slot = wy * 10 + wx) and every lane reads its own four neighbours from shared memory.
-// The first version did these loads on demand, one dependent DRAM round trip per chunk and plane
-// (the coarse map does not fit in L2): 28 k clk per tile, 8 % tensor pipe (profiles/r2_ncu_b64_s2.md).
-// Now (i) the NEXT tile's window is pulled into L2 while this tile is processed, (ii) both planes
+// Loading on demand would cost one dependent DRAM round trip per chunk and plane (the coarse map
+// does not fit in L2), so (i) the NEXT tile's window is pulled into L2 while this tile is processed, (ii) both planes
 // of a chunk are loaded together and (iii) the loads of chunk i+1 are issued before the plane-1
 // math and the stores of chunk i.
 struct EpiConvUp {
@@ -842,10 +871,10 @@ struct EpiConvUp {
     for (int o = c.group * 128; o < bytes; o += 128 * kGroups) asm volatile("prefetch.global.L2 [%0];" ::"l"(px + o));
   }
   __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    if (c.it == 0) {
-      for (int i = c.etid; i < c.ncols; i += 128) sts32f(c.smem_s + 4 * i, p.bias[c.n0 + i]);
-      epi_sync(c);
-    }
+    // the bias of this tile's columns: a persistent CTA may visit both N tiles of a narrowed conv
+    epi_sync(c);
+    for (int i = c.etid; i < c.ncols; i += 128) sts32f(c.smem_s + 4 * i, p.bias[c.n0 + i]);
+    epi_sync(c);
     const int lane = threadIdx.x & 31;
     const int seg = lane & 3;
     // this lane's output pixel and its interpolation weights / neighbour slots
@@ -926,7 +955,7 @@ struct EpiConvUp {
     if (c.col_first < c.ncols) issue(c.col_first);
     for (int col = c.col_first; col < c.ncols; col += c.col_step) {
       float v[32];
-      tmem_ld32(c.tmem + col, v);
+      acc_ld32(c.acc + col, v);
 #pragma unroll
       for (int q4 = 0; q4 < 8; ++q4) {
         const uint4 bq = lds128(c.smem_s + 4 * ((col + 4 * q4) & 255));
@@ -964,13 +993,13 @@ struct EpiLse {
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
   __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
     float m = -INFINITY;
-    tmem_foreach32(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (col + j < c.ncols) m = fmaxf(m, v[j] * p.scale);
     });
     float sum = 0.f;
-    tmem_foreach32(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (col + j < c.ncols) sum += fast_exp(v[j] * p.scale - m);
@@ -1009,7 +1038,7 @@ struct EpiConf {
     float best = -1.f;
     int best_idx = c.n0;
     const bool vec_ok = (s.n_total & 3) == 0;
-    tmem_foreach32_sel<!OPP_CONF_STAGED>(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const float x2 = 2.f * (v[j] * p.scale);
@@ -1080,7 +1109,7 @@ struct EpiLseColT {
       epi_sync(c);
     }
     float m = -INFINITY;
-    tmem_foreach32_lean(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
       float t[32];
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -1122,7 +1151,7 @@ struct EpiLseColT {
       }
     });
     float sum = 0.f;
-    tmem_foreach32_lean(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (col + j < c.ncols) {
@@ -1171,7 +1200,7 @@ struct EpiConfCol {
     const bool vec_ok = (s.n_total & 3) == 0;
     const int lane = threadIdx.x & 31;
     unsigned* cm = p.colmax + (long long)c.b * s.n_total + c.n0;
-    tmem_foreach32_lean(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const float x2 = 2.f * (v[j] * p.scale);
@@ -1217,42 +1246,44 @@ struct EpiConfCol {
 // =============================================================================================
 // The kernel
 // =============================================================================================
+__device__ __forceinline__ void sts64f(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+// keeps the compiler from moving accesses of in-flight wgmma accumulators across the fences
+template <int NSUB>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[NSUB][32]) {
+#pragma unroll
+  for (int j = 0; j < NSUB; ++j)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[j][i])::"memory");
+}
+
 template <int A_MODE, class Epi>
 __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShape& s,
                                           const typename Epi::Params& ep) {
+  static_assert(Epi::kGroups == 2, "each of the two MMA warpgroups is one epilogue group");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int planes = s.split ? 2 : 1;
-  const bool pair = s.pair == 1;
   const bool nsc = s.pair == 2;   // N-split cluster: two independent CTAs, same M tile, N half = cluster rank
-  const int b_rows = pair ? s.block_n / 2 : s.block_n;   // W rows resident in THIS CTA
-  const int b_bytes = b_rows * kBlockK * 2;              // one plane of the (local) W tile
+  const int b_bytes = s.mma_n * kBlockK * 2;   // one plane of the W tile
   const int a_stage = kABytes * planes;
   const int b_stage = b_bytes * planes;
+  const int ring = s.stages * (a_stage + b_stage);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + s.stages * a_stage;
-  float* epi_smem = reinterpret_cast<float*>(smem_b + s.stages * b_stage);
+  uint8_t* smem_acc = s.acc_alias ? smem : smem + ring;
+  float* epi_smem = reinterpret_cast<float*>(smem + ring + (s.acc_alias ? 0 : gemm_acc_bytes(s.mma_n)));
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi_smem) +
                                                epi_smem_bytes<Epi>());
   uint64_t* full = bars;
   uint64_t* empty = bars + kMaxStages;
-  uint64_t* tfull = bars + 2 * kMaxStages;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* accfree = bars + 2 * kMaxStages;
 
-  // Warp roles. The SM's warp arbiter favours the highest warp id on each sub-partition, so the
-  // two latency-critical single-issuer roles get the highest ids and the epilogue warps (long
-  // unrolled ALU streams) the lowest; with the MMA issuer as warp 1 it was starved by epilogue
-  // warps of the same sub-partition and the epilogue cost added to the wall time instead of
-  // overlapping with the next tile's MMAs.
-  constexpr int kEpiWarps = 4 * Epi::kGroups;   // warp w: TMEM lane quarter w % 4, group w / 4
-  constexpr int kProducerWarp = kEpiWarps;
-  constexpr int kMmaWarp = kEpiWarps + 1;
+  constexpr int kProducerWarp = 4 * Epi::kGroups;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int acc_stride = s.block_n <= 128 ? 128 : 256;
-  const uint32_t tmem_cols = 2 * acc_stride;
   // tile schedule: "super tiles" of `cluster` adjacent M tiles; every CTA of a cluster walks the
   // same sequence, so the multicast W loads and the cross-CTA stage releases stay in lockstep.
   // N-split cluster: logically two single-CTA GEMMs (csize 1: no multicast, no shared barriers) that
@@ -1262,7 +1293,6 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
   const int crank = nsc ? 0 : prank;
   const int nrank = nsc ? prank : 0;
   const uint16_t cmask = (uint16_t)((1u << csize) - 1u);
-  const bool leader = crank == 0;
   const int cluster_id = blockIdx.x / s.cluster;
   const int n_clusters = gridDim.x / s.cluster;
   const int tiles_per_batch = s.msup * s.n_tiles;
@@ -1275,14 +1305,11 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
   if (warp == 0 && lane == 0) {
     for (int i = 0; i < s.stages; ++i) {
       mbar_init(&full[i], 1);
-      // multicast clusters: one tcgen05.commit arrival from every CTA; pair: the leader's commit
-      mbar_init(&empty[i], pair ? 1 : csize);
+      // one arrival per MMA warpgroup of every CTA that reads the (multicast) stage
+      mbar_init(&empty[i], 2 * csize);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      // every epilogue thread arrives; pair: the threads of both CTAs arrive on the leader's barrier
-      mbar_init(&tempty[i], 128 * Epi::kGroups * (pair ? 2 : 1));
-    }
+    // acc_alias: one arrival per epilogue warp of every CTA whose ring the producer writes into
+    mbar_init(accfree, 4 * Epi::kGroups * csize);
     if constexpr (EpiExtraSmem<Epi>::value > 0) {
       // EpiLN's DSMEM exchange: the 128 group-0 threads of the peer CTA arrive once per tile
       uint64_t* xbar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi_smem) + epi_smem_bytes<Epi>() -
@@ -1292,37 +1319,23 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
     }
     fence_mbar_init();
   }
-  if (warp == kMmaWarp) {
-    if (pair) {
-      tmem_alloc2(tmem_slot, tmem_cols);
-      tmem_relinquish2();
-    } else {
-      tmem_alloc(tmem_slot, tmem_cols);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   if (s.cluster > 1) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // programmatic dependent launch: everything above overlapped with the previous kernel's tail;
-  // from here on we read what it wrote.  Our own successor may be scheduled right away (it parks
-  // in its prologue until this grid has completed).
+  // from here on we read what it wrote.
   pdl_sync();
 
-  // Producer and MMA warps run their loops warp-uniformly (all 32 lanes evaluate the same
-  // addresses, coordinates and descriptors, so they live in uniform registers) and only the
-  // asynchronous-issue instructions sit under elect_one().  A single divergent lane doing the
-  // whole loop made instruction issue, not the tensor pipe, the limiter (~110 clk per MMA).
   if (warp == kProducerWarp) {
     // ------------------------------------------------------------------ TMA producer
+    // The loop runs warp-uniformly; only the asynchronous-issue instructions sit under elect_one().
     int stage = 0;
     uint32_t phase = 0;
     const bool skip_b = (s.debug_skip & 1) != 0, skip_a = (s.debug_skip & 2) != 0;
-    // pair: both CTAs' loads are credited to the leader's barrier, which expects twice the bytes
     const int a_tx = A_MODE == A_WIN ? s.tiles_x * s.tile_w * s.tile_h * (kBlockK * 2) * planes : a_stage;
-    const uint32_t tx_bytes = ((skip_a ? 0 : a_tx) + (skip_b ? 0 : b_stage)) * (pair ? 2 : 1);
-    for (int t = cluster_id; t < total_tiles; t += n_clusters) {
+    const uint32_t tx_bytes = (skip_a ? 0 : a_tx) + (skip_b ? 0 : b_stage);
+    int it = 0;
+    for (int t = cluster_id; t < total_tiles; t += n_clusters, ++it) {
+      // the accumulator overlays the ring: wait until every epilogue of the cluster is done with it
+      if (s.acc_alias && it > 0) mbar_wait(accfree, (uint32_t)((it - 1) & 1));
       const int b = t / tiles_per_batch;
       const int r = t - b * tiles_per_batch;
       const int msi = r / s.n_tiles;
@@ -1336,7 +1349,7 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
       }
       const int bb = s.b_batched ? b : 0;
       const int nrow0 = n_tile * s.block_n;
-      // A_WIN: input coordinates of the (up to three) windows of this tile, once per tile
+      // A_WIN: input coordinates of the (up to five) windows of this tile, once per tile
       int win_x[5] = {0, 0, 0, 0, 0}, win_y[5] = {0, 0, 0, 0, 0}, win_z[5] = {0, 0, 0, 0, 0};
       if constexpr (A_MODE == A_WIN) {
         const int cnt = s.rows / (s.tile_w * s.tile_h);
@@ -1369,16 +1382,10 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
           const int ba = (first && s.a0_shared) ? 0 : b;
           kb = chunk * kBlockK;
           if (elect_one()) {
-            if (!pair || leader) mbar_expect_tx(&full[stage], tx_bytes);
+            mbar_expect_tx(&full[stage], tx_bytes);
             if (!skip_a) {
-              if (pair) {
-                tma_load_3d_2sm(am, &full[stage], sa, kc, m_tile * kBlockM, ba);
-                if (s.split)
-                  tma_load_3d_2sm(am, &full[stage], sa + kABytes, kc + lo, m_tile * kBlockM, ba);
-              } else {
-                tma_load_3d(am, &full[stage], sa, kc, m_tile * kBlockM, ba);
-                if (s.split) tma_load_3d(am, &full[stage], sa + kABytes, kc + lo, m_tile * kBlockM, ba);
-              }
+              tma_load_3d(am, &full[stage], sa, kc, m_tile * kBlockM, ba);
+              if (s.split) tma_load_3d(am, &full[stage], sa + kABytes, kc + lo, m_tile * kBlockM, ba);
             }
           }
         } else if constexpr (A_MODE == A_WIN) {
@@ -1391,19 +1398,11 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
             if (wi >= s.tiles_x) break;
             const int bx = win_x[wi] + kx, by = win_y[wi] + ky, bz = win_z[wi];
             if (elect_one()) {
-              if (wi == 0 && (!pair || leader)) mbar_expect_tx(&full[stage], tx_bytes);
+              if (wi == 0) mbar_expect_tx(&full[stage], tx_bytes);
               if (!skip_a) {
-                if (pair) {
-                  tma_load_4d_2sm(&maps.a[0], &full[stage], sa + wi * wbytes, cc * kBlockK, bx, by, bz);
-                  if (s.split)
-                    tma_load_4d_2sm(&maps.a[0], &full[stage], sa + kABytes + wi * wbytes,
-                                    s.conv_c + cc * kBlockK, bx, by, bz);
-                } else {
-                  tma_load_4d(&maps.a[0], &full[stage], sa + wi * wbytes, cc * kBlockK, bx, by, bz);
-                  if (s.split)
-                    tma_load_4d(&maps.a[0], &full[stage], sa + kABytes + wi * wbytes,
-                                s.conv_c + cc * kBlockK, bx, by, bz);
-                }
+                tma_load_5d(&maps.a[0], &full[stage], sa + wi * wbytes, cc * kBlockK, 0, bx, by, bz);
+                if (s.split)
+                  tma_load_5d(&maps.a[0], &full[stage], sa + kABytes + wi * wbytes, cc * kBlockK, 1, bx, by, bz);
               }
             }
           }
@@ -1425,19 +1424,11 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
           }
           kb = kb_tap + cc * kBlockK;
           if (elect_one()) {
-            if (!pair || leader) mbar_expect_tx(&full[stage], tx_bytes);
+            mbar_expect_tx(&full[stage], tx_bytes);
             if (!skip_a) {
-              if (pair) {
-                tma_load_4d_2sm(&maps.a[mi], &full[stage], sa, cc * kBlockK, ox0 + dx, oy0 + dy, b);
-                if (s.split)
-                  tma_load_4d_2sm(&maps.a[mi], &full[stage], sa + kABytes, s.conv_c + cc * kBlockK,
-                                  ox0 + dx, oy0 + dy, b);
-              } else {
-                tma_load_4d(&maps.a[mi], &full[stage], sa, cc * kBlockK, ox0 + dx, oy0 + dy, b);
-                if (s.split)
-                  tma_load_4d(&maps.a[mi], &full[stage], sa + kABytes, s.conv_c + cc * kBlockK,
-                              ox0 + dx, oy0 + dy, b);
-              }
+              tma_load_5d(&maps.a[mi], &full[stage], sa, cc * kBlockK, 0, ox0 + dx, oy0 + dy, b);
+              if (s.split)
+                tma_load_5d(&maps.a[mi], &full[stage], sa + kABytes, cc * kBlockK, 1, ox0 + dx, oy0 + dy, b);
             }
           }
           if (++cc == s.conv_cchunks) {
@@ -1450,18 +1441,13 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
           }
         }
         if (!skip_b && elect_one()) {
-          if (pair) {
-            // this CTA keeps W rows [crank*N/2, +N/2) of the tile; the MMA reads both halves
-            const int nrow = nrow0 + crank * b_rows;
-            tma_load_3d_2sm(&maps.b, &full[stage], sb, kb, nrow, bb);
-            if (s.split) tma_load_3d_2sm(&maps.b, &full[stage], sb + b_bytes, s.b_lo + kb, nrow, bb);
-          } else if (csize == 1) {
+          if (csize == 1) {
             tma_load_3d(&maps.b, &full[stage], sb, kb, nrow0, bb);
             if (s.split) tma_load_3d(&maps.b, &full[stage], sb + b_bytes, s.b_lo + kb, nrow0, bb);
           } else {
             // this CTA fetches rows [crank*slice, +slice) of the W tile and multicasts them into
             // every CTA of the cluster (each CTA's full barrier expects the whole tile)
-            const int slice = s.block_n / csize;
+            const int slice = s.mma_n / csize;
             const int soff = crank * slice * (kBlockK * 2);
             const int nrow = nrow0 + crank * slice;
             tma_load_3d_mc(&maps.b, &full[stage], sb + soff, kb, nrow, bb, cmask);
@@ -1476,110 +1462,49 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
         }
       }
     }
-  } else if (warp == kMmaWarp) {
-    // ------------------------------------------------------------------ MMA issuer
-    // The tensor-core instruction queue is shallow: whatever this warp executes between the last
-    // MMA of one chunk and the first MMA of the next is tensor-pipe idle time, so the loop keeps
-    // running smem addresses, a fixed descriptor template and a branch-free full-chunk path.
-    const uint32_t idesc = make_idesc_f16(pair ? 2 * kBlockM : kBlockM, s.block_n);
-    const uint64_t desc_tmpl = make_kmajor_sw128_desc(0);
-    const uint32_t sa0 = (smem_u32(smem_a) >> 4) & 0x3FFF, sb0 = (smem_u32(smem_b) >> 4) & 0x3FFF;  // 16 B units
-    const uint32_t a_step = (uint32_t)a_stage >> 4, b_step = (uint32_t)b_stage >> 4;
-    const uint32_t a_lo_off = kABytes >> 4, b_lo_off = (uint32_t)b_bytes >> 4;
-    const bool split = s.split != 0;
-    int stage = 0;
-    uint32_t phase = 0;
-    uint32_t sa = sa0, sb = sb0;
-    int it = 0;
-    for (int t = cluster_id; t < total_tiles && (!pair || leader); t += n_clusters, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait_hot(&tempty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * acc_stride;
-      int cc = 0;
-      for (int chunk = 0; chunk < s.k_chunks; ++chunk) {
-        int ksteps = 4;
-        if (A_MODE != A_ROWS) {
-          const int rem = (s.conv_c - cc * kBlockK) >> 4;
-          ksteps = rem < 4 ? rem : 4;
-          if (++cc == s.conv_cchunks) cc = 0;
-        }
-        const uint64_t a_hi = desc_tmpl | sa, b_hi = desc_tmpl | sb;
-        const uint64_t a_lo = desc_tmpl | (sa + a_lo_off), b_lo = desc_tmpl | (sb + b_lo_off);
-        mbar_wait_hot(&full[stage], phase);
-        tc_fence_after();
-        if (pair) {
-          if (elect_one()) {
-            tc_mma2_f16(d_tmem, a_hi, b_hi, idesc, chunk != 0);
-            for (int k = 1; k < ksteps; ++k) tc_mma2_f16_acc(d_tmem, a_hi + 2 * k, b_hi + 2 * k, idesc);
-            if (split) {
-              for (int k = 0; k < ksteps; ++k) tc_mma2_f16_acc(d_tmem, a_hi + 2 * k, b_lo + 2 * k, idesc);
-              for (int k = 0; k < ksteps; ++k) tc_mma2_f16_acc(d_tmem, a_lo + 2 * k, b_hi + 2 * k, idesc);
-            }
-            tc_commit2_mc(&empty[stage], 3);   // frees the stage in both CTAs
-          }
-        } else if (elect_one()) {
-          // K advance: 16 fp16 = 32 B inside the 128 B swizzle row = +2 in 16-byte units
-          tc_mma_f16(d_tmem, a_hi, b_hi, idesc, chunk != 0);
-          if (ksteps == 4) {
-            tc_mma_f16_acc(d_tmem, a_hi + 2, b_hi + 2, idesc);
-            tc_mma_f16_acc(d_tmem, a_hi + 4, b_hi + 4, idesc);
-            tc_mma_f16_acc(d_tmem, a_hi + 6, b_hi + 6, idesc);
-            if (split) {
-              tc_mma_f16_acc(d_tmem, a_hi, b_lo, idesc);
-              tc_mma_f16_acc(d_tmem, a_hi + 2, b_lo + 2, idesc);
-              tc_mma_f16_acc(d_tmem, a_hi + 4, b_lo + 4, idesc);
-              tc_mma_f16_acc(d_tmem, a_hi + 6, b_lo + 6, idesc);
-              tc_mma_f16_acc(d_tmem, a_lo, b_hi, idesc);
-              tc_mma_f16_acc(d_tmem, a_lo + 2, b_hi + 2, idesc);
-              tc_mma_f16_acc(d_tmem, a_lo + 4, b_hi + 4, idesc);
-              tc_mma_f16_acc(d_tmem, a_lo + 6, b_hi + 6, idesc);
-            }
-          } else {
-            for (int k = 1; k < ksteps; ++k) tc_mma_f16_acc(d_tmem, a_hi + 2 * k, b_hi + 2 * k, idesc);
-            if (split) {
-              for (int k = 0; k < ksteps; ++k) tc_mma_f16_acc(d_tmem, a_hi + 2 * k, b_lo + 2 * k, idesc);
-              for (int k = 0; k < ksteps; ++k) tc_mma_f16_acc(d_tmem, a_lo + 2 * k, b_hi + 2 * k, idesc);
-            }
-          }
-          if (csize > 1) tc_commit_mc(&empty[stage], cmask); else tc_commit(&empty[stage]);
-        }
-        __syncwarp();
-        sa += a_step;
-        sb += b_step;
-        if (++stage == s.stages) {
-          stage = 0;
-          phase ^= 1;
-          sa = sa0;
-          sb = sb0;
-        }
-      }
-      if (elect_one()) {
-        if (pair) tc_commit2_mc(&tfull[acc], 3); else tc_commit(&tfull[acc]);
-      }
-      __syncwarp();
-    }
   } else {
-    // ------------------------------------------------------------------ epilogue warps
+    // ------------------------------------------------------------------ MMA warpgroup g = epilogue group g
+    const int g = warp >> 2;
     const int q = warp & 3;
-    const int row_in_tile = q * 32 + lane;
     EpiCtx c;
-    c.etid = (warp & 3) * 32 + lane;
+    c.etid = q * 32 + lane;
     c.q = q;
     c.a_mode = A_MODE;
-    c.group = warp >> 2;
-    c.col_first = 32 * c.group;
+    c.group = g;
+    c.col_first = 32 * g;
     c.col_step = 32 * Epi::kGroups;
-    c.smem = epi_smem + c.group * (kEpiParamBytes / 8);   // 2 KB (512 floats) per group
+    c.smem = epi_smem + g * (kEpiParamBytes / 8);   // 2 KB (512 floats) per group
     c.wstage = reinterpret_cast<uint8_t*>(epi_smem) + kEpiParamBytes + warp * EpiWarpStage<Epi>::value;
     c.extra = reinterpret_cast<uint8_t*>(epi_smem) + epi_smem_bytes<Epi>() - EpiExtraSmem<Epi>::value;
     c.smem_s = smem_u32(c.smem);
     c.wstage_s = smem_u32(c.wstage);
+    // descriptors in 16-byte units: this warpgroup's 64 A rows start 64 * 128 B into the A tile;
+    // K advances 16 fp16 = 32 B (+2) inside the 128 B swizzle row; W sub-tile j starts 64 rows in
+    const uint64_t desc_tmpl = make_kmajor_sw128_desc(0);
+    const uint32_t sa0 = ((smem_u32(smem_a) >> 4) & 0x3FFF) + g * ((64 * 128) >> 4);
+    const uint32_t sb0 = (smem_u32(smem_b) >> 4) & 0x3FFF;
+    const uint32_t a_step = (uint32_t)a_stage >> 4, b_step = (uint32_t)b_stage >> 4;
+    const uint32_t a_lo_off = kABytes >> 4, b_lo_off = (uint32_t)b_bytes >> 4;
+    constexpr uint32_t kSubStep = (kWgmmaN * 128) >> 4;
+    const int nsub = s.mma_n / kWgmmaN;
+    const bool split = s.split != 0;
+    const bool is_signal = q == 0 && lane == 0;
+    const uint32_t pitch = (uint32_t)(s.mma_n + kAccPad);
+    const uint32_t acc_w = smem_u32(smem_acc) >> 2;
+    // this thread's accumulator fragment: rows r0 and r0 + 8, columns 64 j + 8 i + c0 + {0, 1}
+    const uint32_t r0 = 64 * g + 16 * q + (lane >> 2), c0 = 2 * (lane & 3);
+    auto release = [&](int st) {
+      if (is_signal) {
+        if (csize == 1) mbar_arrive(&empty[st]);
+        else
+          for (int r = 0; r < csize; ++r) mbar_arrive_cluster(&empty[st], (uint32_t)r);
+      }
+    };
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t sa = sa0, sb = sb0;
     int it = 0;
     for (int t = cluster_id; t < total_tiles; t += n_clusters, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
       c.b = t / tiles_per_batch;
       const int r = t - c.b * tiles_per_batch;
       const int msi = r / s.n_tiles;
@@ -1605,13 +1530,83 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
         int rdummy;
         if (epi_row_info(s, c, (lane >> 2) + 8 * i, c.sgrow[i], rdummy)) c.svalid |= 1u << i;
       }
-      c.tmem = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * acc_stride;
+      c.acc = acc_w + (uint32_t)(q * 32 + lane) * pitch;
       Epi::prefetch(ep, s, c);
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      if (s.debug_skip & 32) {   // bit 5: timing experiment, ONLY the TMEM reads of the epilogue
+
+      // the tile's MMAs and the accumulator dump, with registers for exactly NSUB n64 sub-tiles
+      auto mma_tile = [&](auto nsub_c) {
+        constexpr int NSUB = decltype(nsub_c)::value;
+        float d[NSUB][32];
+#pragma unroll
+        for (int j = 0; j < NSUB; ++j)
+#pragma unroll
+          for (int i = 0; i < 32; ++i) d[j][i] = 0.f;
+        wgmma_fence_acc(d);
+        // Every chunk is 4 K steps: in the conv modes the channel chunk past conv_c (196 -> 208 is
+        // 3 x 64 + 16) reads as zeros (the A map's channel extent is conv_c, TMA fills the rest),
+        // so no wgmma sits under a runtime-bounded loop, which would make ptxas serialise them.
+        int prev = -1;
+        for (int chunk = 0; chunk < s.k_chunks; ++chunk) {
+          const uint64_t a_hi = desc_tmpl | sa, b_hi = desc_tmpl | sb;
+          const uint64_t a_lo = desc_tmpl | (sa + a_lo_off), b_lo = desc_tmpl | (sb + b_lo_off);
+          mbar_wait_hot(&full[stage], phase);
+          wgmma_fence();
+#pragma unroll
+          for (int j = 0; j < NSUB; ++j) {
+            const uint64_t bj_hi = b_hi + j * kSubStep, bj_lo = b_lo + j * kSubStep;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_m64n64k16(d[j], a_hi + 2 * k, bj_hi + 2 * k);
+            if (split) {
+#pragma unroll
+              for (int k = 0; k < 4; ++k) wgmma_m64n64k16(d[j], a_hi + 2 * k, bj_lo + 2 * k);
+#pragma unroll
+              for (int k = 0; k < 4; ++k) wgmma_m64n64k16(d[j], a_lo + 2 * k, bj_hi + 2 * k);
+            }
+          }
+          wgmma_commit();
+          wgmma_fence_acc(d);
+          // the previous chunk's wgmmas have retired: its stage can be refilled
+          if (prev >= 0) {
+            wgmma_wait<1>();
+            release(prev);
+          }
+          prev = stage;
+          sa += a_step;
+          sb += b_step;
+          if (++stage == s.stages) {
+            stage = 0;
+            phase ^= 1;
+            sa = sa0;
+            sb = sb0;
+          }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_acc(d);
+        if (prev >= 0) release(prev);
+
+        // both groups are done reading the previous tile's accumulator
+        named_bar_sync(4, 256);
+#pragma unroll
+        for (int j = 0; j < NSUB; ++j) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const uint32_t col = 64 * j + 8 * i + c0;
+            sts64f((acc_w + r0 * pitch + col) * 4, d[j][4 * i], d[j][4 * i + 1]);
+            sts64f((acc_w + (r0 + 8) * pitch + col) * 4, d[j][4 * i + 2], d[j][4 * i + 3]);
+          }
+        }
+        named_bar_sync(4, 256);
+      };
+      switch (nsub) {
+        case 1: mma_tile(std::integral_constant<int, 1>{}); break;
+        case 2: mma_tile(std::integral_constant<int, 2>{}); break;
+        case 3: mma_tile(std::integral_constant<int, 3>{}); break;
+        default: mma_tile(std::integral_constant<int, 4>{}); break;
+      }
+
+      if (s.debug_skip & 32) {   // bit 5: timing experiment, ONLY the accumulator reads of the epilogue
         float acc_sink = 0.f;
-        tmem_foreach32(c.tmem, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+        acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
 #pragma unroll
           for (int j = 0; j < 32; ++j) acc_sink += v[j];
         });
@@ -1619,19 +1614,22 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
       } else if (!(s.debug_skip & 4)) {
         Epi::run(ep, s, c);   // bit 2: timing experiment, no epilogue at all
       }
-      tc_fence_before();
-      if (pair) mbar_arrive_cluster(&tempty[acc], 0); else mbar_arrive(&tempty[acc]);
+      if (s.acc_alias) {
+        // the producer's next TMA writes land where this warp just read the accumulator
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+          if (csize == 1) mbar_arrive(accfree);
+          else
+            for (int r2 = 0; r2 < csize; ++r2) mbar_arrive_cluster(accfree, (uint32_t)r2);
+        }
+      }
     }
   }
 
   pdl_done();
-  tc_fence_before();
   // a CTA must outlive every multicast write / remote barrier arrival aimed at it
   if (s.cluster > 1) cluster_sync_all(); else __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    if (pair) tmem_dealloc2(tmem_base, tmem_cols); else tmem_dealloc(tmem_base, tmem_cols);
-  }
 }
 
 template <int A_MODE, class Epi>
@@ -1657,19 +1655,32 @@ gemm_kernel_dyn(const __grid_constant__ TensorMaps maps, const GemmShape s_in,
   gemm_body<A_MODE, Epi>(maps, s, ep);
 }
 
-// dynamic shared memory a launch needs (ring + epilogue scratch + barriers + alignment slack)
-inline int gemm_stage_bytes(int block_n, int split, int pair) {
-  return (kABytes + (pair ? block_n / 2 : block_n) * kBlockK * 2) * (split ? 2 : 1);
+// Shared memory of a launch: operand ring, the accumulator tile (beside the ring, or over it when
+// acc_alias), epilogue scratch, barriers and alignment slack.
+inline int gemm_stage_bytes(int mma_n, int split) {
+  return (kABytes + mma_n * kBlockK * 2) * (split ? 2 : 1);
 }
-inline int gemm_smem_bytes(int stages, int block_n, int split, int pair, int epi_bytes = kEpiSmemBytes) {
-  return stages * gemm_stage_bytes(block_n, split, pair) + epi_bytes + (2 * kMaxStages + 4) * 8 +
-         16 + 1024;
+inline int gemm_smem_bytes(const GemmShape& s, int epi_bytes) {
+  return s.stages * gemm_stage_bytes(s.mma_n, s.split) + (s.acc_alias ? 0 : gemm_acc_bytes(s.mma_n)) +
+         epi_bytes + (2 * kMaxStages + 2) * 8 + 16 + 1024;
 }
-inline int gemm_pick_stages(int block_n, int k_chunks, int split, int pair, int epi_bytes = kEpiSmemBytes) {
-  int st = (227 * 1024 - epi_bytes - 2048) / gemm_stage_bytes(block_n, split, pair);
+constexpr int kSmemLimit = 227 * 1024;
+// Ring depth and accumulator placement for s.mma_n: the accumulator gets its own space when that
+// leaves at least two stages, else it overlays the ring (which then holds at least the tile).
+// `cap` (> 1) bounds the ring depth.  Returns false when even the overlay does not fit.
+inline bool gemm_pick_stages(GemmShape& s, int epi_bytes, int cap = 0) {
+  const int avail = kSmemLimit - epi_bytes - 2048;
+  const int sb = gemm_stage_bytes(s.mma_n, s.split), ab = gemm_acc_bytes(s.mma_n);
+  int st = (avail - ab) / sb;
+  s.acc_alias = st < 2;
+  if (s.acc_alias) st = avail / sb;
   if (st > kMaxStages) st = kMaxStages;
-  if (st > k_chunks * 2 && k_chunks * 2 >= 2) st = k_chunks * 2;
-  return st < 2 ? 2 : st;
+  if (st > s.k_chunks * 2 && s.k_chunks * 2 >= 2) st = s.k_chunks * 2;
+  if (cap > 1 && st > cap) st = cap;
+  if (st < 2) st = 2;
+  if (s.acc_alias && st * sb < ab) st = (ab + sb - 1) / sb;
+  s.stages = st;
+  return st <= kMaxStages && gemm_smem_bytes(s, epi_bytes) <= kSmemLimit;
 }
 
 }  // namespace opp

@@ -19,7 +19,7 @@ constexpr int kC1Tile = 16;  // 16x16 output pixels per CTA of the conv1 im2col
 // conv1 as a tensor-core GEMM (backbone/resnet.py:101-103,143): the 7x7 stride-2 pad-3 window of
 // every output pixel is written as one GEMM row  A[pixel][64] = (49 taps, 1.0, 0 x 14)  in fp16
 // planes; the weight matrix W[c][64] = (49 folded-BN taps, folded bias, 0 x 14) then gives
-// conv + bias as ONE 64-wide K chunk of the tcgen05 engine (opp_linear_act_f16 with ReLU), whose
+// conv + bias as ONE 64-wide K chunk of the wgmma engine (opp_linear_act_f16 with ReLU), whose
 // row-major output [pixel][planes*C] IS the NHWC feature map.  This kernel is the im2col: pure
 // streaming (reads the image through a shared-memory patch, writes 128 B per pixel and plane,
 // fully coalesced).  IMG_U8: the image is uint8 and  x = u8 / 255  (data_io.py:34-68 does the
@@ -241,7 +241,7 @@ constexpr int kKvChunk = 256;   // tokens per CTA (128 -> 256: half the partial-
 
 // ---------------------------------------------------------------------------------------------
 // Per head the state is a 32x32 GEMM over the tokens of the chunk, KV[d][v] = sum_t K'[t][d] V[t][v]:
-// M = d, N = v, K = token.  The tile is far too small for tcgen05 (M = 128 would compute 8x the
+// M = d, N = v, K = token.  The tile is far too small for the wgmma engine (M = 128 would compute 8x the
 // needed head blocks and wants token-major operands transposed), so each warp (= head) runs
 // mma.sync m16n8k16 on fragments fetched with ldmatrix.trans straight from the token-major rows:
 // the kernel is a pure stream over kv16 (2 KB per token in split mode) and should sit on the HBM
@@ -775,10 +775,10 @@ __global__ void __launch_bounds__(128) fine_attention_kernel(const __half* __res
                                                              const int* __restrict__ count_dev) {
   pdl_sync();
   if (count_dev && (int)blockIdx.x >= *count_dev) return;
-  // ncu (batch 64, 24 k matches): the first version was bound by shared-memory instructions — 32-bit
-  // loads of values every lane of a head shares, and the per-head state re-read from shared memory
-  // although each thread owns its column.  Now rows are fetched with 16-byte global loads, shared
-  // operands are read as float4 broadcasts and the window state column stays in registers.
+  // Rows are fetched with 16-byte global loads, operands every lane of a head shares are read as
+  // float4 broadcasts, and the window state column each thread owns stays in registers (32-bit
+  // shared loads of shared values and re-reading the state from shared memory made the kernel
+  // bound by shared-memory instructions).
   __shared__ __align__(16) float q_s[26][128];
   __shared__ __align__(16) float k_s[26][128];
   __shared__ __align__(16) float v_s[26][128];

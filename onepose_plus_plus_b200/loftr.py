@@ -1,6 +1,6 @@
 """Drop-in for ``LoFTR_for_OnePose_Plus`` (src/KeypointFreeSfM/loftr_for_sfm/loftr.py:16-167) — the
 2D-2D detector-free matcher OnePose++ uses for its keypoint-free SfM mapping and as the detector
-of demo.py — on the same sm_100a kernels as the 2D-3D matcher (SURVEY §8 f3).
+of demo.py — on the same sm_90a kernels as the 2D-3D matcher (SURVEY §8 f3).
 
 Same constructor (``config, enable_fine_matching=True``; config = the lower-cased dict of
 ``loftr_for_onepose_plus_cfg.py``), same state-dict keys (``backbone.*``, ``loftr_coarse.layers.N.*``,
@@ -137,7 +137,7 @@ class LoFTR_for_OnePose_Plus(_Engine):
     # ------------------------------------------------------------------ forward
     def forward(self, data, **kwargs):
         if self.training:
-            raise NotImplementedError("LoFTR_for_OnePose_Plus (B200) is the inference matcher: call .eval()")
+            raise NotImplementedError("LoFTR_for_OnePose_Plus is the inference matcher: call .eval()")
         if "mask0" in data or "mask1" in data:
             raise NotImplementedError("padding masks (mask0 / mask1) are not built")
         if "mkpts0_c" in data:
@@ -146,7 +146,7 @@ class LoFTR_for_OnePose_Plus(_Engine):
             raise NotImplementedError("feature extraction at the matches (loftr.py:136-165) is not built")
         im0, im1 = data["image0"], data["image1"]
         if not (torch.is_tensor(im0) and im0.is_cuda and im1.is_cuda):
-            raise RuntimeError("LoFTR_for_OnePose_Plus (B200) has no CPU path: move the model and data to a CUDA device")
+            raise RuntimeError("LoFTR_for_OnePose_Plus has no CPU path: move the model and data to a CUDA device")
         if im0.dim() != 4 or im0.shape[1] != 1 or im1.shape != im0.shape:
             raise ValueError(f"image0 / image1 must both be [B, 1, H, W] of one size, got {tuple(im0.shape)}, "
                              f"{tuple(im1.shape)} (differently sized pairs: one call per size)")

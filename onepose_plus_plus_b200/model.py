@@ -3,7 +3,7 @@
 Same constructor (``config, profiler=None, debug=False``), same config keys, same 195 state-dict
 keys (so ``load_state_dict(strict=True)`` of a reference checkpoint works), same in-place
 ``forward(data)`` contract — but ``forward`` runs the whole coarse-to-fine matcher through the
-sm_100a kernels of ``libopp_b200.so``.  The ``nn.Module`` tree below only *holds* parameters with
+sm_90a kernels of ``libopp_b200.so``.  The ``nn.Module`` tree below only *holds* parameters with
 the reference's names and initialisers; there is no PyTorch math on the hot path and no fallback:
 CPU tensors, training mode, or a missing extension raise.
 
@@ -278,7 +278,7 @@ class _Engine(nn.Module):
         self._graphs = {}
         # K'/V rows of the coarse attention state stored as ONE fp16 plane: their only consumer sums
         # them over thousands of tokens, so the 2^-12 rounding averages out (oracle experiment: conf
-        # changes by 1e-4; the whole GPU parity suite passes with it: profiles/r2_kv1_adoption.md)
+        # changes by 1e-4; the whole GPU parity suite passes with it)
         self.kv_single_plane = os.environ.get("OPP_B200_KV1", "1") == "1"
 
     def _pe_module(self):
@@ -343,7 +343,7 @@ class _Engine(nn.Module):
             bp[:co] = b
             P[name] = (ops.to_planes(wp.reshape(_pad16(co), -1), split), bp.contiguous())
 
-        # conv1 runs as ONE 64-wide K chunk of the tcgen05 engine: W[c] = (49 folded taps, folded
+        # conv1 runs as ONE 64-wide K chunk of the wgmma engine: W[c] = (49 folded taps, folded
         # bias, 14 zeros) against im2col rows (49 taps, 1.0, 14 zeros) — ops.conv1_gemm
         w, b = fold("backbone.conv1", "backbone.bn1")
         w64 = torch.zeros(w.shape[0], 64, device=device)
@@ -583,7 +583,7 @@ class _Engine(nn.Module):
 class OnePosePlus_model(_Engine):
     def __init__(self, config, profiler=None, debug=False, precision=None):
         """`precision` (extension; default from $OPP_B200_PRECISION or "fp16x3"):
-        "fp16x3" = 2-term fp16 split operands, three tcgen05 MMAs per K-step (fp32-grade, the
+        "fp16x3" = 2-term fp16 split operands, three wgmma MMAs per K-step (fp32-grade, the
         parity mode); "fp16" = single fp16 operands (fast, ~1e-2 deviations on high-gain inputs)."""
         super().__init__()
         self.config = config
@@ -791,7 +791,7 @@ class OnePosePlus_model(_Engine):
     def _both(self, f2, f3):
         """The 2D-side and the 3D-side update of a layer are independent (cross layers read the
         pre-update tensors, transformer.py:154-159).  At small batches each persistent GEMM fills a
-        fraction of the 148 SMs, so in latency (CUDA-graph) mode the two sides are enqueued on two
+        fraction of the 132 SMs, so in latency (CUDA-graph) mode the two sides are enqueued on two
         streams and run side by side; otherwise one after the other."""
         side = self._side_stream
         if side is None:
@@ -946,7 +946,7 @@ class OnePosePlus_model(_Engine):
         a wrong batch or point count would read out of bounds instead of raising like PyTorch)."""
         img = data["query_image"]
         if not torch.is_tensor(img) or not img.is_cuda:
-            raise RuntimeError("OnePosePlus_model (B200) has no CPU path: move the model and data to "
+            raise RuntimeError("OnePosePlus_model has no CPU path: move the model and data to "
                                "a CUDA device")
         if img.dim() != 4 or img.shape[1] != 1:
             raise ValueError(f"query_image must be [B, 1, H, W], got {tuple(img.shape)}")

@@ -37,7 +37,7 @@ def _chk(t, dtype, name):
 
 
 def conv1_gemm(image, w64, a_buf, out, split):
-    """conv1 7x7/2 + folded BN + ReLU as im2col + ONE 64-wide tcgen05 K chunk (bias rides in K column
+    """conv1 7x7/2 + folded BN + ReLU as im2col + ONE 64-wide wgmma K chunk (bias rides in K column
     49).  image fp32 or uint8 [B,1,H,W]; w64 fp16 [C, planes*64]; a_buf fp16 [B*H/2*W/2, planes*64]."""
     B, _, H, W = image.shape
     if image.dtype not in (torch.float32, torch.uint8):

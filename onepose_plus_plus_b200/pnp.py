@@ -3,7 +3,7 @@ RANSAC-PnP (src/utils/metric_utils.py:121-204 ``ransac_PnP``, :207-292
 ``compute_query_pose_errors``; demo.py:132).
 
 The reference copies the match lists to the host after every forward and runs
-``cv2.solvePnPRansac(EPnP, iterationsCount=10000)`` frame by frame; at the matcher's B200
+``cv2.solvePnPRansac(EPnP, iterationsCount=10000)`` frame by frame; at the matcher's GPU
 throughput that CPU stage is the whole per-frame latency.  Here the batch is solved by one kernel
 launch (``opp_pnp_ransac``: one CTA per image, P3P hypotheses + inlier scoring + Gauss-Newton
 refinement on the inliers) reading ``m_bids / mkpts_3d_db / mkpts_query_f`` where the matcher left

@@ -1,6 +1,6 @@
 """Training-mode forward of ``OnePosePlus_model`` — differentiable PyTorch (autograd) path.
 
-The sm_100a kernels of this package implement the *inference* forward; their backward passes are
+The sm_90a kernels of this package implement the *inference* forward; their backward passes are
 not built.  ``train_onepose_plus.py`` (PL_OnePosePlus.training_step:
 src/lightning_model/OnePosePlus_lightning_model.py:54-60) however calls ``self.matcher(batch)`` in
 ``.train()`` mode, back-propagates through ``conf_matrix`` / ``expec_f`` (losses.py:125-133) and

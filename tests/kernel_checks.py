@@ -89,7 +89,7 @@ def check_linear_ln():
                                                                   # N = 256 at a small grid = N-split cluster
                                                                   # (DSMEM statistics exchange), fp32 output too
                                                                   (1, 600, 256, 256, False, True, True, False),
-                                                                  # > 74 M tiles: the cta_group::2 pair path
+                                                                  # > 66 M tiles: whole-row tiles, accumulator over the operand ring
                                                                   (1, 12000, 256, 256, False, True, False, False)]:
             a0f = _rand(B * rows, k0, seed=1)
             wf = _rand(B if batched else 1, n, k0, scale=0.05, seed=3)
@@ -226,6 +226,24 @@ def check_conv():
         _conv_case(split, 1, 8, 16, 128, 128, 196, 208, 1, 1, 0, False, False, up=True)
 
 
+def _conv_up_cases():
+    for split in (0, 1):
+        _conv_case(split, 2, 60, 80, 196, 208, 256, 256, 1, 1, 0, False, False, up=True)
+        _conv_case(split, 1, 100, 72, 128, 128, 196, 208, 1, 1, 0, False, False, up=True)
+
+
+def check_conv_up_odd_clusters():
+    """The fused-upsample convs with an odd number of clusters in the persistent grid.  In fp16x3
+    the N = 256 tile does not fit next to its fp32 accumulator and runs as 2 x 128 columns; with an
+    odd cluster count a CTA then visits tiles of both column halves, and each tile must use its own
+    bias.  The cluster size is read once per process ($OPP_CLUSTER), hence the child process."""
+    sms = torch.cuda.get_device_properties(DEV).multi_processor_count
+    cluster = next((c for c in (4, 2) if (sms // c) % 2 == 1), 4)
+    env = dict(os.environ, OPP_CLUSTER=str(cluster))
+    r = subprocess.run([sys.executable, os.path.abspath(__file__), "--one", "conv_up"], env=env, timeout=600)
+    assert r.returncode == 0, f"fused-upsample conv checks failed with OPP_CLUSTER={cluster} ({sms} SMs)"
+
+
 def check_conv_win():
     """opp_conv_win (3x3 convolutions on per-match windows, the sparse form of layer1_outconv2)
     against the dense convolutions of the same engine (bit-equal at the window positions: same K
@@ -358,7 +376,7 @@ def check_sim():
 
 # ------------------------------------------------------------------------------------------ SIMT
 def _conv1_gemm_case(split, B, H, W, C, u8):
-    """conv1 as im2col + one 64-wide tcgen05 K chunk (bias in K column 49), fp32 and uint8 images"""
+    """conv1 as im2col + one 64-wide wgmma K chunk (bias in K column 49), fp32 and uint8 images"""
     if u8:
         img = torch.randint(0, 256, (B, 1, H, W), device=DEV, dtype=torch.uint8)
         imgf = img.float() / 255.0
@@ -774,6 +792,7 @@ CHECKS = {
     "linear_q": check_linear_q,
     "linear_act_shared": check_linear_act_shared,
     "conv": check_conv,
+    "conv_up_odd_clusters": check_conv_up_odd_clusters,
     "conv_win": check_conv_win,
     "sim": check_sim,
     "conv1_gemm": check_conv1_gemm,
@@ -789,10 +808,14 @@ CHECKS = {
 }
 
 
+# run only in a child process whose environment selects the launch configuration
+CHILD_CHECKS = {"conv_up": _conv_up_cases}
+
+
 def main(argv):
     if len(argv) == 2 and argv[0] == "--one":
         print(f"[{argv[1]}]")
-        CHECKS[argv[1]]()
+        {**CHECKS, **CHILD_CHECKS}[argv[1]]()
         print(f"[{argv[1]}] OK")
         return 0
     names = argv or list(CHECKS)

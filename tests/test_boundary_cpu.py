@@ -1,16 +1,13 @@
-"""Boundary proof (CPU, build container only — needs /root/reference): the reference's OWN code
-that constructs the matcher runs unchanged when the two import lines of INTEGRATION.md §1 point at
-this package.
+"""Boundary proof (CPU): the drop-in classes accept what the reference's callers hand them.
 
-The reference modules cannot be imported whole here (ray, pytorch_lightning, hydra ... are absent),
-so the relevant definitions are taken from the reference source files with `ast` and executed in a
-namespace where `OnePosePlus_model` is the drop-in class:
-  * `build_model()`  — src/inference/inference_OnePosePlus.py:28-38 (strict=True load, .eval())
-  * `PL_OnePosePlus.__init__` — src/lightning_model/OnePosePlus_lightning_model.py:20-49
-    (matcher slot + full-checkpoint load with the `matcher.` prefix)
-and the object is pickled as Ray does when it ships the model to its workers (:86-94)."""
-import ast
-import copy
+INTEGRATION.md §1 changes only import lines in the reference, so its callers keep doing what they
+do with the matcher:
+  * the inference builder (src/inference/inference_OnePosePlus.py:28-38) constructs the model from
+    the config, loads the `matcher.`-prefixed state dict of a Lightning checkpoint with
+    strict=True and calls .eval(); Ray then pickles the module for its workers (:86-94);
+  * PL_OnePosePlus (src/lightning_model/OnePosePlus_lightning_model.py:20-49) holds the model as
+    its `matcher` submodule and loads the whole checkpoint into itself.
+The tests below perform those operations on the drop-in with plain PyTorch calls."""
 import os
 import pickle
 
@@ -18,18 +15,8 @@ import pytest
 import torch
 import torch.nn as nn
 
-from oracle import oracle, ref_shims, workload
+from oracle import oracle, workload
 from onepose_plus_plus_b200 import OnePosePlus_model
-
-pytestmark = pytest.mark.skipif(not ref_shims.available(), reason="needs /root/reference")
-
-
-def _extract(path, name):
-    src = open(os.path.join(ref_shims.REFERENCE_ROOT, path)).read()
-    for node in ast.parse(src).body:
-        if isinstance(node, (ast.FunctionDef, ast.ClassDef)) and node.name == name:
-            return ast.get_source_segment(src, node)
-    raise KeyError(name)
 
 
 def _pl_checkpoint(tmp_path):
@@ -39,16 +26,16 @@ def _pl_checkpoint(tmp_path):
     return sd, path
 
 
-def test_reference_build_model_runs_on_the_drop_in(tmp_path):
-    from loguru import logger
+def test_inference_builder_loads_checkpoint_and_pickles(tmp_path):
     sd, ckpt = _pl_checkpoint(tmp_path)
-    ns = {"OnePosePlus_model": OnePosePlus_model, "torch": torch, "logger": logger}
-    exec(_extract("src/inference/inference_OnePosePlus.py", "build_model"), ns)   # the reference's code, verbatim
-    model = ns["build_model"](copy.deepcopy(oracle.DEFAULT_CONFIG), ckpt)
+    model = OnePosePlus_model(oracle.DEFAULT_CONFIG)
+    state = torch.load(ckpt, map_location="cpu")["state_dict"]
+    model.load_state_dict({k.replace("matcher.", "", 1): v for k, v in state.items()}, strict=True)
+    model.eval()
     assert isinstance(model, OnePosePlus_model) and not model.training
     got = model.state_dict()
     assert set(got) == set(sd) and all(torch.equal(got[k], sd[k]) for k in sd)
-    # Ray serialises the module object for its workers (inference_OnePosePlus.py:86-94)
+    # Ray serialises the module object for its workers
     clone = pickle.loads(pickle.dumps(model))
     assert not clone.training and all(torch.equal(clone.state_dict()[k], sd[k]) for k in sd)
     assert clone._plan is None and clone._ws == {}          # device caches never travel
@@ -57,50 +44,43 @@ def test_reference_build_model_runs_on_the_drop_in(tmp_path):
         clone(workload.random_workload(64, 64, 50))
 
 
-def test_reference_lightning_module_builds_around_the_drop_in(tmp_path):
-    from loguru import logger
+def test_lightning_module_holds_the_drop_in_as_matcher(tmp_path):
     sd, ckpt = _pl_checkpoint(tmp_path)
 
-    class LightningModule(nn.Module):                       # the two pl features __init__ uses
-        def save_hyperparameters(self):
-            pass
-
-    class Loss(nn.Module):                                  # losses.py:7-16 holds no parameters
+    class Holder(nn.Module):                                # the matcher slot of PL_OnePosePlus
         def __init__(self, config):
             super().__init__()
-            self.config = config
+            self.matcher = OnePosePlus_model(config)
 
-    pl = type("pl", (), {"LightningModule": LightningModule})
-    ns = {"pl": pl, "OnePosePlus_model": OnePosePlus_model, "Loss": Loss, "torch": torch, "logger": logger}
-    src = _extract("src/lightning_model/OnePosePlus_lightning_model.py", "PL_OnePosePlus")
-    exec(src, ns)
-    PL = ns["PL_OnePosePlus"]
-    hparams = {"OnePosePlus": copy.deepcopy(oracle.DEFAULT_CONFIG), "loss": {},
-               "trainer": {"n_val_pairs_to_plot": 4, "world_size": 2}, "pretrained_ckpt": ckpt}
-    PL.hparams = property(lambda self: hparams)            # what save_hyperparameters() provides
-    module = PL()
-    assert isinstance(module.matcher, OnePosePlus_model) and module.n_vals_plot == 2
+    module = Holder(oracle.DEFAULT_CONFIG)
+    module.load_state_dict(torch.load(ckpt, map_location="cpu")["state_dict"], strict=True)
     got = module.matcher.state_dict()
     assert all(torch.equal(got[k], sd[k]) for k in sd)      # the strict full-checkpoint load went through
-    # the hooks Lightning drives on the matcher
     module.eval()
     assert not module.matcher.training
+    module.train()
+    assert module.matcher.training
     assert sum(p.numel() for p in module.parameters()) == 10_226_480
 
 
 def test_loftr_drop_in_has_the_reference_layout():
     """LoFTR_for_OnePose_Plus (SURVEY §8 f3): same ctor, same state-dict keys / shapes as the reference
-    class built from submodules/LoFTR/src/loftr (strict load both ways), non-persistent pos-enc buffer."""
+    class built from submodules/LoFTR/src/loftr (stored by oracle/make_reference_golden.py; the
+    reference loads this layout strictly), non-persistent pos-enc buffer."""
+    import numpy as np
     from oracle import loftr_oracle
     from onepose_plus_plus_b200 import LoFTR_for_OnePose_Plus
-    sd = workload.synthetic_loftr_state_dict(0)
-    ref = ref_shims.build_reference_loftr(sd, dict(loftr_oracle.DEFAULT_CONFIG))
+    from tests import golden_io
+    z = np.load(os.path.join(golden_io.GOLDEN_DIR, "reference", "loftr_layout.npz"))
+    rs = workload.synthetic_loftr_state_dict(0)
     ours = LoFTR_for_OnePose_Plus(dict(loftr_oracle.DEFAULT_CONFIG), enable_fine_matching=True)
-    rs, os_ = ref.state_dict(), ours.state_dict()
-    assert set(rs) == set(os_) and all(rs[k].shape == os_[k].shape for k in rs)
+    os_ = ours.state_dict()
+    assert sorted(os_) == list(z["keys"])
+    assert [str(tuple(os_[k].shape)) for k in sorted(os_)] == list(z["shapes"])
     ours.load_state_dict(rs, strict=True)
-    ref.load_state_dict(ours.state_dict(), strict=True)
-    assert torch.equal(ours.pos_encoding.pe, ref.pos_encoding.pe) and "pos_encoding.pe" not in os_
+    pe = ours.pos_encoding.pe
+    assert tuple(pe.shape) == tuple(z["pe_shape"]) and "pos_encoding.pe" not in os_
+    assert torch.equal(pe.flatten()[torch.from_numpy(z["pe_idx"])], torch.from_numpy(z["pe"]))
     clone = pickle.loads(pickle.dumps(ours.eval()))
     assert all(torch.equal(clone.state_dict()[k], rs[k]) for k in rs)
     with pytest.raises(RuntimeError, match="no CPU path"):
