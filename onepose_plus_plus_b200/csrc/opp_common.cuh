@@ -282,7 +282,7 @@ __device__ __forceinline__ void cluster_sync_all() {
 }
 
 // ---------------------------------------------------------------------------------------------
-// wgmma (warpgroup MMA, sm_90a): D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, fp16 operands from
+// wgmma (warpgroup MMA, sm_90a): D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 operands from
 // shared memory, fp32 accumulators in the registers of the 128 threads of one warpgroup
 // ---------------------------------------------------------------------------------------------
 // K-major operand tile in shared memory, 128-byte swizzle (what TMA SWIZZLE_128B produces for a
@@ -303,25 +303,95 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// d += A * B^T for one m64n64k16 step (both operands K-major, no transpose, unit scales)
-__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+// d += A * B^T for one m64nNk16 step (both operands K-major, no transpose, unit scales).  The
+// accumulator of 64 rows x N columns over the 128 threads is N/2 floats per thread: element
+// 4 i + {0, 1} is row r0, columns 8 i + c0 + {0, 1}, and 4 i + {2, 3} the same columns of row r0 + 8
+// (r0 = 16 * warp + lane / 4, c0 = 2 * (lane % 4)), so an n128 fragment is two n64 fragments
+// concatenated.  Instantiated for the tile widths of kMmaWidths (opp_gemm.cuh).
+template <int N>
+__device__ __forceinline__ void wgmma_m64nNk16(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc);
+#define OPP_WG_ACC8(i)                                                                              \
+  "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]),    \
+      "+f"(d[i + 6]), "+f"(d[i + 7])
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<64>(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
       "setp.eq.u32 p, 0, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1, 0, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1, 0, 0;\n\t"
       "}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
-        "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
-        "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
-        "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),
-        "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : OPP_WG_ACC8(0), OPP_WG_ACC8(8), OPP_WG_ACC8(16), OPP_WG_ACC8(24)
       : "l"(a_desc), "l"(b_desc)
       : "memory");
 }
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<128>(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.eq.u32 p, 0, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, 0;\n\t"
+      "}\n"
+      : OPP_WG_ACC8(0), OPP_WG_ACC8(8), OPP_WG_ACC8(16), OPP_WG_ACC8(24), OPP_WG_ACC8(32), OPP_WG_ACC8(40),
+        OPP_WG_ACC8(48), OPP_WG_ACC8(56)
+      : "l"(a_desc), "l"(b_desc)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<208>(float (&d)[104], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.eq.u32 p, 0, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n208k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103"
+      "}, %104, %105, p, 1, 1, 0, 0;\n\t"
+      "}\n"
+      : OPP_WG_ACC8(0), OPP_WG_ACC8(8), OPP_WG_ACC8(16), OPP_WG_ACC8(24), OPP_WG_ACC8(32), OPP_WG_ACC8(40),
+        OPP_WG_ACC8(48), OPP_WG_ACC8(56), OPP_WG_ACC8(64), OPP_WG_ACC8(72), OPP_WG_ACC8(80), OPP_WG_ACC8(88),
+        OPP_WG_ACC8(96)
+      : "l"(a_desc), "l"(b_desc)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_m64nNk16<256>(float (&d)[128], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.eq.u32 p, 0, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n\t"
+      "}\n"
+      : OPP_WG_ACC8(0), OPP_WG_ACC8(8), OPP_WG_ACC8(16), OPP_WG_ACC8(24), OPP_WG_ACC8(32), OPP_WG_ACC8(40),
+        OPP_WG_ACC8(48), OPP_WG_ACC8(56), OPP_WG_ACC8(64), OPP_WG_ACC8(72), OPP_WG_ACC8(80), OPP_WG_ACC8(88),
+        OPP_WG_ACC8(96), OPP_WG_ACC8(104), OPP_WG_ACC8(112), OPP_WG_ACC8(120)
+      : "l"(a_desc), "l"(b_desc)
+      : "memory");
+}
+#undef OPP_WG_ACC8
 // generic-proxy shared-memory accesses ordered before later TMA (async-proxy) writes to them
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -350,6 +420,13 @@ __device__ __forceinline__ float lds32f(uint32_t addr) {
 __device__ __forceinline__ void sts32f(uint32_t addr, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
 }
+
+// register rebalancing between the warpgroups of a CTA: every warp of a warpgroup executes the same
+// one; .inc waits until enough registers have been released by .dec in other warpgroups
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // named barrier among a subset of warps (id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {

@@ -98,6 +98,29 @@ static int map_rows(CUtensorMap* map, const void* ptr, long long k, long long ro
   return make_map(map, ptr, 3, dims, str, box);
 }
 
+// $OPP_LOG_TILES=1: print every distinct GEMM tile configuration to stderr once, when it is first
+// launched (which wgmma widths, ring depths and clusters a workload actually uses)
+static void log_tile_once(int a_mode, const GemmShape& s) {
+  static int on = -1;
+  if (on < 0) {
+    const char* e = getenv("OPP_LOG_TILES");
+    on = e ? atoi(e) : 0;
+  }
+  if (!on) return;
+  static std::mutex mu;
+  static char seen[256][128];
+  static int n_seen = 0;
+  char key[128];
+  snprintf(key, sizeof(key), "mode %d n %d block_n %d mma_n %d k %d conv_c %d stages %d alias %d cluster %d pair %d",
+           a_mode, s.n_total, s.block_n, s.mma_n, s.k_chunks * kBlockK, s.conv_c, s.stages, s.acc_alias,
+           s.cluster, s.pair);
+  std::lock_guard<std::mutex> lock(mu);
+  for (int i = 0; i < n_seen; ++i)
+    if (!strcmp(seen[i], key)) return;
+  if (n_seen < 256) strcpy(seen[n_seen++], key);
+  fprintf(stderr, "opp gemm tile: %s\n", key);
+}
+
 // rows_dev != nullptr: the DYN kernel (device-side row count, rows = *rows_dev * rows_mult)
 template <int A_MODE, class Epi, bool DYN = false>
 static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Params& ep,
@@ -115,10 +138,13 @@ static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Param
       const char* e = getenv("OPP_STAGES");
       cap = e ? atoi(e) : 0;
     }
+    OPP_REQUIRE(s.mma_n >= EpiMinMmaN<Epi>::value, "GEMM tile width %d below the epilogue's minimum %d",
+                s.mma_n, EpiMinMmaN<Epi>::value);
     OPP_REQUIRE(s.mma_n > 0 && gemm_pick_stages(s, kEpiBytes, cap),
                 "GEMM tile N=%d (split %d) does not fit in shared memory", s.block_n, s.split);
   }
   const int smem = gemm_smem_bytes(s, kEpiBytes);
+  log_tile_once(A_MODE, s);
   const void* kern;
   if constexpr (DYN) kern = (const void*)gemm_kernel_dyn<A_MODE, Epi>;
   else kern = (const void*)gemm_kernel<A_MODE, Epi>;
@@ -170,7 +196,8 @@ static void pick_grouping(GemmShape& s) {
   s.msup = (s.m_tiles + s.cluster - 1) / s.cluster;
 }
 
-// cluster size for a GEMM: W-tile slices must be whole 8-row swizzle groups; $OPP_CLUSTER overrides
+// cluster size for a GEMM: the W-tile slices (mma_n / cluster rows) must be whole 8-row swizzle
+// groups; $OPP_CLUSTER overrides
 static int pick_cluster(int block_n, int m_tiles) {
   static int forced = -1;
   if (forced < 0) {
@@ -178,7 +205,7 @@ static int pick_cluster(int block_n, int m_tiles) {
     forced = e ? atoi(e) : 0;
   }
   int c = forced > 1 ? forced : 2;
-  while (c > 1 && (block_n % (8 * c) != 0 || m_tiles < c)) c >>= 1;
+  while (c > 1 && (mma_width_for(block_n) % (8 * c) != 0 || m_tiles < c)) c >>= 1;
   return c;
 }
 
@@ -228,11 +255,12 @@ static void ln_nsplit_cluster(GemmShape& s) {
 }
 
 // The fp32 accumulator tile lives in shared memory, beside the operand ring or over it: narrow the
-// N tile until ring, accumulator and epilogue scratch fit.  Sets mma_n; call before the W map is
-// built (its box is mma_n / cluster rows).
-static int fit_tile(GemmShape& s, int epi_bytes) {
+// N tile until ring, accumulator and epilogue scratch fit.  Sets mma_n (the smallest compiled wgmma
+// width >= block_n, and >= min_mma_n); call before the W map is built (its box is mma_n / cluster rows).
+static int fit_tile(GemmShape& s, int epi_bytes, int min_mma_n = 64) {
   for (;;) {
-    s.mma_n = (s.block_n + kWgmmaN - 1) / kWgmmaN * kWgmmaN;
+    s.mma_n = mma_width_for(s.block_n);
+    if (s.mma_n < min_mma_n) s.mma_n = min_mma_n;
     GemmShape t = s;
     if (gemm_pick_stages(t, epi_bytes)) return OPP_OK;
     OPP_REQUIRE(s.pair == 0 && s.block_n > 16, "GEMM tile N=%d (split %d) does not fit in shared memory",
@@ -248,7 +276,8 @@ constexpr int kRowsEpiBytes = epi_smem_bytes<EpiLN>();
 // A_i rows are [hi(k_i) | lo(k_i)], W rows are [hi(k0+k1) | lo(k0+k1)].
 static int setup_rows(TensorMaps& maps, GemmShape& s, const void* a0, int k0, const void* a1,
                       int k1, const void* w, int w_batched, int batches, long long rows, int n,
-                      int split, int n_align = 16, int a0_shared = 0, int nsplit_ok = 0) {
+                      int split, int n_align = 16, int a0_shared = 0, int nsplit_ok = 0,
+                      int min_mma_n = 64) {
   OPP_REQUIRE(a0 && w, "null operand");
   OPP_REQUIRE(k0 > 0 && k0 % 64 == 0 && k1 % 64 == 0, "K (%d,%d) must be multiples of 64", k0,
               k1);
@@ -286,7 +315,7 @@ static int setup_rows(TensorMaps& maps, GemmShape& s, const void* a0, int k0, co
   pick_grouping(s);
   if (nsplit_ok == 1) split_n_for_latency(s);
   if (nsplit_ok == 2) ln_nsplit_cluster(s);
-  rc = fit_tile(s, kRowsEpiBytes);
+  rc = fit_tile(s, kRowsEpiBytes, min_mma_n);
   if (rc) return rc;
   const long long kt = (long long)planes * (k0 + k1);
   return map_rows(&maps.b, w, kt, n, w_batched ? batches : 1, kt, (long long)n * kt,
@@ -444,7 +473,7 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   s.out_h = out_h;
   s.split = split ? 1 : 0;
   // A maps are 5-D (channel, plane, x, y, image) with channel extent c_in_pad: the last 64-channel
-  // box of a row reads zeros past c_in_pad, so every K chunk is 4 full MMA steps
+  // box of a row reads zeros past c_in_pad (the mainloop skips the MMA steps of a 16-channel tail)
   const long long C = (long long)planes * c_in_pad;  // pixel stride in elements
   const __half* base = (const __half*)in;
   int rc;
@@ -588,7 +617,8 @@ int opp_sim_lse_cols(const void* a, const void* b, float* part_m, float* part_s,
                      const unsigned char* col_mask, opp_stream_t stream) {
   TensorMaps maps;
   GemmShape s;
-  int rc = setup_rows(maps, s, a, k, nullptr, 0, b, 1, batches, rows, cols, split, 1);
+  int rc = setup_rows(maps, s, a, k, nullptr, 0, b, 1, batches, rows, cols, split, 1, 0, 0,
+                      EpiLseCol::kMinMmaN);
   if (rc) return rc;
   OPP_REQUIRE(part_m && part_s && col_m && col_s, "null pointer");
   EpiLseColParams ep{part_m, part_s, scale, col_m, col_s, (rows + 31) / 32, col_mask};
@@ -601,7 +631,8 @@ int opp_sim_conf_colmax(const void* a, const void* b, const float* lse_own, cons
                         int rows, int cols, int k, float scale, int split, opp_stream_t stream) {
   TensorMaps maps;
   GemmShape s;
-  int rc = setup_rows(maps, s, a, k, nullptr, 0, b, 1, batches, rows, cols, split, 1);
+  int rc = setup_rows(maps, s, a, k, nullptr, 0, b, 1, batches, rows, cols, split, 1, 0, 0,
+                      EpiConfCol::kMinMmaN);
   if (rc) return rc;
   OPP_REQUIRE(lse_own && lse_other && part_val && part_idx && colmax, "null pointer");
   OPP_CHECK_CUDA(cudaMemsetAsync(colmax, 0, (size_t)batches * cols * sizeof(unsigned),

@@ -19,10 +19,13 @@
 // Everything after the accumulator (bias / BN / activation / residual / LayerNorm / elu+1 /
 // linear-attention normaliser / dual-softmax statistics) is a fused epilogue functor.
 //
-// Warp roles (32 + 256 threads): two warpgroups, then the TMA producer warp.  Warpgroup g issues
-// the wgmmas of tile rows 64g .. 64g+63 into its registers, writes them to the fp32 accumulator
-// tile in shared memory, and then runs the epilogue as epilogue group g: warp w owns accumulator
-// rows 32*(w%4) .. +31, one row per thread, and the two groups take alternate 32-column chunks.
+// Warp roles (384 threads): two MMA warpgroups, then the producer warpgroup, whose first warp issues
+// the TMA loads (the other three only wait for the end of the CTA).  The producer warpgroup gives
+// its registers up (setmaxnreg 40) so that the MMA warpgroups can hold 232 each.  Warpgroup g
+// issues one full-width wgmma per K step (m64nNk16, N = the tile's mma_n) for tile rows
+// 64g .. 64g+63 into its registers, writes them to the fp32 accumulator tile in shared memory, and
+// then runs the epilogue as epilogue group g: warp w owns accumulator rows 32*(w%4) .. +31, one
+// row per thread, and the two groups take alternate 32-column chunks.
 //
 // Reference semantics implemented by the epilogues are cited at each functor
 // (paths relative to the reference repo zju3dv/OnePose_Plus_Plus).
@@ -67,9 +70,19 @@ constexpr int kABytes = kBlockM * kBlockK * 2;
 constexpr int kMaxStages = 8;
 constexpr int kEpiParamBytes = 4096;   // bias / gamma,beta / lse vectors: 2 KB per epilogue group
 constexpr int kMaxEpiWarps = 8;
-// two MMA / epilogue warpgroups (Epi::kGroups must be 2) + the producer warp
-constexpr int gemm_threads(int groups) { return 32 + 128 * groups; }
-constexpr int kWgmmaN = 64;               // N of one wgmma; an N tile is 1..4 of them
+// two MMA / epilogue warpgroups (Epi::kGroups must be 2) + the producer warpgroup
+constexpr int gemm_threads(int groups) { return 128 + 128 * groups; }
+constexpr int kProducerRegs = 40;         // setmaxnreg of the producer warpgroup
+constexpr int kMmaRegs = 232;             // ... and of the MMA / epilogue warpgroups
+static_assert(128 * kProducerRegs + 256 * kMmaRegs <= 65536, "register file of one SM");
+// Accumulator widths the mainloop is compiled for (the N of its m64nNk16): a tile of block_n
+// columns runs at the smallest one >= block_n.  208 = the 196-channel layers padded to 16.
+constexpr int kMmaWidths[] = {64, 128, 208, 256};
+constexpr int mma_width_for(int block_n) {
+  for (int w : kMmaWidths)
+    if (w >= block_n) return w;
+  return 0;
+}
 
 enum AMode : int { A_ROWS = 0, A_CONV = 1, A_WIN = 2 };
 
@@ -85,7 +98,7 @@ struct GemmShape {
   int n_tiles;
   int n_total;      // valid output columns
   int block_n;      // output columns per tile (multiple of 16, <= 256)
-  int mma_n;        // block_n rounded up to kWgmmaN: W rows staged per tile and accumulator width
+  int mma_n;        // mma_width_for(block_n): W rows staged per tile and accumulator width
   int k_chunks;     // number of 64-wide K chunks per tile (per plane)
   int stages;
   int b_batched;    // W operand has a leading batch dim
@@ -170,6 +183,17 @@ template <class E>
 constexpr int epi_smem_bytes() {
   return 4096 + 8 * EpiWarpStage<E>::value + EpiExtraSmem<E>::value;   // kEpiParamBytes + kMaxEpiWarps * stage
 }
+
+// the narrowest mainloop an epilogue is compiled with: epilogues declare `static constexpr int
+// kMinMmaN` (fit_tile then widens narrower tiles to it; the columns past ncols are never used)
+template <class E, class = void>
+struct EpiMinMmaN {
+  static constexpr int value = 64;
+};
+template <class E>
+struct EpiMinMmaN<E, std::void_t<decltype(E::kMinMmaN)>> {
+  static constexpr int value = E::kMinMmaN;
+};
 
 // epilogues that look one tile ahead declare `static constexpr bool kNeedsNext`
 template <class E, class = void>
@@ -1095,6 +1119,10 @@ struct EpiLseColParams {
 template <bool kMask>
 struct EpiLseColT {
   static constexpr int kGroups = OPP_ROW_GROUPS;   // row partial slot = kGroups*n_tile + group
+  // With an n64 mainloop in the same kernel, ptxas serialises every wgmma of it (C7514) next to
+  // this epilogue's column butterflies; its GEMMs have >= 4096 columns, so tiles of <= 64 columns
+  // (tiny inputs only) run at 128
+  static constexpr int kMinMmaN = 128;
   using Params = EpiLseColParams;
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
   __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
@@ -1179,6 +1207,10 @@ using EpiLseColMasked = EpiLseColT<true>;   // + query_image_mask (-1e9 on the p
 // an exact comparison of two copies of the same register value.
 struct EpiConfCol {
   static constexpr int kGroups = OPP_ROW_GROUPS;   // partial slot = kGroups*n_tile + group
+  // With an n64 mainloop in the same kernel, ptxas serialises every wgmma of it (C7514) next to
+  // this epilogue's column butterfly; its GEMMs have >= 4096 columns, so tiles of <= 64 columns
+  // (tiny inputs only) run at 128
+  static constexpr int kMinMmaN = 128;
   struct Params {
     const float* lse_own;    // [batches*rows]   (3D points)
     const float* lse_other;  // [batches][n_total] (query cells)
@@ -1250,12 +1282,26 @@ __device__ __forceinline__ void sts64f(uint32_t addr, float a, float b) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 // keeps the compiler from moving accesses of in-flight wgmma accumulators across the fences
-template <int NSUB>
-__device__ __forceinline__ void wgmma_fence_acc(float (&d)[NSUB][32]) {
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
 #pragma unroll
-  for (int j = 0; j < NSUB; ++j)
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// KS K steps of one chunk into the accumulator, per element in the order hi*hi, hi*lo, lo*hi.
+// Every step count has its own fully unrolled body: a wgmma under a runtime-bounded loop makes
+// ptxas serialise all of them.
+template <int N, int KS>
+__device__ __forceinline__ void mma_k_steps(float (&d)[N / 2], bool split, uint64_t a_hi, uint64_t a_lo,
+                                            uint64_t b_hi, uint64_t b_lo) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[j][i])::"memory");
+  for (int k = 0; k < KS; ++k) wgmma_m64nNk16<N>(d, a_hi + 2 * k, b_hi + 2 * k);
+  if (split) {
+#pragma unroll
+    for (int k = 0; k < KS; ++k) wgmma_m64nNk16<N>(d, a_hi + 2 * k, b_lo + 2 * k);
+#pragma unroll
+    for (int k = 0; k < KS; ++k) wgmma_m64nNk16<N>(d, a_lo + 2 * k, b_hi + 2 * k);
+  }
 }
 
 template <int A_MODE, class Epi>
@@ -1281,7 +1327,7 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
   uint64_t* empty = bars + kMaxStages;
   uint64_t* accfree = bars + 2 * kMaxStages;
 
-  constexpr int kProducerWarp = 4 * Epi::kGroups;
+  constexpr int kProducerWarp = 4 * Epi::kGroups;   // first warp of the producer warpgroup
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   // tile schedule: "super tiles" of `cluster` adjacent M tiles; every CTA of a cluster walks the
@@ -1324,146 +1370,152 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
   // from here on we read what it wrote.
   pdl_sync();
 
-  if (warp == kProducerWarp) {
-    // ------------------------------------------------------------------ TMA producer
-    // The loop runs warp-uniformly; only the asynchronous-issue instructions sit under elect_one().
-    int stage = 0;
-    uint32_t phase = 0;
-    const bool skip_b = (s.debug_skip & 1) != 0, skip_a = (s.debug_skip & 2) != 0;
-    const int a_tx = A_MODE == A_WIN ? s.tiles_x * s.tile_w * s.tile_h * (kBlockK * 2) * planes : a_stage;
-    const uint32_t tx_bytes = (skip_a ? 0 : a_tx) + (skip_b ? 0 : b_stage);
-    int it = 0;
-    for (int t = cluster_id; t < total_tiles; t += n_clusters, ++it) {
-      // the accumulator overlays the ring: wait until every epilogue of the cluster is done with it
-      if (s.acc_alias && it > 0) mbar_wait(accfree, (uint32_t)((it - 1) & 1));
-      const int b = t / tiles_per_batch;
-      const int r = t - b * tiles_per_batch;
-      const int msi = r / s.n_tiles;
-      const int n_tile = nsc ? nrank : r - msi * s.n_tiles;
-      const int m_tile = msi * csize + crank;
-      int ox0 = 0, oy0 = 0;
-      if (A_MODE == A_CONV) {
-        const int ty = m_tile / s.tiles_x;
-        oy0 = ty * s.tile_h;
-        ox0 = (m_tile - ty * s.tiles_x) * s.tile_w;
-      }
-      const int bb = s.b_batched ? b : 0;
-      const int nrow0 = n_tile * s.block_n;
-      // A_WIN: input coordinates of the (up to five) windows of this tile, once per tile
-      int win_x[5] = {0, 0, 0, 0, 0}, win_y[5] = {0, 0, 0, 0, 0}, win_z[5] = {0, 0, 0, 0, 0};
-      if constexpr (A_MODE == A_WIN) {
-        const int cnt = s.rows / (s.tile_w * s.tile_h);
-#pragma unroll
-        for (int wi = 0; wi < 5; ++wi) {
-          int m = m_tile * s.tiles_x + wi;
-          m = m < cnt ? m : cnt - 1;
-          win_z[wi] = m;
-          if (ep.j_ids) {
-            const int j = (int)ep.j_ids[m];
-            const int cy = j / ep.wc;
-            win_z[wi] = (int)ep.b_ids[m];
-            win_x[wi] = ep.stride * (j - cy * ep.wc) + ep.org - s.conv_pad;
-            win_y[wi] = ep.stride * cy + ep.org - s.conv_pad;
-          }
+  if (warp >= kProducerWarp) {
+    // ------------------------------------------------------------------ producer warpgroup
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kProducerWarp) {
+      // TMA producer.  The loop runs warp-uniformly; only the asynchronous-issue instructions sit
+      // under elect_one().
+      int stage = 0;
+      uint32_t phase = 0;
+      const bool skip_b = (s.debug_skip & 1) != 0, skip_a = (s.debug_skip & 2) != 0;
+      const int a_tx = A_MODE == A_WIN ? s.tiles_x * s.tile_w * s.tile_h * (kBlockK * 2) * planes : a_stage;
+      const uint32_t tx_bytes = (skip_a ? 0 : a_tx) + (skip_b ? 0 : b_stage);
+      int it = 0;
+      for (int t = cluster_id; t < total_tiles; t += n_clusters, ++it) {
+        // the accumulator overlays the ring: wait until every epilogue of the cluster is done with it
+        if (s.acc_alias && it > 0) mbar_wait(accfree, (uint32_t)((it - 1) & 1));
+        const int b = t / tiles_per_batch;
+        const int r = t - b * tiles_per_batch;
+        const int msi = r / s.n_tiles;
+        const int n_tile = nsc ? nrank : r - msi * s.n_tiles;
+        const int m_tile = msi * csize + crank;
+        int ox0 = 0, oy0 = 0;
+        if (A_MODE == A_CONV) {
+          const int ty = m_tile / s.tiles_x;
+          oy0 = ty * s.tile_h;
+          ox0 = (m_tile - ty * s.tiles_x) * s.tile_w;
         }
-      }
-      // incremental (tap, channel-chunk) counters instead of per-chunk divisions
-      int cc = 0, ky = 0, kx = 0, kb_tap = 0;
-      for (int chunk = 0; chunk < s.k_chunks; ++chunk) {
-        mbar_wait(&empty[stage], phase ^ 1);
-        uint8_t* sa = smem_a + stage * a_stage;
-        uint8_t* sb = smem_b + stage * b_stage;
-        int kb;
-        if (A_MODE == A_ROWS) {
-          const bool first = chunk < s.k_chunks_a0;
-          const int kc = (first ? chunk : chunk - s.k_chunks_a0) * kBlockK;
-          const CUtensorMap* am = first ? &maps.a[0] : &maps.a[1];
-          const int lo = first ? s.a0_lo : s.a1_lo;
-          const int ba = (first && s.a0_shared) ? 0 : b;
-          kb = chunk * kBlockK;
-          if (elect_one()) {
-            mbar_expect_tx(&full[stage], tx_bytes);
-            if (!skip_a) {
-              tma_load_3d(am, &full[stage], sa, kc, m_tile * kBlockM, ba);
-              if (s.split) tma_load_3d(am, &full[stage], sa + kABytes, kc + lo, m_tile * kBlockM, ba);
-            }
-          }
-        } else if constexpr (A_MODE == A_WIN) {
-          // one TMA box (64 channels x tile_w x tile_h) per window and plane; windows past the match
-          // count re-read the last one (their rows are never stored)
-          kb = kb_tap + cc * kBlockK;
-          const int wbytes = s.tile_w * s.tile_h * (kBlockK * 2);
+        const int bb = s.b_batched ? b : 0;
+        const int nrow0 = n_tile * s.block_n;
+        // A_WIN: input coordinates of the (up to five) windows of this tile, once per tile
+        int win_x[5] = {0, 0, 0, 0, 0}, win_y[5] = {0, 0, 0, 0, 0}, win_z[5] = {0, 0, 0, 0, 0};
+        if constexpr (A_MODE == A_WIN) {
+          const int cnt = s.rows / (s.tile_w * s.tile_h);
 #pragma unroll
           for (int wi = 0; wi < 5; ++wi) {
-            if (wi >= s.tiles_x) break;
-            const int bx = win_x[wi] + kx, by = win_y[wi] + ky, bz = win_z[wi];
+            int m = m_tile * s.tiles_x + wi;
+            m = m < cnt ? m : cnt - 1;
+            win_z[wi] = m;
+            if (ep.j_ids) {
+              const int j = (int)ep.j_ids[m];
+              const int cy = j / ep.wc;
+              win_z[wi] = (int)ep.b_ids[m];
+              win_x[wi] = ep.stride * (j - cy * ep.wc) + ep.org - s.conv_pad;
+              win_y[wi] = ep.stride * cy + ep.org - s.conv_pad;
+            }
+          }
+        }
+        // incremental (tap, channel-chunk) counters instead of per-chunk divisions
+        int cc = 0, ky = 0, kx = 0, kb_tap = 0;
+        for (int chunk = 0; chunk < s.k_chunks; ++chunk) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          uint8_t* sa = smem_a + stage * a_stage;
+          uint8_t* sb = smem_b + stage * b_stage;
+          int kb;
+          if (A_MODE == A_ROWS) {
+            const bool first = chunk < s.k_chunks_a0;
+            const int kc = (first ? chunk : chunk - s.k_chunks_a0) * kBlockK;
+            const CUtensorMap* am = first ? &maps.a[0] : &maps.a[1];
+            const int lo = first ? s.a0_lo : s.a1_lo;
+            const int ba = (first && s.a0_shared) ? 0 : b;
+            kb = chunk * kBlockK;
             if (elect_one()) {
-              if (wi == 0) mbar_expect_tx(&full[stage], tx_bytes);
+              mbar_expect_tx(&full[stage], tx_bytes);
               if (!skip_a) {
-                tma_load_5d(&maps.a[0], &full[stage], sa + wi * wbytes, cc * kBlockK, 0, bx, by, bz);
+                tma_load_3d(am, &full[stage], sa, kc, m_tile * kBlockM, ba);
+                if (s.split) tma_load_3d(am, &full[stage], sa + kABytes, kc + lo, m_tile * kBlockM, ba);
+              }
+            }
+          } else if constexpr (A_MODE == A_WIN) {
+            // one TMA box (64 channels x tile_w x tile_h) per window and plane; windows past the match
+            // count re-read the last one (their rows are never stored)
+            kb = kb_tap + cc * kBlockK;
+            const int wbytes = s.tile_w * s.tile_h * (kBlockK * 2);
+#pragma unroll
+            for (int wi = 0; wi < 5; ++wi) {
+              if (wi >= s.tiles_x) break;
+              const int bx = win_x[wi] + kx, by = win_y[wi] + ky, bz = win_z[wi];
+              if (elect_one()) {
+                if (wi == 0) mbar_expect_tx(&full[stage], tx_bytes);
+                if (!skip_a) {
+                  tma_load_5d(&maps.a[0], &full[stage], sa + wi * wbytes, cc * kBlockK, 0, bx, by, bz);
+                  if (s.split)
+                    tma_load_5d(&maps.a[0], &full[stage], sa + kABytes + wi * wbytes, cc * kBlockK, 1, bx, by, bz);
+                }
+              }
+            }
+            if (++cc == s.conv_cchunks) {
+              cc = 0;
+              kb_tap += s.conv_c;
+              if (++kx == s.conv_kw) {
+                kx = 0;
+                ++ky;
+              }
+            }
+          } else {
+            int dy = ky - s.conv_pad, dx = kx - s.conv_pad, mi = 0;
+            if (s.conv_stride == 2) {
+              const int py = dy & 1, px = dx & 1;
+              dy = (dy - py) >> 1;
+              dx = (dx - px) >> 1;
+              mi = py * 2 + px;
+            }
+            kb = kb_tap + cc * kBlockK;
+            if (elect_one()) {
+              mbar_expect_tx(&full[stage], tx_bytes);
+              if (!skip_a) {
+                tma_load_5d(&maps.a[mi], &full[stage], sa, cc * kBlockK, 0, ox0 + dx, oy0 + dy, b);
                 if (s.split)
-                  tma_load_5d(&maps.a[0], &full[stage], sa + kABytes + wi * wbytes, cc * kBlockK, 1, bx, by, bz);
+                  tma_load_5d(&maps.a[mi], &full[stage], sa + kABytes, cc * kBlockK, 1, ox0 + dx, oy0 + dy, b);
+              }
+            }
+            if (++cc == s.conv_cchunks) {
+              cc = 0;
+              kb_tap += s.conv_c;
+              if (++kx == s.conv_kw) {
+                kx = 0;
+                ++ky;
               }
             }
           }
-          if (++cc == s.conv_cchunks) {
-            cc = 0;
-            kb_tap += s.conv_c;
-            if (++kx == s.conv_kw) {
-              kx = 0;
-              ++ky;
-            }
-          }
-        } else {
-          int dy = ky - s.conv_pad, dx = kx - s.conv_pad, mi = 0;
-          if (s.conv_stride == 2) {
-            const int py = dy & 1, px = dx & 1;
-            dy = (dy - py) >> 1;
-            dx = (dx - px) >> 1;
-            mi = py * 2 + px;
-          }
-          kb = kb_tap + cc * kBlockK;
-          if (elect_one()) {
-            mbar_expect_tx(&full[stage], tx_bytes);
-            if (!skip_a) {
-              tma_load_5d(&maps.a[mi], &full[stage], sa, cc * kBlockK, 0, ox0 + dx, oy0 + dy, b);
+          if (!skip_b && elect_one()) {
+            if (csize == 1) {
+              tma_load_3d(&maps.b, &full[stage], sb, kb, nrow0, bb);
+              if (s.split) tma_load_3d(&maps.b, &full[stage], sb + b_bytes, s.b_lo + kb, nrow0, bb);
+            } else {
+              // this CTA fetches rows [crank*slice, +slice) of the W tile and multicasts them into
+              // every CTA of the cluster (each CTA's full barrier expects the whole tile)
+              const int slice = s.mma_n / csize;
+              const int soff = crank * slice * (kBlockK * 2);
+              const int nrow = nrow0 + crank * slice;
+              tma_load_3d_mc(&maps.b, &full[stage], sb + soff, kb, nrow, bb, cmask);
               if (s.split)
-                tma_load_5d(&maps.a[mi], &full[stage], sa + kABytes, cc * kBlockK, 1, ox0 + dx, oy0 + dy, b);
+                tma_load_3d_mc(&maps.b, &full[stage], sb + b_bytes + soff, s.b_lo + kb, nrow, bb, cmask);
             }
           }
-          if (++cc == s.conv_cchunks) {
-            cc = 0;
-            kb_tap += s.conv_c;
-            if (++kx == s.conv_kw) {
-              kx = 0;
-              ++ky;
-            }
+          __syncwarp();
+          if (++stage == s.stages) {
+            stage = 0;
+            phase ^= 1;
           }
-        }
-        if (!skip_b && elect_one()) {
-          if (csize == 1) {
-            tma_load_3d(&maps.b, &full[stage], sb, kb, nrow0, bb);
-            if (s.split) tma_load_3d(&maps.b, &full[stage], sb + b_bytes, s.b_lo + kb, nrow0, bb);
-          } else {
-            // this CTA fetches rows [crank*slice, +slice) of the W tile and multicasts them into
-            // every CTA of the cluster (each CTA's full barrier expects the whole tile)
-            const int slice = s.mma_n / csize;
-            const int soff = crank * slice * (kBlockK * 2);
-            const int nrow = nrow0 + crank * slice;
-            tma_load_3d_mc(&maps.b, &full[stage], sb + soff, kb, nrow, bb, cmask);
-            if (s.split)
-              tma_load_3d_mc(&maps.b, &full[stage], sb + b_bytes + soff, s.b_lo + kb, nrow, bb, cmask);
-          }
-        }
-        __syncwarp();
-        if (++stage == s.stages) {
-          stage = 0;
-          phase ^= 1;
         }
       }
     }
+    // warps 1-3 of the producer warpgroup go straight to the final CTA / cluster sync
   } else {
     // ------------------------------------------------------------------ MMA warpgroup g = epilogue group g
+    setmaxnreg_inc<kMmaRegs>();
     const int g = warp >> 2;
     const int q = warp & 3;
     EpiCtx c;
@@ -1479,19 +1531,17 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
     c.smem_s = smem_u32(c.smem);
     c.wstage_s = smem_u32(c.wstage);
     // descriptors in 16-byte units: this warpgroup's 64 A rows start 64 * 128 B into the A tile;
-    // K advances 16 fp16 = 32 B (+2) inside the 128 B swizzle row; W sub-tile j starts 64 rows in
+    // K advances 16 fp16 = 32 B (+2) inside the 128 B swizzle row; one wgmma reads all mma_n W rows
     const uint64_t desc_tmpl = make_kmajor_sw128_desc(0);
     const uint32_t sa0 = ((smem_u32(smem_a) >> 4) & 0x3FFF) + g * ((64 * 128) >> 4);
     const uint32_t sb0 = (smem_u32(smem_b) >> 4) & 0x3FFF;
     const uint32_t a_step = (uint32_t)a_stage >> 4, b_step = (uint32_t)b_stage >> 4;
     const uint32_t a_lo_off = kABytes >> 4, b_lo_off = (uint32_t)b_bytes >> 4;
-    constexpr uint32_t kSubStep = (kWgmmaN * 128) >> 4;
-    const int nsub = s.mma_n / kWgmmaN;
     const bool split = s.split != 0;
     const bool is_signal = q == 0 && lane == 0;
     const uint32_t pitch = (uint32_t)(s.mma_n + kAccPad);
     const uint32_t acc_w = smem_u32(smem_acc) >> 2;
-    // this thread's accumulator fragment: rows r0 and r0 + 8, columns 64 j + 8 i + c0 + {0, 1}
+    // this thread's accumulator fragment: rows r0 and r0 + 8, columns 8 i + c0 + {0, 1}
     const uint32_t r0 = 64 * g + 16 * q + (lane >> 2), c0 = 2 * (lane & 3);
     auto release = [&](int st) {
       if (is_signal) {
@@ -1503,6 +1553,11 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
     int stage = 0;
     uint32_t phase = 0;
     uint32_t sa = sa0, sb = sb0;
+    // K steps of a chunk: 4, but in the conv modes the last channel chunk of every filter tap holds
+    // only conv_c % 64 channels when conv_c is not a multiple of 64 (196 -> 208 = 3 x 64 + 16); the
+    // TMA box reads zeros past conv_c, and the steps that would multiply only those are not issued
+    // (for a 16-channel tail; see the dispatch below)
+    const int tail_steps = (A_MODE != A_ROWS && (s.conv_c & 63)) ? (s.conv_c & 63) / 16 : 4;
     int it = 0;
     for (int t = cluster_id; t < total_tiles; t += n_clusters, ++it) {
       c.b = t / tiles_per_batch;
@@ -1533,39 +1588,27 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
       c.acc = acc_w + (uint32_t)(q * 32 + lane) * pitch;
       Epi::prefetch(ep, s, c);
 
-      // the tile's MMAs and the accumulator dump, with registers for exactly NSUB n64 sub-tiles
-      auto mma_tile = [&](auto nsub_c) {
-        constexpr int NSUB = decltype(nsub_c)::value;
-        float d[NSUB][32];
+      // the tile's MMAs and the accumulator dump, with registers for exactly N accumulator columns
+      auto mma_tile = [&](auto n_c, auto tail_c) {
+        constexpr int N = decltype(n_c)::value;
+        // K steps of each filter tap's last chunk (0: every chunk is 4 steps).  A compile-time
+        // count keeps the branch between full and tail chunks out of the mainloop: ptxas
+        // serialises wgmmas that sit behind a branch it cannot prove uniform.
+        constexpr int TAIL = decltype(tail_c)::value;
+        float d[N / 2];
 #pragma unroll
-        for (int j = 0; j < NSUB; ++j)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) d[j][i] = 0.f;
+        for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
         wgmma_fence_acc(d);
-        // Every chunk is 4 K steps: in the conv modes the channel chunk past conv_c (196 -> 208 is
-        // 3 x 64 + 16) reads as zeros (the A map's channel extent is conv_c, TMA fills the rest),
-        // so no wgmma sits under a runtime-bounded loop, which would make ptxas serialise them.
         int prev = -1;
-        for (int chunk = 0; chunk < s.k_chunks; ++chunk) {
+        // one chunk: wait for its stage, KS K steps, then release the previous chunk's stage
+        auto chunk_step = [&](auto ks_c, auto& acc) {
           const uint64_t a_hi = desc_tmpl | sa, b_hi = desc_tmpl | sb;
           const uint64_t a_lo = desc_tmpl | (sa + a_lo_off), b_lo = desc_tmpl | (sb + b_lo_off);
           mbar_wait_hot(&full[stage], phase);
           wgmma_fence();
-#pragma unroll
-          for (int j = 0; j < NSUB; ++j) {
-            const uint64_t bj_hi = b_hi + j * kSubStep, bj_lo = b_lo + j * kSubStep;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) wgmma_m64n64k16(d[j], a_hi + 2 * k, bj_hi + 2 * k);
-            if (split) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) wgmma_m64n64k16(d[j], a_hi + 2 * k, bj_lo + 2 * k);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) wgmma_m64n64k16(d[j], a_lo + 2 * k, bj_hi + 2 * k);
-            }
-          }
+          mma_k_steps<N, decltype(ks_c)::value>(acc, split, a_hi, a_lo, b_hi, b_lo);
           wgmma_commit();
-          wgmma_fence_acc(d);
-          // the previous chunk's wgmmas have retired: its stage can be refilled
+          wgmma_fence_acc(acc);
           if (prev >= 0) {
             wgmma_wait<1>();
             release(prev);
@@ -1579,6 +1622,15 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
             sa = sa0;
             sb = sb0;
           }
+        };
+        if constexpr (TAIL == 0) {
+          for (int chunk = 0; chunk < s.k_chunks; ++chunk) chunk_step(std::integral_constant<int, 4>{}, d);
+        } else {
+          const int taps = s.k_chunks / s.conv_cchunks;
+          for (int tap = 0; tap < taps; ++tap) {
+            for (int cc = 1; cc < s.conv_cchunks; ++cc) chunk_step(std::integral_constant<int, 4>{}, d);
+            chunk_step(std::integral_constant<int, TAIL>{}, d);
+          }
         }
         wgmma_wait<0>();
         wgmma_fence_acc(d);
@@ -1587,21 +1639,34 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
         // both groups are done reading the previous tile's accumulator
         named_bar_sync(4, 256);
 #pragma unroll
-        for (int j = 0; j < NSUB; ++j) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const uint32_t col = 64 * j + 8 * i + c0;
-            sts64f((acc_w + r0 * pitch + col) * 4, d[j][4 * i], d[j][4 * i + 1]);
-            sts64f((acc_w + (r0 + 8) * pitch + col) * 4, d[j][4 * i + 2], d[j][4 * i + 3]);
-          }
+        for (int i = 0; i < N / 8; ++i) {
+          const uint32_t col = 8 * i + c0;
+          sts64f((acc_w + r0 * pitch + col) * 4, d[4 * i], d[4 * i + 1]);
+          sts64f((acc_w + (r0 + 8) * pitch + col) * 4, d[4 * i + 2], d[4 * i + 3]);
         }
         named_bar_sync(4, 256);
       };
-      switch (nsub) {
-        case 1: mma_tile(std::integral_constant<int, 1>{}); break;
-        case 2: mma_tile(std::integral_constant<int, 2>{}); break;
-        case 3: mma_tile(std::integral_constant<int, 3>{}); break;
-        default: mma_tile(std::integral_constant<int, 4>{}); break;
+      // one case per entry of kMmaWidths (fit_tile only produces those)
+      auto mma_width = [&](auto tail_c) {
+        switch (s.mma_n) {
+          case 64:
+            if constexpr (EpiMinMmaN<Epi>::value <= 64) mma_tile(std::integral_constant<int, 64>{}, tail_c);
+            break;
+          case 128: mma_tile(std::integral_constant<int, 128>{}, tail_c); break;
+          case 208: mma_tile(std::integral_constant<int, 208>{}, tail_c); break;
+          default: mma_tile(std::integral_constant<int, 256>{}, tail_c); break;
+        }
+      };
+      if constexpr (A_MODE == A_ROWS) {
+        mma_width(std::integral_constant<int, 0>{});
+      } else {
+        // a one-step tail is what the 196 -> 208 channel layers need; a 32- or 48-channel tail runs
+        // as a full chunk (its extra steps multiply zeros): each further tail variant is one more
+        // copy of every mainloop, and the copies together made ptxas spill
+        switch (tail_steps) {
+          case 1: mma_width(std::integral_constant<int, 1>{}); break;
+          default: mma_width(std::integral_constant<int, 0>{}); break;
+        }
       }
 
       if (s.debug_skip & 32) {   // bit 5: timing experiment, ONLY the accumulator reads of the epilogue
