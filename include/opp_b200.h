@@ -352,6 +352,29 @@ int opp_pnp_ransac(const float* pts3d, const float* pts2d, const long long* m_bi
                    unsigned seed, int refine_rounds, float* poses, int* n_inliers,
                    unsigned char* inlier_mask, int* status, opp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * LINEMOD pose metrics — add_metric / projection_2d_error (src/utils/metric_utils.py:31-88, per
+ * frame on the CPU with a scipy cKDTree for ADD-S; caller: the eval_ADD_metric branch of
+ * compute_query_pose_errors :233-289)
+ * ---------------------------------------------------------------------------------------- */
+
+/* ADD / ADD-S and proj2D of `batch` frames of one object model, three launches.
+ *   verts fp32 [num_verts][3] (model points); pose_pred, pose_gt fp32 [batch][3][4] = [R | t]
+ *   (pose_pred as opp_pnp_ransac writes it); intrinsics fp32 [batch][3][3] (the ORIGINAL K);
+ *   symmetric uint8 [batch]; scratch: at least opp_pose_metrics_scratch_bytes(num_verts, batch)
+ *   bytes, 8-byte aligned.
+ * Outputs fp64 [batch]: add_dist = mean_j |pred_j - tgt_j| (symmetric = 0) or the ADD-S mean
+ * nearest-neighbour distance mean_j min_i |pred_i - tgt_j| (symmetric = 1), with pred = R_p x + t_p,
+ * tgt = R_g x + t_g; proj2d = mean_j |pi(pred_j) - pi(tgt_j)| px, pi(p) = (K p)_xy / (K p)_z with no
+ * guard on z (non-finite values propagate).  Deterministic: no floating-point atomics. */
+int opp_pose_metrics(const float* verts, int num_verts, const float* pose_pred, const float* pose_gt,
+                     const float* intrinsics, const unsigned char* symmetric, int batch, void* scratch,
+                     long long scratch_bytes, double* add_dist, double* proj2d, opp_stream_t stream);
+
+/* Scratch bytes opp_pose_metrics needs for num_verts model points and `batch` frames (0 if either
+ * is not positive). */
+long long opp_pose_metrics_scratch_bytes(int num_verts, int batch);
+
 #ifdef __cplusplus
 }
 #endif

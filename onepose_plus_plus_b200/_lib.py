@@ -56,11 +56,13 @@ SIGNATURES = {
     "opp_seq_attention": [P, P, P, I, I, I, F, I, P],
     "opp_fine_match_2d": [P, P, P, P, P, P, I, I, F, P],
     "opp_pnp_ransac": [P, P, P, I, P, I, F, F, I, ctypes.c_uint, I, P, P, P, P, P],
+    "opp_pose_metrics": [P, I, P, P, P, P, I, P, L, P, P, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),
          "opp_kv_chunks_b": ([I, I], c_int),
          "opp_conv_win_pitch": ([I], c_int),
+         "opp_pose_metrics_scratch_bytes": ([I, I], c_longlong),
          "opp_last_error": ([], ctypes.c_char_p)}
 
 
@@ -96,7 +98,7 @@ def stream():
 
 
 # kernels launched per entry point (bench.py reports the per-step total as gpu_launches)
-KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3}
+KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_pose_metrics": 3}
 LAUNCHES = 0
 _PROFILE = None
 
