@@ -125,7 +125,6 @@ static void log_tile_once(int a_mode, const GemmShape& s) {
 template <int A_MODE, class Epi, bool DYN = false>
 static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Params& ep,
                   cudaStream_t stream, const int* rows_dev = nullptr, int rows_mult = 1) {
-  constexpr int kEpiBytes = epi_smem_bytes<Epi>();
   {
     static int dbg = -1;
     if (dbg < 0) {
@@ -140,10 +139,10 @@ static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Param
     }
     OPP_REQUIRE(s.mma_n >= EpiMinMmaN<Epi>::value, "GEMM tile width %d below the epilogue's minimum %d",
                 s.mma_n, EpiMinMmaN<Epi>::value);
-    OPP_REQUIRE(s.mma_n > 0 && gemm_pick_stages(s, kEpiBytes, cap),
+    OPP_REQUIRE(s.mma_n > 0 && gemm_pick_stages<Epi>(s, cap),
                 "GEMM tile N=%d (split %d) does not fit in shared memory", s.block_n, s.split);
   }
-  const int smem = gemm_smem_bytes(s, kEpiBytes);
+  const int smem = gemm_smem_bytes<Epi>(s);
   log_tile_once(A_MODE, s);
   const void* kern;
   if constexpr (DYN) kern = (const void*)gemm_kernel_dyn<A_MODE, Epi>;
@@ -254,23 +253,22 @@ static void ln_nsplit_cluster(GemmShape& s) {
   s.n_tiles = 1;
 }
 
-// The fp32 accumulator tile lives in shared memory, beside the operand ring or over it: narrow the
-// N tile until ring, accumulator and epilogue scratch fit.  Sets mma_n (the smallest compiled wgmma
-// width >= block_n, and >= min_mma_n); call before the W map is built (its box is mma_n / cluster rows).
-static int fit_tile(GemmShape& s, int epi_bytes, int min_mma_n = 64) {
+// Narrow the N tile until the operand ring, the accumulator tile (token-row epilogues: beside the ring
+// or over it) and the epilogue scratch of Epi fit.  Sets mma_n (the smallest compiled wgmma width
+// >= block_n, and >= min_mma_n); call before the W map is built (its box is mma_n / cluster rows).
+template <class Epi>
+static int fit_tile(GemmShape& s, int min_mma_n = 64) {
   for (;;) {
     s.mma_n = mma_width_for(s.block_n);
     if (s.mma_n < min_mma_n) s.mma_n = min_mma_n;
     GemmShape t = s;
-    if (gemm_pick_stages(t, epi_bytes)) return OPP_OK;
+    if (gemm_pick_stages<Epi>(t)) return OPP_OK;
     OPP_REQUIRE(s.pair == 0 && s.block_n > 16, "GEMM tile N=%d (split %d) does not fit in shared memory",
                 s.block_n, s.split);
     s.block_n = (s.block_n / 2 + 15) & ~15;
     s.n_tiles = (s.n_total + s.block_n - 1) / s.block_n;
   }
 }
-// the largest epilogue scratch of the token-row GEMMs (EpiLN: DSMEM exchange slots on top)
-constexpr int kRowsEpiBytes = epi_smem_bytes<EpiLN>();
 
 // common shape / map setup for token-row GEMMs.  With split, every operand row holds two planes:
 // A_i rows are [hi(k_i) | lo(k_i)], W rows are [hi(k0+k1) | lo(k0+k1)].
@@ -315,7 +313,7 @@ static int setup_rows(TensorMaps& maps, GemmShape& s, const void* a0, int k0, co
   pick_grouping(s);
   if (nsplit_ok == 1) split_n_for_latency(s);
   if (nsplit_ok == 2) ln_nsplit_cluster(s);
-  rc = fit_tile(s, kRowsEpiBytes, min_mma_n);
+  rc = fit_tile<EpiLN>(s, min_mma_n);   // the largest scratch of the token-row epilogues
   if (rc) return rc;
   const long long kt = (long long)planes * (k0 + k1);
   return map_rows(&maps.b, w, kt, n, w_batched ? batches : 1, kt, (long long)n * kt,
@@ -502,7 +500,7 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   const long long kt = kplane * planes;
   pick_grouping(s);
   split_n_for_latency(s);   // the 1/8-resolution layers at batch 1: 16 clusters -> 64
-  rc = fit_tile(s, up ? epi_smem_bytes<EpiConvUp>() : epi_smem_bytes<EpiConv>());
+  rc = up ? fit_tile<EpiConvUp>(s) : fit_tile<EpiConv>(s);
   if (rc) return rc;
   rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.mma_n / s.cluster);
   if (rc) return rc;
@@ -581,7 +579,7 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
   s.b_lo = (int)kplane;
   const long long kt = kplane * planes;
   pick_grouping(s);
-  rc = fit_tile(s, epi_smem_bytes<EpiWin>());
+  rc = fit_tile<EpiWin>(s);
   if (rc) return rc;
   rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.mma_n / s.cluster);
   if (rc) return rc;

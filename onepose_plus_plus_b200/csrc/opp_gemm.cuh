@@ -23,9 +23,14 @@
 // the TMA loads (the other three only wait for the end of the CTA).  The producer warpgroup gives
 // its registers up (setmaxnreg 40) so that the MMA warpgroups can hold 232 each.  Warpgroup g
 // issues one full-width wgmma per K step (m64nNk16, N = the tile's mma_n) for tile rows
-// 64g .. 64g+63 into its registers, writes them to the fp32 accumulator tile in shared memory, and
-// then runs the epilogue as epilogue group g: warp w owns accumulator rows 32*(w%4) .. +31, one
-// row per thread, and the two groups take alternate 32-column chunks.
+// 64g .. 64g+63 into its registers and then runs the epilogue as epilogue group g, in one of two ways:
+//   * the conv epilogues (EpiConv, EpiWin: per-element math) read the accumulator registers
+//     directly (EpiFromRegs): warp q holds tile rows 64g+16q .. +15 over all N columns.  There is no
+//     accumulator tile in shared memory, so the ring takes its space and the producer never waits
+//     for an epilogue; the two warpgroups run their epilogues independently.
+//   * the token-row epilogues (row / column reductions) write the fp32 accumulator tile to shared
+//     memory: warp w owns accumulator rows 32*(w%4) .. +31, one row per thread, and the two groups
+//     take alternate 32-column chunks.
 //
 // Reference semantics implemented by the epilogues are cited at each functor
 // (paths relative to the reference repo zju3dv/OnePose_Plus_Plus).
@@ -51,15 +56,6 @@
 #endif
 #ifndef OPP_CONF_STAGED
 #define OPP_CONF_STAGED 1
-#endif
-// BasicBlock residual of the conv epilogue through the transpose buffer (coalesced) instead of
-// row-per-thread 16 B loads.
-#ifndef OPP_CONV_RESID_STAGED
-#define OPP_CONV_RESID_STAGED 1
-#endif
-// positional-encoding add of the token epilogue with 16 B loads instead of scalar ones
-#ifndef OPP_PE_VEC
-#define OPP_PE_VEC 1
 #endif
 
 namespace opp {
@@ -149,8 +145,9 @@ struct EpiCtx {
   uint32_t smem_s, wstage_s;   // the same two regions as 32-bit shared-space addresses
   int group;       // epilogue warp group (0/1); groups take alternate 32-column chunks
   int col_first, col_step;
-  // rows (lane>>2) + 8*i, i = 0..3 of this warp's quarter: element offset grow*ld is NOT stored,
-  // only grow (row index in the output) and validity, computed once per tile
+  // rows (lane>>2) + 8*i, i = 0..3 of this warp's quarter (EpiFromRegs: i = 0..1, the two rows of
+  // this thread's accumulator fragment): element offset grow*ld is NOT stored, only grow (row index
+  // in the output) and validity, computed once per tile
   long long sgrow[4];
   unsigned svalid;
   int next_b, next_m_tile;   // the (batch, M tile) this CTA processes next, or next_b = -1
@@ -201,10 +198,17 @@ struct EpiNeedsNext : std::false_type {};
 template <class E>
 struct EpiNeedsNext<E, std::void_t<decltype(E::kNeedsNext)>> : std::true_type {};
 
-// (global row, validity) of row `rr` (0..31) of this warp's quarter of the tile
-__device__ __forceinline__ bool epi_row_info(const GemmShape& s, const EpiCtx& c, int rr,
-                                             long long& grow, int& row) {
-  const int rit = c.q * 32 + rr;
+// epilogues that run on the accumulator registers declare `static constexpr bool kFromRegs` and
+// `template <int N> static void run_frag(const Params&, const GemmShape&, const EpiCtx&, float (&d)[N / 2])`;
+// their kernels have no accumulator tile in shared memory
+template <class E, class = void>
+struct EpiFromRegs : std::false_type {};
+template <class E>
+struct EpiFromRegs<E, std::void_t<decltype(E::kFromRegs)>> : std::true_type {};
+
+// (global row, validity) of tile row `rit` (0..127)
+__device__ __forceinline__ bool epi_row_at(const GemmShape& s, const EpiCtx& c, int rit,
+                                           long long& grow, int& row) {
   bool ok;
   if (c.a_mode == A_ROWS) {
     row = c.m_tile * kBlockM + rit;
@@ -224,6 +228,11 @@ __device__ __forceinline__ bool epi_row_info(const GemmShape& s, const EpiCtx& c
   }
   grow = (long long)c.b * s.rows + row;
   return ok;
+}
+// (global row, validity) of row `rr` (0..31) of this warp's quarter of the tile
+__device__ __forceinline__ bool epi_row_info(const GemmShape& s, const EpiCtx& c, int rr,
+                                             long long& grow, int& row) {
+  return epi_row_at(s, c, c.q * 32 + rr, grow, row);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -652,6 +661,173 @@ struct EpiLN {
   }
 };
 
+// ---------------------------------------------------------------------------------------------
+// Register-fragment epilogue I/O (EpiFromRegs).  Warp q of MMA warpgroup g holds tile rows
+// 64g + 16q .. +15 over all mma_n columns; this lane holds rows (lane>>2) + 8h, h = 0, 1 of them
+// (c.sgrow[h], bit h of c.svalid) at columns 8i + 2(lane&3) + {0, 1}: d[4i + 2h + {0, 1}].  Those
+// 16 rows are 16 consecutive output rows (one 16-pixel image row of a conv tile, or 16 consecutive
+// window rows), so the global I/O of a 32-column slice (fragment columns i = 4j .. 4j+3) goes through
+// the warp's stage: lane moves the 16-byte segment (lane&3) of its two rows, 8 rows x 64 B per
+// instruction, and the fragment side reads / writes 4 (fp16 pair) or 8 (fp32 pair) bytes, without
+// bank conflicts at these row pitches.  A slice's values are v[4 ii + 2h + e] for i = 4j + ii.
+// ---------------------------------------------------------------------------------------------
+constexpr int kFragRowH = 80;                  // fp16 slice row: 64 B + 16 B pad
+constexpr int kFragPlaneH = 16 * kFragRowH;    // one plane of a 16 x 32 fp16 slice (1280 B)
+constexpr int kFragRowF = 160;                 // fp32 slice row: 128 B + 32 B pad (16 rows = the whole stage)
+
+__device__ __forceinline__ void sts32u(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t lds32u(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ float2 lds64f(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
+
+// the (tile-row) fragment values of slice j: v[4 ii + 2h + e] = d[4 (4j + ii) + 2h + e]; columns
+// past the accumulator width (the second half of the last slice at N = 208) read as 0
+template <int N>
+__device__ __forceinline__ void frag_slice(const float (&d)[N / 2], int j, float (&v)[16]) {
+#pragma unroll
+  for (int k = 0; k < 16; ++k) v[k] = 16 * j + k < N / 2 ? d[16 * j + k] : 0.f;
+}
+
+// + the fp32 vector at smem word address `base` (the epilogue group's bias) per fragment column
+__device__ __forceinline__ void frag_add_cols(uint32_t base_s, int col, float (&v)[16]) {
+  const int c0 = 2 * (threadIdx.x & 3);
+#pragma unroll
+  for (int ii = 0; ii < 4; ++ii) {
+    const float2 b = lds64f(base_s + 4 * ((col + 8 * ii + c0) & 255));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      v[4 * ii + 2 * h] += b.x;
+      v[4 * ii + 2 * h + 1] += b.y;
+    }
+  }
+}
+
+// fp16 planes of slice columns [gcol, gcol + 32) of this warp's 16 rows (hi, and lo when lo_off != 0);
+// nvalid = valid columns of the slice (multiple of 8)
+__device__ __forceinline__ void frag_store_h(const GemmShape& s, const EpiCtx& c, __half* out, long long ld,
+                                             int lo_off, int gcol, const float (&v)[16], int nvalid) {
+  if (s.debug_skip & 8) return;   // bit 3: timing experiment, epilogue math without the stores
+  const int lane = threadIdx.x & 31, t = lane & 3, rq = lane >> 2;
+  const uint32_t st = c.wstage_s;
+#pragma unroll
+  for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float a = v[4 * ii + 2 * h], b = v[4 * ii + 2 * h + 1];
+      const uint32_t addr = st + (rq + 8 * h) * kFragRowH + 16 * ii + 4 * t;
+      sts32u(addr, pack_half2(a, b));
+      if (lo_off)
+        sts32u(addr + kFragPlaneH, pack_half2(a - __half2float(__float2half_rn(a)),
+                                              b - __half2float(__float2half_rn(b))));
+    }
+  __syncwarp();
+#pragma unroll
+  for (int plane = 0; plane < 2; ++plane) {
+    if (plane == 1 && lo_off == 0) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (((c.svalid >> h) & 1u) && t * 8 < nvalid)
+        *reinterpret_cast<uint4*>(out + c.sgrow[h] * ld + plane * lo_off + gcol + t * 8) =
+            lds128(st + plane * kFragPlaneH + (rq + 8 * h) * kFragRowH + 16 * t);
+  }
+  __syncwarp();
+}
+
+// Residual rows (same layout as the output) of one slice: copied into the warp's stage without
+// passing through registers (rows / columns outside the tensor read as 0); frag_load_add then adds
+// hi, then lo to the fragment values.
+__device__ __forceinline__ void frag_load_issue(const EpiCtx& c, const __half* src, long long ld, int lo_off,
+                                                int gcol, int nvalid) {
+  const int lane = threadIdx.x & 31, t = lane & 3, rq = lane >> 2;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const bool in = ((c.svalid >> h) & 1u) && t * 8 < nvalid;
+    const __half* row = in ? src + c.sgrow[h] * ld + gcol + t * 8 : src;
+    const uint32_t dst = c.wstage_s + (rq + 8 * h) * kFragRowH + 16 * t;
+    cp_async16_zfill(dst, row, in ? 16 : 0);
+    if (lo_off) cp_async16_zfill(dst + kFragPlaneH, in ? row + lo_off : src, in ? 16 : 0);
+  }
+  cp_async_commit();
+}
+__device__ __forceinline__ void frag_load_add(const EpiCtx& c, int lo_off, float (&v)[16]) {
+  const int lane = threadIdx.x & 31, t = lane & 3, rq = lane >> 2;
+  const uint32_t st = c.wstage_s;
+  cp_async_wait<0>();
+  __syncwarp();
+#pragma unroll
+  for (int plane = 0; plane < 2; ++plane) {
+    if (plane == 1 && lo_off == 0) break;
+#pragma unroll
+    for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t u = lds32u(st + plane * kFragPlaneH + (rq + 8 * h) * kFragRowH + 16 * ii + 4 * t);
+        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&u));
+        v[4 * ii + 2 * h] += f.x;
+        v[4 * ii + 2 * h + 1] += f.y;
+      }
+  }
+  __syncwarp();
+}
+
+// + an fp32 row-major matrix (row stride ld floats) at rows row[h], slice columns [gcol, gcol + 32),
+// for the rows of c.svalid (the others are left unchanged)
+__device__ __forceinline__ void frag_add_f32(const EpiCtx& c, const float* src, long long ld, const int (&row)[2],
+                                             int gcol, int nvalid, float (&v)[16]) {
+  const int lane = threadIdx.x & 31, t = lane & 3, rq = lane >> 2;
+  const uint32_t st = c.wstage_s;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {   // 16-byte segments t and t + 4 of the 128-byte row slice
+      const int seg = t + 4 * k;
+      if (((c.svalid >> h) & 1u) && seg * 4 < nvalid)
+        sts128(st + (rq + 8 * h) * kFragRowF + 16 * seg,
+               *reinterpret_cast<const uint4*>(src + (long long)row[h] * ld + gcol + seg * 4));
+    }
+  __syncwarp();
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (!((c.svalid >> h) & 1u)) continue;
+#pragma unroll
+    for (int ii = 0; ii < 4; ++ii)
+      if (8 * ii < nvalid) {
+        const float2 f = lds64f(st + (rq + 8 * h) * kFragRowF + 4 * (8 * ii + 2 * t));
+        v[4 * ii + 2 * h] += f.x;
+        v[4 * ii + 2 * h + 1] += f.y;
+      }
+  }
+  __syncwarp();
+}
+
+__device__ __forceinline__ void frag_act(int act, float slope, float (&v)[16]) {
+  if (act == 1) {
+#pragma unroll
+    for (int k = 0; k < 16; ++k) v[k] = fmaxf(v[k], 0.f);
+  } else if (act == 2) {
+#pragma unroll
+    for (int k = 0; k < 16; ++k) v[k] = v[k] > 0.f ? v[k] : v[k] * slope;
+  }
+}
+
+// the tile's columns of a per-column fp32 vector into this epilogue group's parameter smem: once per
+// CTA when the launch has one N tile (every tile has the same columns), else per tile
+__device__ __forceinline__ void epi_stage_cols(const GemmShape& s, const EpiCtx& c, const float* src) {
+  if (c.it > 0 && s.n_tiles == 1) return;
+  epi_sync(c);
+  for (int i = c.etid; i < c.ncols; i += 128) sts32f(c.smem_s + 4 * i, src[c.n0 + i]);
+  epi_sync(c);
+}
+
 // Convolution epilogue: folded-BN bias, residual add, ReLU / LeakyReLU (resnet.py:36-45,112-124,
 // 141-147).  Optionally also emits the coarse tokens  x3_out + pe  in token-major order
 // (position_encoding.py:37-42 + OnePosePlusModel.py:137-142: NHWC *is* 'n (h w) c').
@@ -673,110 +849,54 @@ struct EpiConvParams {
 };
 struct EpiConv {
   static constexpr int kGroups = OPP_CONV_GROUPS;
+  static constexpr bool kFromRegs = true;
   using Params = EpiConvParams;
-  // Called before the accumulator wait: pull this row of the residual towards L2 while the MMAs
-  // of the tile are still running (the conv2 of a BasicBlock was epilogue-bound on this read).
+  // Called before the MMAs of the tile: pull this lane's share of the residual rows towards L2
+  // while they run (the conv2 of a BasicBlock was epilogue-bound on this read).
   __device__ static void prefetch(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    if (!p.resid || !c.valid) return;
-    const char* row = reinterpret_cast<const char*>(p.resid + c.grow * p.ld + c.n0);
-    const int bytes = c.ncols * 2;
-    for (int o = 0; o < bytes; o += 128) {
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(row + o));
-      if (p.out_lo) asm volatile("prefetch.global.L2 [%0];" ::"l"(row + 2 * p.out_lo + o));
+    if (!p.resid) return;
+    const int t = threadIdx.x & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!((c.svalid >> h) & 1u)) continue;
+      const char* row = reinterpret_cast<const char*>(p.resid + c.sgrow[h] * p.ld + c.n0);
+      for (int o = 128 * t; o < c.ncols * 2; o += 512) {
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(row + o));
+        if (p.out_lo) asm volatile("prefetch.global.L2 [%0];" ::"l"(row + 2 * p.out_lo + o));
+      }
     }
   }
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    epi_sync(c);
-    for (int i = c.etid; i < c.ncols; i += 128) sts32f(c.smem_s + 4 * i, p.bias[c.n0 + i]);
-    epi_sync(c);
-#if OPP_CONV_RESID_STAGED
-    // residual through the transpose buffer (coalesced: 8 rows x 64 B per load instruction), issued
-    // one 32-column chunk ahead of its use; warp-uniform, row validity is per staged row
+  // Per element, in this order: acc + bias, + residual hi, + residual lo, activation, the (hi, lo)
+  // store, then + pe and the token store.
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
     const bool has_res = p.resid != nullptr;
-    StagedRows pre;
-    if (has_res && c.col_first < c.ncols)
-      staged_load_issue(c, p.resid, p.ld, p.out_lo, c.n0 + c.col_first, c.ncols - c.col_first, pre);
-#else
-    // residual: row-per-thread 16 B loads, issued one 32-column chunk ahead of their use
-    const bool has_res = p.resid != nullptr && c.valid;
-    uint4 rq[8];
-    auto issue = [&](int col) {
-      const __half* rrow = p.resid + c.grow * p.ld + c.n0 + col;
+    // the residual of a slice is copied into the stage when the stage is free: before the bias of
+    // the tile is staged, and after the stores of the previous slice
+    if (has_res) frag_load_issue(c, p.resid, p.ld, p.out_lo, c.n0, c.ncols);
+    epi_stage_cols(s, c, p.bias);
+    int prow[2] = {0, 0};   // pixel index inside the image of the two fragment rows (tokens)
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const bool in = col + g * 8 < c.ncols;
-        rq[g] = in ? *reinterpret_cast<const uint4*>(rrow + g * 8) : make_uint4(0, 0, 0, 0);
-        rq[4 + g] = (in && p.out_lo) ? *reinterpret_cast<const uint4*>(rrow + p.out_lo + g * 8)
-                                     : make_uint4(0, 0, 0, 0);
-      }
-    };
-    if (has_res && c.col_first < c.ncols) issue(c.col_first);
-#endif
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-      const int g0 = c.n0 + col;
-      const int nvalid = c.ncols - col;   // >= 8, multiple of 8; columns past it are padding
+    for (int h = 0; h < 2; ++h) prow[h] = (int)(c.sgrow[h] - (long long)c.b * s.rows);
 #pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        const uint4 bq = lds128(c.smem_s + 4 * ((col + 4 * g) & 255));
-        v[4 * g + 0] += __uint_as_float(bq.x);
-        v[4 * g + 1] += __uint_as_float(bq.y);
-        v[4 * g + 2] += __uint_as_float(bq.z);
-        v[4 * g + 3] += __uint_as_float(bq.w);
-      }
-#if OPP_CONV_RESID_STAGED
-      if (has_res) {
-        staged_load_add(c, p.out_lo, pre, v);
-        if (col + c.col_step < c.ncols)
-          staged_load_issue(c, p.resid, p.ld, p.out_lo, c.n0 + col + c.col_step,
-                            c.ncols - col - c.col_step, pre);
-      }
-#else
-      if (has_res) {
-#pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          const __half2* h = reinterpret_cast<const __half2*>(&rq[g]);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float2 f = __half22float2(h[j]);
-            v[(g & 3) * 8 + 2 * j] += f.x;
-            v[(g & 3) * 8 + 2 * j + 1] += f.y;
-          }
+    for (int j = 0; j < (N + 31) / 32; ++j) {
+      const int col = 32 * j;
+      if (col < c.ncols) {
+        const int g0 = c.n0 + col;
+        const int nvalid = c.ncols - col;   // >= 8, multiple of 8; columns past it are padding
+        float v[16];
+        frag_slice<N>(d, j, v);
+        frag_add_cols(c.smem_s, col, v);
+        if (has_res) frag_load_add(c, p.out_lo, v);
+        frag_act(p.act, p.slope, v);
+        if (p.out) frag_store_h(s, c, p.out, p.ld, p.out_lo, g0, v, nvalid);
+        if (p.tok) {
+          frag_add_f32(c, p.pe, s.n_total, prow, g0, nvalid, v);
+          frag_store_h(s, c, p.tok, p.ld, p.out_lo, g0, v, nvalid);
         }
-        if (col + c.col_step < c.ncols) issue(col + c.col_step);
+        if (has_res && col + 32 < c.ncols) frag_load_issue(c, p.resid, p.ld, p.out_lo, g0 + 32, nvalid - 32);
       }
-#endif
-      if (p.act == 1) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-      } else if (p.act == 2) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = v[j] > 0.f ? v[j] : v[j] * p.slope;
-      }
-      if (p.out) staged_store_h32<false>(s, c, p.out, p.ld, p.out_lo, g0, v, nvalid);
-      if (p.tok) {
-        if (c.valid) {
-#if OPP_PE_VEC
-          // 8 x 16 B loads per chunk (scalar loads cost 32 L1 wavefronts each: rows are 1 KB apart)
-          const float4* pe4 = reinterpret_cast<const float4*>(p.pe + (long long)c.row * s.n_total + g0);
-#pragma unroll
-          for (int g = 0; g < 8; ++g)
-            if (4 * g < nvalid) {
-              const float4 q4 = pe4[g];
-              v[4 * g + 0] += q4.x;
-              v[4 * g + 1] += q4.y;
-              v[4 * g + 2] += q4.z;
-              v[4 * g + 3] += q4.w;
-            }
-#else
-          const float* pe = p.pe + (long long)c.row * s.n_total + g0;
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (j < nvalid) v[j] += pe[j];
-#endif
-        }
-        staged_store_h32<false>(s, c, p.tok, p.ld, p.out_lo, g0, v, nvalid);
-      }
-    });
+    }
   }
 };
 
@@ -792,6 +912,7 @@ struct EpiConv {
 // compact window tensor [matches][tile_h + 2][8][C] of a previous A_WIN launch.
 struct EpiWin {
   static constexpr int kGroups = OPP_CONV_GROUPS;
+  static constexpr bool kFromRegs = true;
   struct Params {
     __half* out;
     long long ld;
@@ -807,44 +928,40 @@ struct EpiWin {
     int in_h, in_w;           // dense map size
   };
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    epi_sync(c);
-    for (int i = c.etid; i < c.ncols; i += 128) sts32f(c.smem_s + 4 * i, p.bias[c.n0 + i]);
-    epi_sync(c);
-    bool inside = true;
-    if (p.j_ids && c.valid) {
-      const int rpm = s.tile_w * s.tile_h;
-      const int m = (int)(c.grow / rpm);
-      const int local = (int)(c.grow - (long long)m * rpm);
-      const int ly = local / s.tile_w, lx = local - ly * s.tile_w;
-      const int j = (int)p.j_ids[m];
-      const int cy = j / p.wc;
-      const int y = p.stride * cy + p.org + ly, x = p.stride * (j - cy * p.wc) + p.org + lx;
-      inside = y >= 0 && y < p.in_h && x >= 0 && x < p.in_w;
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
+    epi_stage_cols(s, c, p.bias);
+    bool inside[2] = {true, true};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (p.j_ids && ((c.svalid >> h) & 1u)) {
+        const int rpm = s.tile_w * s.tile_h;
+        const int m = (int)(c.sgrow[h] / rpm);
+        const int local = (int)(c.sgrow[h] - (long long)m * rpm);
+        const int ly = local / s.tile_w, lx = local - ly * s.tile_w;
+        const int jj = (int)p.j_ids[m];
+        const int cy = jj / p.wc;
+        const int y = p.stride * cy + p.org + ly, x = p.stride * (jj - cy * p.wc) + p.org + lx;
+        inside[h] = y >= 0 && y < p.in_h && x >= 0 && x < p.in_w;
+      }
     }
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-      const int nvalid = c.ncols - col;
 #pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        const uint4 bq = lds128(c.smem_s + 4 * ((col + 4 * g) & 255));
-        v[4 * g + 0] += __uint_as_float(bq.x);
-        v[4 * g + 1] += __uint_as_float(bq.y);
-        v[4 * g + 2] += __uint_as_float(bq.z);
-        v[4 * g + 3] += __uint_as_float(bq.w);
+    for (int j = 0; j < (N + 31) / 32; ++j) {
+      const int col = 32 * j;
+      if (col < c.ncols) {
+        float v[16];
+        frag_slice<N>(d, j, v);
+        frag_add_cols(c.smem_s, col, v);
+        frag_act(p.act, p.slope, v);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (!inside[h]) {
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii) v[4 * ii + 2 * h] = v[4 * ii + 2 * h + 1] = 0.f;
+          }
+        frag_store_h(s, c, p.out, p.ld, p.out_lo, c.n0 + col, v, c.ncols - col);
       }
-      if (p.act == 1) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-      } else if (p.act == 2) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = v[j] > 0.f ? v[j] : v[j] * p.slope;
-      }
-      if (!inside) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-      }
-      staged_store_h32<false>(s, c, p.out, p.ld, p.out_lo, c.n0 + col, v, nvalid);
-    });
+    }
   }
 };
 
@@ -1319,8 +1436,10 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
   const int ring = s.stages * (a_stage + b_stage);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + s.stages * a_stage;
+  // register-fragment epilogues have no accumulator tile (and acc_alias = 0)
+  constexpr bool kAccTile = !EpiFromRegs<Epi>::value;
   uint8_t* smem_acc = s.acc_alias ? smem : smem + ring;
-  float* epi_smem = reinterpret_cast<float*>(smem + ring + (s.acc_alias ? 0 : gemm_acc_bytes(s.mma_n)));
+  float* epi_smem = reinterpret_cast<float*>(smem + ring + (kAccTile && !s.acc_alias ? gemm_acc_bytes(s.mma_n) : 0));
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi_smem) +
                                                epi_smem_bytes<Epi>());
   uint64_t* full = bars;
@@ -1578,12 +1697,21 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
         }
       }
       c.it = it;
-      c.valid = epi_row_info(s, c, lane, c.grow, c.row);
       c.svalid = 0;
+      if constexpr (kAccTile) {
+        c.valid = epi_row_info(s, c, lane, c.grow, c.row);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        int rdummy;
-        if (epi_row_info(s, c, (lane >> 2) + 8 * i, c.sgrow[i], rdummy)) c.svalid |= 1u << i;
+        for (int i = 0; i < 4; ++i) {
+          int rdummy;
+          if (epi_row_info(s, c, (lane >> 2) + 8 * i, c.sgrow[i], rdummy)) c.svalid |= 1u << i;
+        }
+      } else {
+        // the two accumulator-fragment rows of this thread
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          int rdummy;
+          if (epi_row_at(s, c, (int)r0 + 8 * h, c.sgrow[h], rdummy)) c.svalid |= 1u << h;
+        }
       }
       c.acc = acc_w + (uint32_t)(q * 32 + lane) * pitch;
       Epi::prefetch(ep, s, c);
@@ -1636,15 +1764,19 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
         wgmma_fence_acc(d);
         if (prev >= 0) release(prev);
 
-        // both groups are done reading the previous tile's accumulator
-        named_bar_sync(4, 256);
+        if constexpr (!kAccTile) {
+          if (!(s.debug_skip & 4)) Epi::template run_frag<N>(ep, s, c, d);   // bit 2: timing experiment, no epilogue
+        } else {
+          // both groups are done reading the previous tile's accumulator
+          named_bar_sync(4, 256);
 #pragma unroll
-        for (int i = 0; i < N / 8; ++i) {
-          const uint32_t col = 8 * i + c0;
-          sts64f((acc_w + r0 * pitch + col) * 4, d[4 * i], d[4 * i + 1]);
-          sts64f((acc_w + (r0 + 8) * pitch + col) * 4, d[4 * i + 2], d[4 * i + 3]);
+          for (int i = 0; i < N / 8; ++i) {
+            const uint32_t col = 8 * i + c0;
+            sts64f((acc_w + r0 * pitch + col) * 4, d[4 * i], d[4 * i + 1]);
+            sts64f((acc_w + (r0 + 8) * pitch + col) * 4, d[4 * i + 2], d[4 * i + 3]);
+          }
+          named_bar_sync(4, 256);
         }
-        named_bar_sync(4, 256);
       };
       // one case per entry of kMmaWidths (fit_tile only produces those)
       auto mma_width = [&](auto tail_c) {
@@ -1669,24 +1801,26 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
         }
       }
 
-      if (s.debug_skip & 32) {   // bit 5: timing experiment, ONLY the accumulator reads of the epilogue
-        float acc_sink = 0.f;
-        acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+      if constexpr (kAccTile) {
+        if (s.debug_skip & 32) {   // bit 5: timing experiment, ONLY the accumulator reads of the epilogue
+          float acc_sink = 0.f;
+          acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) acc_sink += v[j];
-        });
-        if (acc_sink == 12345.678f) c.smem[0] = acc_sink;
-      } else if (!(s.debug_skip & 4)) {
-        Epi::run(ep, s, c);   // bit 2: timing experiment, no epilogue at all
-      }
-      if (s.acc_alias) {
-        // the producer's next TMA writes land where this warp just read the accumulator
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          if (csize == 1) mbar_arrive(accfree);
-          else
-            for (int r2 = 0; r2 < csize; ++r2) mbar_arrive_cluster(accfree, (uint32_t)r2);
+            for (int j = 0; j < 32; ++j) acc_sink += v[j];
+          });
+          if (acc_sink == 12345.678f) c.smem[0] = acc_sink;
+        } else if (!(s.debug_skip & 4)) {
+          Epi::run(ep, s, c);   // bit 2: timing experiment, no epilogue at all
+        }
+        if (s.acc_alias) {
+          // the producer's next TMA writes land where this warp just read the accumulator
+          fence_proxy_async_smem();
+          __syncwarp();
+          if (lane == 0) {
+            if (csize == 1) mbar_arrive(accfree);
+            else
+              for (int r2 = 0; r2 < csize; ++r2) mbar_arrive_cluster(accfree, (uint32_t)r2);
+          }
         }
       }
     }
@@ -1720,24 +1854,29 @@ gemm_kernel_dyn(const __grid_constant__ TensorMaps maps, const GemmShape s_in,
   gemm_body<A_MODE, Epi>(maps, s, ep);
 }
 
-// Shared memory of a launch: operand ring, the accumulator tile (beside the ring, or over it when
-// acc_alias), epilogue scratch, barriers and alignment slack.
+// Shared memory of a launch with epilogue Epi: operand ring, the accumulator tile (token-row
+// epilogues only: beside the ring, or over it when acc_alias), epilogue scratch, barriers and
+// alignment slack.
 inline int gemm_stage_bytes(int mma_n, int split) {
   return (kABytes + mma_n * kBlockK * 2) * (split ? 2 : 1);
 }
-inline int gemm_smem_bytes(const GemmShape& s, int epi_bytes) {
-  return s.stages * gemm_stage_bytes(s.mma_n, s.split) + (s.acc_alias ? 0 : gemm_acc_bytes(s.mma_n)) +
-         epi_bytes + (2 * kMaxStages + 2) * 8 + 16 + 1024;
+template <class Epi>
+inline int gemm_smem_bytes(const GemmShape& s) {
+  const bool acc_tile = !EpiFromRegs<Epi>::value && !s.acc_alias;
+  return s.stages * gemm_stage_bytes(s.mma_n, s.split) + (acc_tile ? gemm_acc_bytes(s.mma_n) : 0) +
+         epi_smem_bytes<Epi>() + (2 * kMaxStages + 2) * 8 + 16 + 1024;
 }
 constexpr int kSmemLimit = 227 * 1024;
-// Ring depth and accumulator placement for s.mma_n: the accumulator gets its own space when that
-// leaves at least two stages, else it overlays the ring (which then holds at least the tile).
-// `cap` (> 1) bounds the ring depth.  Returns false when even the overlay does not fit.
-inline bool gemm_pick_stages(GemmShape& s, int epi_bytes, int cap = 0) {
-  const int avail = kSmemLimit - epi_bytes - 2048;
-  const int sb = gemm_stage_bytes(s.mma_n, s.split), ab = gemm_acc_bytes(s.mma_n);
+// Ring depth and accumulator placement for s.mma_n: the accumulator tile (if Epi has one) gets its
+// own space when that leaves at least two stages, else it overlays the ring (which then holds at
+// least the tile).  `cap` (> 1) bounds the ring depth.  Returns false when even that does not fit.
+template <class Epi>
+inline bool gemm_pick_stages(GemmShape& s, int cap = 0) {
+  const int avail = kSmemLimit - epi_smem_bytes<Epi>() - 2048;
+  const int sb = gemm_stage_bytes(s.mma_n, s.split);
+  const int ab = EpiFromRegs<Epi>::value ? 0 : gemm_acc_bytes(s.mma_n);
   int st = (avail - ab) / sb;
-  s.acc_alias = st < 2;
+  s.acc_alias = ab > 0 && st < 2;
   if (s.acc_alias) st = avail / sb;
   if (st > kMaxStages) st = kMaxStages;
   if (st > s.k_chunks * 2 && s.k_chunks * 2 >= 2) st = s.k_chunks * 2;
@@ -1745,7 +1884,7 @@ inline bool gemm_pick_stages(GemmShape& s, int epi_bytes, int cap = 0) {
   if (st < 2) st = 2;
   if (s.acc_alias && st * sb < ab) st = (ab + sb - 1) / sb;
   s.stages = st;
-  return st <= kMaxStages && gemm_smem_bytes(s, epi_bytes) <= kSmemLimit;
+  return st <= kMaxStages && gemm_smem_bytes<Epi>(s) <= kSmemLimit;
 }
 
 }  // namespace opp
