@@ -3,10 +3,13 @@
 (`python tests/kernel_checks.py [name ...]`), where every check runs in its own subprocess so that
 a device-side trap in one kernel cannot poison the others.
 """
+import contextlib
+import functools
 import math
 import subprocess
 import sys
 import os
+import tempfile
 
 import torch
 import torch.nn.functional as F
@@ -22,15 +25,45 @@ def _rand(*shape, scale=1.0, seed=0):
     return (torch.randn(*shape, generator=g) * scale).to(DEV)
 
 
+class _Tally:
+    """|got - ref| <= atol + rtol |ref| over one tensor compared in chunks; a NaN in `got` (an
+    element the kernel never wrote into a NaN-prefilled output) counts as out of tolerance."""
+
+    def __init__(self, name, rtol, atol):
+        self.name, self.rtol, self.atol = name, rtol, atol
+        self.n = self.bad = 0
+        self.max_err = self.worst = 0.0
+
+    def add(self, got, ref, slack=0.0):
+        """slack: a per-element term added to the tolerance"""
+        got, ref = got.float(), ref.float()
+        err = (got - ref).abs()
+        tol = self.atol + self.rtol * ref.abs() + slack
+        self.bad += (~(err <= tol)).sum().item()
+        self.n += err.numel()
+        if err.numel():
+            self.max_err = max(self.max_err, err.max().item())
+            self.worst = max(self.worst, (err / tol).max().item())
+
+    def check(self):
+        print(f"  {self.name}: max_abs_err={self.max_err:.3e} worst/tol={self.worst:.3f} bad={self.bad}/{self.n}")
+        assert self.bad == 0, f"{self.name}: {self.bad} elements out of tolerance (worst {self.worst:.2f}x)"
+
+
 def _close(name, got, ref, rtol, atol):
-    got, ref = got.float(), ref.float()
-    err = (got - ref).abs()
-    tol = atol + rtol * ref.abs()
-    bad = (err > tol).sum().item()
-    worst = (err / tol).max().item() if err.numel() else 0.0
-    print(f"  {name}: max_abs_err={err.max().item() if err.numel() else 0:.3e} "
-          f"worst/tol={worst:.3f} bad={bad}/{err.numel()}")
-    assert bad == 0, f"{name}: {bad} elements out of tolerance (worst {worst:.2f}x)"
+    t = _Tally(name, rtol, atol)
+    t.add(got, ref)
+    t.check()
+
+
+def _chunk(per_image):
+    """images per chunk of a reference computation: about 2^24 elements per tensor (128 MB in fp64)"""
+    return max(1, (1 << 24) // per_image)
+
+
+def _bits_equal(a, b):
+    """bit-identical fp16 tensors (torch.equal alone takes -0 for +0)"""
+    return torch.equal(a.view(torch.int16), b.view(torch.int16))
 
 
 def _elu1(x):
@@ -158,57 +191,193 @@ def check_linear_act_shared():
                *_tol(split, (2e-3, 2e-3), (2e-5, 2e-5)))
 
 
-def _conv_case(split, B, H, W, cin, cin_pad, cout, cout_pad, k, stride, act, resid, tokens, up=False):
-    xf = torch.zeros(B, H, W, cin_pad, device=DEV)
-    xf[..., :cin] = _rand(B, H, W, cin, seed=1)
+def _pad16(c):
+    return (c + 15) // 16 * 16
+
+
+def _nhwc_planes(B, H, W, c, c_pad, split, seed, scale=1.0):
+    """fp16 planes [B, H, W, planes * c_pad] of N(0, scale^2) values in channels [0, c) and zeros in
+    the padding channels, drawn on the device a few images at a time (a batch-64 map of the bench
+    shape is 2 GiB; no fp32 copy of it is made)"""
+    pl = 2 if split else 1
+    out = torch.empty(B, H, W, pl * c_pad, device=DEV, dtype=torch.half)
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    step = _chunk(H * W * c_pad)
+    for b0 in range(0, B, step):
+        n = min(step, B - b0)
+        xf = torch.zeros(n, H, W, c_pad, device=DEV)
+        xf[..., :c] = torch.randn(n, H, W, c, device=DEV, generator=g) * scale
+        out[b0:b0 + n] = _planes(xf, split)
+    return out
+
+
+def _up2x_ref(u, oh, ow):
+    """Bilinear x2 upsample (align_corners=True) of the NHWC map u [n, h, w, C] to oh x ow, sampled where
+    F.interpolate samples an fp32 map (scale (in-1)/(out-1) and scale * dst in fp32; the kernel's
+    epilogue does the same) and blended in fp64.  At a 256-wide output an fp32 position near 127 is
+    off by up to 7.6e-6, which times the difference of two neighbours is a few 1e-5 - as much as the
+    fp16x3 tolerance, although the kernel samples exactly where the model does."""
+    def axis(n_in, n_out):
+        f = torch.arange(n_out, dtype=torch.float32) * (torch.tensor(n_in - 1.0) / torch.tensor(n_out - 1.0))
+        i0 = f.long()
+        return i0.to(DEV), (i0 + 1).clamp(max=n_in - 1).to(DEV), (f - i0.float()).double().to(DEV)
+    y0, y1, wy = axis(u.shape[1], oh)
+    x0, x1, wx = axis(u.shape[2], ow)
+    wy, wx = wy.view(1, -1, 1, 1), wx.view(1, 1, -1, 1)
+    top, bot = u[:, y0], u[:, y1]
+    return ((top[:, :, x0] * (1 - wx) + top[:, :, x1] * wx) * (1 - wy)
+            + (bot[:, :, x0] * (1 - wx) + bot[:, :, x1] * wx) * wy)
+
+
+def _conv_params(cin, cin_pad, cout, cout_pad, k, split):
+    """filter planes [cout_pad, planes * k*k*cin_pad] (zero in the padding rows / channels) and bias"""
     wf = torch.zeros(cout_pad, k, k, cin_pad, device=DEV)
     wf[:cout, :, :, :cin] = _rand(cout, k, k, cin, scale=1.0 / math.sqrt(k * k * cin), seed=2)
     bias = torch.zeros(cout_pad, device=DEV)
     bias[:cout] = _rand(cout, seed=3) * 0.1
+    return _planes(wf.reshape(cout_pad, -1), split), bias
+
+
+def _accum_slack(k, cin):
+    """Tolerance term per unit |convolution sum| for fp16x3 convolutions at production K.  The wgmma
+    accumulator is rounded toward zero once per instruction: on the H100 the convolution sum shrinks
+    by about 1.7e-8 of itself per accumulating wgmma (regression of the error on the sum: R^2 0.75,
+    spread evenly over columns, images and tile rows; 3x3 convs at K = 1152, 1764, 2304).  The error
+    therefore grows with K and with the running sum, not with the output (the residual and the
+    upsampled map are added afterwards in fp32), and at K >= 1764 it exceeds 2e-5 + 2e-5 |out| in
+    about 1e-5 of the elements.  Bound: less than one ulp (2^-23) per wgmma, 3 per 16-channel K step
+    (hi.hi, hi.lo, lo.hi), of the running sum, taken as |sum| + the rms of the sums (a sum that ends
+    near zero has run through values of the usual size)."""
+    return 3 * k * k * -(-cin // 16) * 2.0 ** -23
+
+
+def _conv_case(split, B, H, W, cin, cin_pad, cout, cout_pad, k, stride, act, resid, tokens, up=False,
+               resid_is_input=False, check=True, accum_tol=False):
+    """One opp_conv2d_nhwc launch into NaN-prefilled outputs, checked against F.conv2d in fp64 on the
+    values the stored planes represent, + bias, bilinear x2 upsample-add, residual, activation and
+    (tokens) + pe, computed a few images at a time so that production batches stay within a few GB.
+    resid_is_input: the input map itself is the residual (the stride-1 BasicBlock's shortcut is the
+    block input, model.py:459-462).  check=False: launch only.  accum_tol: see _accum_slack.
+    Returns (out, tok)."""
     pad = k // 2
     oh, ow = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
     pl = 2 if split else 1
-    x16 = _planes(xf, split)
-    w16 = _planes(wf.reshape(cout_pad, -1), split)
-    res = resf = None
-    if resid:
-        resf = torch.zeros(B, oh, ow, cout_pad, device=DEV)
-        resf[..., :cout] = _rand(B, oh, ow, cout, seed=4)
-        res = _planes(resf, split)
+    x16 = _nhwc_planes(B, H, W, cin, cin_pad, split, seed=1)
+    w16, bias = _conv_params(cin, cin_pad, cout, cout_pad, k, split)
+    res = None
+    if resid_is_input:
+        assert resid and stride == 1 and (cin, cin_pad) == (cout, cout_pad)
+        res = x16
+    elif resid:
+        res = _nhwc_planes(B, oh, ow, cout, cout_pad, split, seed=4)
     out = torch.full((B, oh, ow, pl * cout_pad), float("nan"), device=DEV, dtype=torch.half)
     tok = pe = None
     if tokens:
         tok = torch.full((B, oh * ow, pl * cout_pad), float("nan"), device=DEV, dtype=torch.half)
         pe = _rand(oh * ow, cout_pad, seed=5)
-    up16 = upf = None
-    if up:   # FPN top-down merge: + bilinear x2 (align_corners=True) of a coarser map, fused in the epilogue
-        upf = torch.zeros(B, oh // 2, ow // 2, cout_pad, device=DEV)
-        upf[..., :cout] = _rand(B, oh // 2, ow // 2, cout, seed=6)
-        up16 = _planes(upf, split)
+    # FPN top-down merge: + bilinear x2 (align_corners=True) of a coarser map, fused in the epilogue
+    up16 = _nhwc_planes(B, oh // 2, ow // 2, cout, cout_pad, split, seed=6) if up else None
     _lib.call("opp_conv2d_nhwc", _lib.ptr(x16), _lib.ptr(w16), _lib.ptr(bias), _lib.ptr(res),
               _lib.ptr(out), B, H, W, cin_pad, cout_pad, k, stride, act, 0.01, _lib.ptr(tok),
               _lib.ptr(pe), _lib.ptr(up16), split, _lib.stream())
     torch.cuda.synchronize()
-    ref = F.conv2d(_q(xf, split).double().permute(0, 3, 1, 2), _q(wf, split).double().permute(0, 3, 1, 2),
-                   bias.double(), stride=stride, padding=pad).permute(0, 2, 3, 1)
-    if up:
-        ref = ref + F.interpolate(_q(upf, split).double().permute(0, 3, 1, 2), scale_factor=2.0, mode="bilinear",
-                                  align_corners=True).permute(0, 2, 3, 1)
-    if resid:
-        ref = ref + _q(resf, split).double()
-    if act == 1:
-        ref = torch.relu(ref)
-    elif act == 2:
-        ref = F.leaky_relu(ref, 0.01)
-    ref = ref.float()
-    name = f"conv split={split} k={k} s={stride} {cin}->{cout} {H}x{W} act={act} resid={resid} up={up}"
-    got = _unplanes(out, split)
-    _close(name, got, ref, *_tol(split, (2e-3, 3e-3), (2e-5, 2e-5)))
-    if cout_pad > cout:
-        assert got[..., cout:].abs().max().item() == 0.0, "padding channels must stay zero"
+    if not check:
+        return out, tok
+    name = (f"conv split={split} B={B} k={k} s={stride} {cin}->{cout} {H}x{W} act={act} resid={resid}"
+            f"{' (input)' if resid_is_input else ''} tokens={tokens} up={up}")
+    tol = _tol(split, (2e-3, 3e-3), (2e-5, 2e-5))
+    t_out, t_tok = _Tally(name, *tol), _Tally(name + " tok", *tol)
+    g = _accum_slack(k, cin) if (accum_tol and split) else 0.0
+    w64 = _unplanes(w16, split).view(cout_pad, k, k, cin_pad)[..., :cin].double().permute(0, 3, 1, 2)
+    step = _chunk(max(H * W * cin, oh * ow * cout_pad))
+    for b0 in range(0, B, step):
+        sl = slice(b0, b0 + step)
+        xin = _unplanes(x16[sl], split)[..., :cin].double().permute(0, 3, 1, 2)
+        acc = F.conv2d(xin, w64, None, stride=stride, padding=pad)
+        ref = (acc + bias.double().view(1, -1, 1, 1)).permute(0, 2, 3, 1)
+        if up:
+            ref = ref + _up2x_ref(_unplanes(up16[sl], split).double(), oh, ow)
+        if resid:
+            ref = ref + _unplanes(res[sl], split).double()
+        if act == 1:
+            ref = torch.relu(ref)
+        elif act == 2:
+            ref = F.leaky_relu(ref, 0.01)
+        got = _unplanes(out[sl], split)
+        slack = g * (acc.abs() + acc.square().mean().sqrt()).permute(0, 2, 3, 1) if g else 0.0
+        t_out.add(got, ref, slack)
+        if cout_pad > cout:
+            assert got[..., cout:].abs().max().item() == 0.0, "padding channels must stay zero"
+        if tokens:
+            t_tok.add(_unplanes(tok[sl], split), ref.reshape(-1, oh * ow, cout_pad) + pe.double(),
+                      slack.reshape(-1, oh * ow, cout_pad) if g else 0.0)
+    t_out.check()
     if tokens:
-        _close(name + " tok", _unplanes(tok, split), ref.reshape(B, oh * ow, cout_pad) + pe,
-               *_tol(split, (2e-3, 3e-3), (2e-5, 2e-5)))
+        t_tok.check()
+    return out, tok
+
+
+# ------------------------------------------------------------------ engine tile log ($OPP_LOG_TILES=1)
+TILE_PREFIX = "opp gemm tile: "
+_TILES_SEEN = []   # every tile configuration this process has printed, as dicts
+
+
+@contextlib.contextmanager
+def _tile_log():
+    """Collects the tile configurations the engine prints while the block runs ($OPP_LOG_TILES=1):
+    the yielded list holds them, as dicts ("mode", "n", "block_n", "mma_n", "stages", "cluster", ...),
+    when the block ends.  The engine writes them to file descriptor 2, which is redirected meanwhile;
+    everything else written there is passed on."""
+    new = []
+    sys.stderr.flush()
+    saved = os.dup(2)
+    with tempfile.TemporaryFile() as f:
+        os.dup2(f.fileno(), 2)
+        try:
+            yield new
+        finally:
+            os.dup2(saved, 2)
+            os.close(saved)
+            f.seek(0)
+            for line in f.read().decode(errors="replace").splitlines():
+                if line.startswith(TILE_PREFIX):
+                    fl = line[len(TILE_PREFIX):].split()
+                    new.append({fl[i]: int(fl[i + 1]) for i in range(0, len(fl) - 1, 2)})
+                else:
+                    sys.stderr.write(line + "\n")
+            _TILES_SEEN.extend(new)
+
+
+def _launch_tile(new, mode, n, k, conv_c):
+    """Tile configuration of the one GEMM launch that ran under _tile_log (`new`).  The engine prints a
+    configuration once per process: a launch that printed nothing has the configuration of an earlier
+    one with the same (mode, n, k, conv_c), which must then be unique."""
+    same = lambda t: (t["mode"], t["n"], t["k"], t["conv_c"]) == (mode, n, k, conv_c)   # noqa: E731
+    mine = [t for t in new if same(t)] or [t for t in _TILES_SEEN if same(t)]
+    assert len(mine) == 1, f"no unique tile line for mode {mode} n {n} k {k} conv_c {conv_c}: {mine}"
+    return mine[0]
+
+
+def _cluster_tiles(t, batches, m_tiles, grid_m_tiles=None):
+    """(fewest, most) tiles one cluster of the persistent grid walks: super tiles of `cluster` adjacent
+    M tiles per N tile, dealt round-robin to min(super tiles, SMs / cluster) clusters.  grid_m_tiles:
+    the M tiles the grid was sized for when the kernel reads a smaller row count from the device."""
+    def sup(m):
+        return batches * -(-m // t["cluster"]) * -(-t["n"] // t["block_n"])
+    clusters = min(sup(grid_m_tiles or m_tiles), _lib.load().opp_num_sms() // t["cluster"])
+    return sup(m_tiles) // clusters, -(-sup(m_tiles) // clusters)
+
+
+def _conv_tile(new, cin_pad, cout_pad, k, mode=1):
+    return _launch_tile(new, mode, cout_pad, k * k * -(-cin_pad // 64) * 64, cin_pad)
+
+
+def _run_child(name, timeout=900, **env):
+    """CHECKS/CHILD_CHECKS entry `name` in a child process with `env` added: the engine reads its knobs
+    ($OPP_CLUSTER, $OPP_STAGES, $OPP_NSPLIT, $OPP_LOG_TILES) once per process"""
+    r = subprocess.run([sys.executable, os.path.abspath(__file__), "--one", name], env=dict(os.environ, **env),
+                       timeout=timeout)
+    assert r.returncode == 0, f"{name} failed in a child process with {env}"
 
 
 def check_conv():
@@ -239,9 +408,210 @@ def check_conv_up_odd_clusters():
     bias.  The cluster size is read once per process ($OPP_CLUSTER), hence the child process."""
     sms = torch.cuda.get_device_properties(DEV).multi_processor_count
     cluster = next((c for c in (4, 2) if (sms // c) % 2 == 1), 4)
-    env = dict(os.environ, OPP_CLUSTER=str(cluster))
-    r = subprocess.run([sys.executable, os.path.abspath(__file__), "--one", "conv_up"], env=env, timeout=600)
-    assert r.returncode == 0, f"fused-upsample conv checks failed with OPP_CLUSTER={cluster} ({sms} SMs)"
+    print(f"  OPP_CLUSTER={cluster} ({sms} SMs)")
+    _run_child("conv_up", timeout=600, OPP_CLUSTER=str(cluster))
+
+
+# Every opp_conv2d_nhwc launch of the backbone (model.py _backbone and _fine_head_dense) for 512x512
+# images: feature maps of 256^2, 128^2 and 64^2 pixels, batch 8 at the first two output sizes and 32 at
+# the last, so that each cluster of the persistent grid walks several tiles (as at bench.py's batch 64:
+# the bias staged once per CTA, the ring phase carried from tile to tile, the two warpgroups apart).
+# extra: "resid" (a residual map), "resid=input" (the input map is the residual), "tokens" (+ pe into
+# the token rows), "up" (+ bilinear x2 of a coarser map).  The expected tile configuration of the
+# fp16x3 mode (mma_n, N tiles, ring stages, cluster) is the one bench.py's batch 64 runs with; the
+# fp16 mode has deeper rings, so only (mma_n, N tiles) is pinned there.
+#  name                  batch  in  cin  cout k  s act extra          fp16x3            fp16
+BACKBONE_CONVS = [
+    ("layer1 conv1",         8, 256, 128, 128, 3, 1, 1, "",            (128, 1, 3, 2), (128, 1)),
+    ("layer1 conv2",         8, 256, 128, 128, 3, 1, 1, "resid=input", (128, 1, 3, 2), (128, 1)),
+    ("layer2.0 conv1",       8, 256, 128, 196, 3, 2, 1, "",            (208, 1, 2, 2), (208, 1)),
+    ("layer2.0 down",        8, 256, 128, 196, 1, 2, 0, "",            (208, 1, 2, 2), (208, 1)),
+    ("layer2 conv2",         8, 128, 196, 196, 3, 1, 1, "resid=input", (208, 1, 2, 2), (208, 1)),
+    ("layer3.0 conv1",      32, 128, 196, 256, 3, 2, 1, "",            (256, 1, 2, 2), (256, 1)),
+    ("layer3.0 down",       32, 128, 196, 256, 1, 2, 0, "",            (256, 1, 2, 2), (256, 1)),
+    ("layer3 conv2",        32,  64, 256, 256, 3, 1, 1, "resid",       (256, 1, 2, 2), (256, 1)),
+    ("layer3_outconv",      32,  64, 256, 256, 1, 1, 0, "tokens",      (256, 1, 2, 2), (256, 1)),
+    ("layer2_outconv",       8, 128, 196, 256, 1, 1, 0, "up",          (128, 2, 2, 2), (256, 1)),
+    ("layer2_outconv2.0",    8, 128, 256, 256, 3, 1, 2, "",            (256, 1, 2, 2), (256, 1)),
+    ("layer2_outconv2.3",    8, 128, 256, 196, 3, 1, 0, "",            (208, 1, 2, 2), (208, 1)),
+    ("layer1_outconv",       8, 256, 128, 196, 1, 1, 0, "up",          (208, 1, 2, 2), (208, 1)),
+    ("layer1_outconv2.0",    8, 256, 196, 196, 3, 1, 2, "",            (208, 1, 2, 2), (208, 1)),
+    ("layer1_outconv2.3",    8, 256, 196, 128, 3, 1, 0, "",            (128, 1, 3, 2), (128, 1)),
+]
+
+
+def _backbone_conv(split, name, check=True):
+    """one BACKBONE_CONVS launch through _conv_case -> (out, tok, tile line, (fewest, most) tiles per cluster)"""
+    (_, B, hw, cin, cout, k, stride, act, extra, _, _) = next(c for c in BACKBONE_CONVS if c[0] == name)
+    with _tile_log() as new:
+        out, tok = _conv_case(split, B, hw, hw, cin, _pad16(cin), cout, _pad16(cout), k, stride, act,
+                              extra.startswith("resid"), extra == "tokens", up=extra == "up",
+                              resid_is_input=extra == "resid=input", check=check, accum_tol=True)
+    t = _conv_tile(new, _pad16(cin), _pad16(cout), k)
+    oh = (hw - 1) // stride + 1
+    return out, tok, t, _cluster_tiles(t, B, -(-oh // 16) * -(-oh // 8))
+
+
+def _conv_layers(split):
+    failed = []
+    for (name, B, hw, cin, cout, k, stride, act, extra, want1, want0) in BACKBONE_CONVS:
+        try:
+            _, _, t, (lo, hi) = _backbone_conv(split, name)
+            got = (t["mma_n"], -(-t["n"] // t["block_n"]), t["stages"], t["cluster"])
+            print(f"  {name}: mma_n {got[0]} N tiles {got[1]} stages {got[2]} alias {t['alias']} cluster {got[3]} "
+                  f"tiles per cluster {lo}-{hi}")
+            if split:
+                assert got == want1, f"{name}: tile (mma_n, N tiles, stages, cluster) = {got}, expected {want1}"
+            else:
+                assert got[:2] == want0, f"{name}: tile (mma_n, N tiles) = {got[:2]}, expected {want0}"
+            assert hi >= 8, f"{name}: only {hi} tiles per cluster at batch {B}"
+        except AssertionError as e:   # go on: which launches fail locates a defect
+            print(f"  {name}: FAILED: {e}")
+            failed.append(name)
+    assert not failed, f"split={split}: {failed}"
+
+
+def check_conv_layers():
+    """The backbone's convolutions at production widths and tile configurations against fp64
+    (BACKBONE_CONVS), in both operand modes; the tile log shows which configuration each one ran."""
+    for split in (1, 0):
+        _run_child(f"conv_layers_split{split}", OPP_LOG_TILES="1")
+
+
+# conv_launch_invariance: per output element the K order, the MMA sequence and the epilogue order do
+# not depend on the grid, so which CTA computes a pixel must not change it.  Launch configurations
+# forced through the engine's knobs, and the tile fields each must show in the log.
+INVARIANCE_VARIANTS = {
+    "default": ({}, {"layer1 conv2": {"cluster": 2, "stages": 3}, "layer2 conv2": {"cluster": 2},
+                     "layer3_outconv": {"cluster": 2}, "layer3 conv2 batch 1": {"mma_n": 64, "block_n": 64}}),
+    # pick_cluster takes 4 where the W slices stay whole swizzle groups (N = 128, 256), not at 208
+    "cluster4": ({"OPP_CLUSTER": "4"}, {"layer1 conv2": {"cluster": 4}, "layer2 conv2": {"cluster": 2},
+                                        "layer3_outconv": {"cluster": 4}}),
+    "stages2": ({"OPP_STAGES": "2"}, {"layer1 conv2": {"stages": 2}}),
+    # batch 1 at 64^2: the latency split runs 4 N tiles of 64 columns; without it, one of 256
+    "nsplit0": ({"OPP_NSPLIT": "0"}, {"layer3 conv2 batch 1": {"mma_n": 256, "block_n": 256}}),
+}
+
+
+def _conv_variant(tag):
+    """The INVARIANCE_VARIANTS[tag] launches (fp16x3) under this process's knobs; outputs saved to
+    $KERNEL_CHECK_DIR/<tag>.pt.  The default configuration is also checked against fp64."""
+    _, launches = INVARIANCE_VARIANTS[tag]
+    saved = {}
+    for name, want in launches.items():
+        if name == "layer3 conv2 batch 1":
+            with _tile_log() as new:
+                out, tok = _conv_case(1, 1, 64, 64, 256, 256, 256, 256, 3, 1, 1, True, False, check=tag == "default",
+                                      accum_tol=True)
+            t = _conv_tile(new, 256, 256, 3)
+        else:
+            out, tok, t, _ = _backbone_conv(1, name, check=tag == "default")
+        print(f"  [{tag}] {name}: mma_n {t['mma_n']} block_n {t['block_n']} stages {t['stages']} cluster {t['cluster']}")
+        assert all(t[f] == v for f, v in want.items()), f"[{tag}] {name}: tile {t}, expected {want}"
+        saved[name] = (out.cpu(), tok.cpu() if tok is not None else None)
+    torch.save(saved, os.path.join(os.environ["KERNEL_CHECK_DIR"], f"{tag}.pt"))
+
+
+def _conv_batch_slices():
+    """The dominant launch as bench.py runs it: layer1.x conv2 (3x3 128->128 + the block input, ReLU)
+    over batch 64 of 512x512 images in the fp16x3 mode, with the conv input, the block input and the
+    output 2 GiB each.  NaN-free, and every 8-image slice bit-identical to a batch-8 launch on the same
+    images (the configuration conv_layers checks against fp64) - every tile of the batch-64 launch is
+    checked without an fp64 reference at batch 64.  Likewise at N = 208, where no knob changes the
+    launch: each image of the batch-8 layer2 conv2 (7-8 tiles per cluster) against a batch-1 launch
+    of that image (one tile per cluster)."""
+    B, hw, c = 64, 256, 128
+    t64 = _nhwc_planes(B, hw, hw, c, c, 1, seed=1)     # t: the output of the block's conv1
+    x64 = _nhwc_planes(B, hw, hw, c, c, 1, seed=4)     # the block input, added as the residual
+    w16, bias = _conv_params(c, c, c, c, 3, 1)
+    out64 = torch.full((B, hw, hw, 2 * c), float("nan"), device=DEV, dtype=torch.half)
+    with _tile_log() as new:
+        ops.conv2d_nhwc(t64, w16, bias, out64, 3, 1, 1, act=1, resid=x64)
+    t_big = _conv_tile(new, c, c, 3)
+    lo, hi = _cluster_tiles(t_big, B, (hw // 16) * (hw // 8))
+    print(f"  batch 64: mma_n {t_big['mma_n']} stages {t_big['stages']} cluster {t_big['cluster']} "
+          f"tiles per cluster {lo}-{hi}")
+    out8 = torch.empty(8, hw, hw, 2 * c, device=DEV, dtype=torch.half)
+    differ = []
+    for b0 in range(0, B, 8):
+        sl = slice(b0, b0 + 8)
+        assert not torch.isnan(out64[sl]).any(), f"batch 64: NaN (unwritten) outputs in images {b0}-{b0 + 7}"
+        out8.fill_(float("nan"))
+        with _tile_log() as new:
+            ops.conv2d_nhwc(t64[sl], w16, bias, out8, 3, 1, 1, act=1, resid=x64[sl])
+        t8 = _conv_tile(new, c, c, 3)
+        assert all(t8[f] == t_big[f] for f in ("mma_n", "stages", "cluster")), (t8, t_big)
+        if not _bits_equal(out8, out64[sl]):
+            differ.append(f"images {b0}-{b0 + 7}: {int((out8 != out64[sl]).sum())} elements")
+    assert not differ, f"batch-64 launch differs from batch-8 launches of the same images: {differ}"
+    print("  batch 64: NaN-free, every 8-image slice bit-identical to its batch-8 launch")
+    del t64, x64, out64, out8
+    B, hw, c, c_pad = 8, 128, 196, 208
+    x8 = _nhwc_planes(B, hw, hw, c, c_pad, 1, seed=1)
+    w16, bias = _conv_params(c, c_pad, c, c_pad, 3, 1)
+    out8 = torch.full((B, hw, hw, 2 * c_pad), float("nan"), device=DEV, dtype=torch.half)
+    with _tile_log() as new:
+        ops.conv2d_nhwc(x8, w16, bias, out8, 3, 1, 1, act=1, resid=x8)
+    t8 = _conv_tile(new, c_pad, c_pad, 3)
+    lo8 = _cluster_tiles(t8, B, (hw // 16) * (hw // 8))[0]
+    assert t8["mma_n"] == 208 and lo8 > 1, t8
+    assert not torch.isnan(out8).any(), "N = 208: NaN (unwritten) outputs in the batch-8 launch"
+    out1 = torch.empty(1, hw, hw, 2 * c_pad, device=DEV, dtype=torch.half)
+    for b in range(B):
+        out1.fill_(float("nan"))
+        with _tile_log() as new:
+            ops.conv2d_nhwc(x8[b:b + 1], w16, bias, out1, 3, 1, 1, act=1, resid=x8[b:b + 1])
+        t1 = _conv_tile(new, c_pad, c_pad, 3)
+        assert t1["mma_n"] == 208 and _cluster_tiles(t1, 1, (hw // 16) * (hw // 8))[1] < lo8, t1
+        if not _bits_equal(out1, out8[b:b + 1]):
+            differ.append(f"image {b}: {int((out1 != out8[b:b + 1]).sum())} elements")
+    assert not differ, f"N = 208: batch-8 launch differs from batch-1 launches of the same images: {differ}"
+    print("  N = 208: every image of the batch-8 launch bit-identical to its batch-1 launch")
+
+
+def check_conv_launch_invariance():
+    """INVARIANCE_VARIANTS against the default configuration, bit for bit, and _conv_batch_slices."""
+    with tempfile.TemporaryDirectory() as d:
+        for tag, (env, _) in INVARIANCE_VARIANTS.items():
+            _run_child(f"conv_variant_{tag}", OPP_LOG_TILES="1", KERNEL_CHECK_DIR=d, **env)
+        base = torch.load(os.path.join(d, "default.pt"))
+        differ = []
+        for tag in INVARIANCE_VARIANTS:
+            if tag == "default":
+                continue
+            for name, tensors in torch.load(os.path.join(d, f"{tag}.pt")).items():
+                for what, a, b in zip(("out", "tok"), tensors, base[name]):
+                    if a is None:
+                        continue
+                    if _bits_equal(a, b):
+                        print(f"  {tag} vs default, {name} {what}: bit-identical")
+                        continue
+                    diff = (_unplanes(a, 1) - _unplanes(b, 1)).abs().max().item()
+                    print(f"  {tag} vs default, {name} {what}: {int((a != b).sum())} fp16 elements differ, "
+                          f"max |diff| of the represented values {diff:.3e}")
+                    differ.append(f"{tag}: {name} {what}")
+    _run_child("conv_batch_slices", OPP_LOG_TILES="1")
+    assert not differ, f"outputs depend on the launch configuration: {differ}"
+
+
+def _win_mismatches(got, dense, b_ids, j_ids, wc, win, org, outside_zero, stride=4):
+    """Window positions (match, ly, lx) of opp_conv_win's compact output `got` [>= M, win, pitch, C]
+    whose fp16 bits differ from the dense map `dense` [B, H, W, C] at image position
+    (stride * cell + org + (ly, lx)), for the M = len(j_ids) matches.  Positions outside the image
+    must be zero when outside_zero (conv A's 7x7 windows: they are conv B's zero padding), else they
+    are not compared (conv B's 5x5 windows: the gather never reads them)."""
+    M = j_ids.numel()
+    _, H, W, _ = dense.shape
+    r = torch.arange(win, device=DEV)
+    y = (stride * (j_ids // wc) + org).view(M, 1, 1) + r.view(1, win, 1)
+    x = (stride * (j_ids % wc) + org).view(M, 1, 1) + r.view(1, 1, win)
+    inside = (y >= 0) & (y < H) & (x >= 0) & (x < W)
+    want = dense[b_ids.view(M, 1, 1), y.clamp(0, H - 1), x.clamp(0, W - 1)]
+    want = torch.where(inside[..., None], want, torch.zeros_like(want))
+    differs = (got[:M, :, :win].view(torch.int16) != want.view(torch.int16)).any(-1)
+    if not outside_zero:
+        differs &= inside
+    return int(differs.sum())
 
 
 def check_conv_win():
@@ -287,22 +657,8 @@ def check_conv_win():
                          count=count)
             ops.conv_win(t_w, w1, b1, o_w, 5, split, cap, count=count)
             torch.cuda.synchronize()
-            cy, cx = (j_ids // wc).cpu(), (j_ids % wc).cpu()
-            bad_t = bad_o = 0
-            for m in range(M):
-                for (win, org, got, dense) in ((7, -3, t_w, t_d), (5, -2, o_w, o_d)):
-                    for ly in range(win):
-                        for lx in range(win):
-                            y, x = 4 * int(cy[m]) + org + ly, 4 * int(cx[m]) + org + lx
-                            inside = 0 <= y < H and 0 <= x < W
-                            if win == 5 and not inside:
-                                continue      # the gather never reads these
-                            want = dense[int(b_ids[m]), y, x] if inside else torch.zeros_like(got[m, ly, lx])
-                            if not torch.equal(got[m, ly, lx], want):
-                                if win == 7:
-                                    bad_t += 1
-                                else:
-                                    bad_o += 1
+            bad_t = _win_mismatches(t_w, t_d, b_ids, j_ids, wc, 7, -3, True)
+            bad_o = _win_mismatches(o_w, o_d, b_ids, j_ids, wc, 5, -2, False)
             assert bad_t == 0 and bad_o == 0, (f"conv_win split={split} B={B} {H}x{W} M={M} dyn={dyn}: {bad_t} window "
                                                f"positions of conv A and {bad_o} of conv B differ from the dense conv")
             if dyn:
@@ -313,6 +669,65 @@ def check_conv_win():
             _close(f"conv_win dense-ref split={split}", _unplanes(t_d, split), ref.permute(0, 2, 3, 1).float(),
                    *_tol(split, (2e-3, 3e-3), (2e-5, 2e-5)))
             print(f"conv_win split={split} B={B} {H}x{W} M={M} dyn={dyn}: windows bit-equal to the dense conv")
+
+
+def _conv_win_production():
+    """The window head (layer1_outconv2 on the match windows, model.py _fine_head_windows) at what a
+    batch of 512x512 images produces: 3000 matches over four 256x256 half-resolution maps, a
+    device-side match count below the capacity, windows on all four image borders.  Both window convs
+    must equal the dense convolutions of the same engine bit for bit (conv_layers checks those against
+    fp64 at this configuration), rows past the count must stay NaN, and every cluster of the
+    persistent grid must walk more than one tile."""
+    B, H, W, M, cap, stride = 4, 256, 256, 3000, 3100, 4
+    hc, wc = H // stride, W // stride
+    cin, cmid, cout = 196, 196, 128
+    for split in (0, 1):
+        pl = 2 if split else 1
+        x16 = _nhwc_planes(B, H, W, cin, _pad16(cin), split, seed=1)
+        w0, b0 = _conv_params(cin, _pad16(cin), cmid, _pad16(cmid), 3, split)
+        w1, b1 = _conv_params(cmid, _pad16(cmid), cout, cout, 3, split)
+        t_d = torch.empty(B, H, W, pl * _pad16(cmid), device=DEV, dtype=torch.half)
+        o_d = torch.empty(B, H, W, pl * cout, device=DEV, dtype=torch.half)
+        ops.conv2d_nhwc(x16, w0, b0, t_d, 3, 1, split, 2)
+        ops.conv2d_nhwc(t_d, w1, b1, o_d, 3, 1, split, 0)
+        g = torch.Generator().manual_seed(11)
+        b_ids = torch.randint(0, B, (M,), generator=g).sort().values
+        cy, cx = torch.randint(0, hc, (M,), generator=g), torch.randint(0, wc, (M,), generator=g)
+        # every 7th match on an image border: top, bottom, left, right in turn (the corners among them)
+        side = torch.arange(0, M, 7) // 7 % 4
+        cy[::7] = torch.where(side == 0, 0, torch.where(side == 1, hc - 1, cy[::7]))
+        cx[::7] = torch.where(side == 2, 0, torch.where(side == 3, wc - 1, cx[::7]))
+        cy[:4], cx[:4] = torch.tensor([0, 0, hc - 1, hc - 1]), torch.tensor([0, wc - 1, 0, wc - 1])
+        b_ids, j_ids = b_ids.to(DEV), (cy * wc + cx).to(DEV)
+        count = torch.tensor([M], dtype=torch.int32, device=DEV)
+        bi, ji = torch.cat([b_ids, b_ids.new_zeros(cap - M)]), torch.cat([j_ids, j_ids.new_zeros(cap - M)])
+        t_w = torch.full((cap, 7, 8, pl * _pad16(cmid)), float("nan"), device=DEV, dtype=torch.half)
+        o_w = torch.full((cap, 5, ops.conv_win_pitch(5), pl * cout), float("nan"), device=DEV, dtype=torch.half)
+        with _tile_log() as new_a:
+            ops.conv_win(x16, w0, b0, t_w, 7, split, cap, act=2, b_ids=bi, j_ids=ji, wc=wc, stride=stride, org=-3,
+                         count=count)
+        with _tile_log() as new_b:
+            ops.conv_win(t_w, w1, b1, o_w, 5, split, cap, count=count)
+        torch.cuda.synchronize()
+        name = f"conv_win_production split={split} B={B} {H}x{W} M={M} of {cap}"
+        for (new, win, c_in, c_out) in ((new_a, 7, _pad16(cin), _pad16(cmid)), (new_b, 5, _pad16(cmid), cout)):
+            t = _conv_tile(new, c_in, c_out, 3, mode=2)
+            per_tile = 128 // (ops.conv_win_pitch(win) * win)
+            lo, hi = _cluster_tiles(t, 1, -(-M // per_tile), grid_m_tiles=-(-cap // per_tile))
+            print(f"  {name} {win}x{win} windows: mma_n {t['mma_n']} stages {t['stages']} cluster {t['cluster']} "
+                  f"tiles per cluster {lo}-{hi}")
+            assert lo > 1, f"{name}: a cluster walks only {lo} tile(s) of the {win}x{win} window conv"
+        bad_t = _win_mismatches(t_w, t_d, b_ids, j_ids, wc, 7, -3, True, stride)
+        bad_o = _win_mismatches(o_w, o_d, b_ids, j_ids, wc, 5, -2, False, stride)
+        assert bad_t == 0 and bad_o == 0, (f"{name}: {bad_t} window positions of conv A and {bad_o} of conv B "
+                                           f"differ from the dense conv")
+        assert torch.isnan(t_w[M:].float()).all() and torch.isnan(o_w[M:].float()).all(), \
+            f"{name}: rows past the device-side match count were written"
+        print(f"  {name}: windows bit-equal to the dense conv, rows past the count untouched")
+
+
+def check_conv_win_production():
+    _run_child("conv_win_production_tiles", OPP_LOG_TILES="1")
 
 
 def check_sim():
@@ -393,16 +808,23 @@ def _conv1_gemm_case(split, B, H, W, C, u8):
     out = torch.full((B, H // 2, W // 2, pl * C), float("nan"), device=DEV, dtype=torch.half)
     ops.conv1_gemm(img, w16, a_buf, out, split)
     torch.cuda.synchronize()
-    ref = torch.relu(F.conv2d(imgf.double(), _q(w64, split)[:, :49].reshape(C, 1, 7, 7).double(),
-                              _q(w64, split)[:, 49].double(), stride=2, padding=3)).permute(0, 2, 3, 1).float()
-    _close(f"conv1_gemm split={split} u8={u8} {H}x{W}", _unplanes(out, split), ref,
-           *_tol(split, (2e-3, 2e-3), (2e-5, 2e-5)))
+    wq = _q(w64, split).double()
+    tally = _Tally(f"conv1_gemm split={split} u8={u8} B={B} {H}x{W}", *_tol(split, (2e-3, 2e-3), (2e-5, 2e-5)))
+    step = _chunk(H * W * C // 4)
+    for b0 in range(0, B, step):
+        sl = slice(b0, b0 + step)
+        ref = torch.relu(F.conv2d(imgf[sl].double(), wq[:, :49].reshape(C, 1, 7, 7), wq[:, 49], stride=2, padding=3))
+        tally.add(_unplanes(out[sl], split), ref.permute(0, 2, 3, 1))
+    tally.check()
 
 
 def check_conv1_gemm():
     for split in (0, 1):
         _conv1_gemm_case(split, 2, 96, 128, 128, False)
         _conv1_gemm_case(split, 1, 72, 200, 128, True)     # ragged 16x16 im2col tiles, uint8 image
+        # bench.py's image size: 524288 im2col rows per batch of 8
+        _conv1_gemm_case(split, 8, 512, 512, 128, False)
+        _conv1_gemm_case(split, 8, 512, 512, 128, True)
 
 
 def check_kpt_encode():
@@ -794,6 +1216,9 @@ CHECKS = {
     "conv": check_conv,
     "conv_up_odd_clusters": check_conv_up_odd_clusters,
     "conv_win": check_conv_win,
+    "conv_layers": check_conv_layers,
+    "conv_launch_invariance": check_conv_launch_invariance,
+    "conv_win_production": check_conv_win_production,
     "sim": check_sim,
     "conv1_gemm": check_conv1_gemm,
     "kpt_encode": check_kpt_encode,
@@ -809,14 +1234,20 @@ CHECKS = {
 
 
 # run only in a child process whose environment selects the launch configuration
-CHILD_CHECKS = {"conv_up": _conv_up_cases}
+CHILD_CHECKS = {"conv_up": _conv_up_cases,
+                "conv_layers_split1": functools.partial(_conv_layers, 1),
+                "conv_layers_split0": functools.partial(_conv_layers, 0),
+                "conv_batch_slices": _conv_batch_slices,
+                "conv_win_production_tiles": _conv_win_production,
+                **{f"conv_variant_{tag}": functools.partial(_conv_variant, tag) for tag in INVARIANCE_VARIANTS}}
+assert not CHECKS.keys() & CHILD_CHECKS.keys(), "`--one name` must name one function"
 
 
 def main(argv):
     if len(argv) == 2 and argv[0] == "--one":
         print(f"[{argv[1]}]")
         {**CHECKS, **CHILD_CHECKS}[argv[1]]()
-        print(f"[{argv[1]}] OK")
+        print(f"[{argv[1]}] OK (peak {torch.cuda.max_memory_allocated() / 2 ** 30:.2f} GiB allocated by torch)")
         return 0
     names = argv or list(CHECKS)
     failed = []
