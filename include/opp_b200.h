@@ -352,6 +352,24 @@ int opp_pnp_ransac(const float* pts3d, const float* pts2d, const long long* m_bi
                    unsigned seed, int refine_rounds, float* poses, int* n_inliers,
                    unsigned char* inlier_mask, int* status, opp_stream_t stream);
 
+/* The use_pycolmap_ransac branch of ransac_PnP (metric_utils.py:137-170:
+ * pycolmap.absolute_pose_estimation on a SIMPLE_PINHOLE camera), batched like opp_pnp_ransac and
+ * with the same inputs and outputs, except:
+ *   camera: f = K[0][0], principal point (K[0][2], K[1][2]); K[1][1] and the skew are not read;
+ *   no scale: the 3D points are used as given and t is in their units;
+ *   max_error_px: inlier = squared pixel error <= max_error_px^2 and in front of the camera;
+ *   support of a model = (inlier count, then the smaller sum of squared errors of the inliers);
+ *   lo_rounds: LO-RANSAC rounds (least squares on the inliers, kept while the support improves);
+ *   the pose is then refined on that fixed inlier set by minimising sum log(1 + |r_i|^2) over the
+ *   pixel residuals r_i (Cauchy loss of scale 1 per point), at most 100 iterations;
+ *   inlier_mask / n_inliers: the inliers of the RANSAC model, before that refinement.
+ * A frame with fewer than 4 matches, no admissible hypothesis or fewer than 4 inliers gets the
+ * identity pose, n_inliers 0, a zero mask and status 0. */
+int opp_pnp_ransac_colmap(const float* pts3d, const float* pts2d, const long long* m_bids, int m,
+                          const float* intrinsics, int batch, float max_error_px, int hypotheses,
+                          unsigned seed, int lo_rounds, float* poses, int* n_inliers,
+                          unsigned char* inlier_mask, int* status, opp_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * LINEMOD pose metrics — add_metric / projection_2d_error (src/utils/metric_utils.py:31-88, per
  * frame on the CPU with a scipy cKDTree for ADD-S; caller: the eval_ADD_metric branch of

@@ -56,6 +56,7 @@ SIGNATURES = {
     "opp_seq_attention": [P, P, P, I, I, I, F, I, P],
     "opp_fine_match_2d": [P, P, P, P, P, P, I, I, F, P],
     "opp_pnp_ransac": [P, P, P, I, P, I, F, F, I, ctypes.c_uint, I, P, P, P, P, P],
+    "opp_pnp_ransac_colmap": [P, P, P, I, P, I, F, I, ctypes.c_uint, I, P, P, P, P, P],
     "opp_pose_metrics": [P, I, P, P, P, P, I, P, L, P, P, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),

@@ -17,6 +17,8 @@
 //      inliers is what cv2's iterative refinement converges to as well, which is what the parity
 //      test compares against.
 // All geometry runs in fp64 (a few MFLOP per image); inputs / outputs are fp32.
+// The same kernel, instantiated for PnpSolver::kColmap (opp_pnp_ransac_colmap), is the reference's
+// use_pycolmap_ransac branch (metric_utils.py:137-170); see pnp_ransac_kernel.
 #include <cstdint>
 #include <cstdio>
 
@@ -238,12 +240,199 @@ __device__ double block_sum(double v, double* red) {
   return s;
 }
 
+// Adds the Gauss-Newton terms of match (p, u, v) at pose `ps` to acc[27]: the upper triangle of
+// J^T J, then J^T r, with r the pixel residual and J its derivative in (w, t) of the update
+// R <- exp([w]x) R, t <- t + dt.  A point behind the camera adds nothing.  kCauchy weights the
+// terms by w = 1 / (1 + |r|^2), the IRLS weight of the per-point loss log(1 + |r|^2), and adds
+// that loss to *cost (+inf behind the camera, so that a step moving an inlier there is refused).
+template <bool kCauchy>
+__device__ __forceinline__ void gn_terms(const Pose& ps, const Cam& cam, const double* p, double u, double v,
+                                         double* acc, double* cost) {
+  const double Y0 = ps.R[0] * p[0] + ps.R[1] * p[1] + ps.R[2] * p[2];
+  const double Y1 = ps.R[3] * p[0] + ps.R[4] * p[1] + ps.R[5] * p[2];
+  const double Y2 = ps.R[6] * p[0] + ps.R[7] * p[1] + ps.R[8] * p[2];
+  const double x = Y0 + ps.t[0], y = Y1 + ps.t[1], z = Y2 + ps.t[2];
+  if (!(z > 1e-9)) {
+    if constexpr (kCauchy) *cost = INFINITY;
+    return;
+  }
+  const double iz = 1.0 / z, xn = x * iz, yn = y * iz;
+  double ru = cam.fx * xn + cam.skew * yn + cam.cx - u;
+  double rv = cam.fy * yn + cam.cy - v;
+  // d(u)/dXc, d(v)/dXc
+  const double gu[3] = {cam.fx * iz, cam.skew * iz, -(cam.fx * xn + cam.skew * yn) * iz};
+  const double gv[3] = {0.0, cam.fy * iz, -cam.fy * yn * iz};
+  // Xc = exp(w) Y + t  ->  dXc/dw = -[Y]x ; J row = (g x ... ) : g^T (-[Y]x) = (Y x g)^T
+  const double Yv[3] = {Y0, Y1, Y2};
+  double ju[6], jv[6];
+  cross3(Yv, gu, ju);
+  cross3(Yv, gv, jv);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    ju[3 + k] = gu[k];
+    jv[3 + k] = gv[k];
+  }
+  if constexpr (kCauchy) {
+    const double s = ru * ru + rv * rv;
+    *cost += log1p(s);
+    const double sw = sqrt(1.0 / (1.0 + s));   // rows scaled by sqrt(w): J^T w J, J^T w r
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      ju[k] *= sw;
+      jv[k] *= sw;
+    }
+    ru *= sw;
+    rv *= sw;
+  }
+  int o = 0;
+#pragma unroll
+  for (int r_ = 0; r_ < 6; ++r_) {
+#pragma unroll
+    for (int c_ = r_; c_ < 6; ++c_) acc[o++] += ju[r_] * ju[c_] + jv[r_] * jv[c_];
+  }
+#pragma unroll
+  for (int r_ = 0; r_ < 6; ++r_) acc[21 + r_] += ju[r_] * ru + jv[r_] * rv;
+}
+
+// Solves (H + damping diag H) d = -g by Cholesky, H and g packed in Hs as gn_terms accumulates
+// them.  Returns false when the damped H is not positive definite.
+__device__ __forceinline__ bool solve_damped(const double* Hs, double damping, double* d) {
+  double H[6][6], g[6], L[6][6];
+  int o = 0;
+  for (int r_ = 0; r_ < 6; ++r_)
+    for (int c_ = r_; c_ < 6; ++c_) {
+      H[r_][c_] = Hs[o];
+      H[c_][r_] = Hs[o];
+      ++o;
+    }
+  for (int r_ = 0; r_ < 6; ++r_) {
+    g[r_] = Hs[21 + r_];
+    H[r_][r_] *= 1.0 + damping;
+  }
+  bool okc = true;
+  for (int r_ = 0; r_ < 6 && okc; ++r_)
+    for (int c_ = 0; c_ <= r_; ++c_) {
+      double s = H[r_][c_];
+      for (int k = 0; k < c_; ++k) s -= L[r_][k] * L[c_][k];
+      if (r_ == c_) {
+        if (!(s > 1e-300)) {
+          okc = false;
+          break;
+        }
+        L[r_][r_] = sqrt(s);
+      } else {
+        L[r_][c_] = s / L[c_][c_];
+      }
+    }
+  if (okc) {
+    double yv[6];
+    for (int r_ = 0; r_ < 6; ++r_) {
+      double s = -g[r_];
+      for (int k = 0; k < r_; ++k) s -= L[r_][k] * yv[k];
+      yv[r_] = s / L[r_][r_];
+    }
+    for (int r_ = 5; r_ >= 0; --r_) {
+      double s = yv[r_];
+      for (int k = r_ + 1; k < 6; ++k) s -= L[k][r_] * d[k];
+      d[r_] = s / L[r_][r_];
+    }
+  }
+  return okc;
+}
+
+// to = (exp([d0 d1 d2]x) from.R, from.t + (d3, d4, d5)) (Rodrigues); `to` may be `from`
+__device__ __forceinline__ void apply_step(const Pose& from, const double* d, Pose& to) {
+  const double th = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+  double E[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  if (th > 1e-16) {
+    const double kx = d[0] / th, ky = d[1] / th, kz = d[2] / th;
+    const double sn = sin(th), cs = 1.0 - cos(th);
+    const double Kx[9] = {0, -kz, ky, kz, 0, -kx, -ky, kx, 0};
+    double K2[9];
+    for (int r_ = 0; r_ < 3; ++r_)
+      for (int c_ = 0; c_ < 3; ++c_)
+        K2[r_ * 3 + c_] = Kx[r_ * 3] * Kx[c_] + Kx[r_ * 3 + 1] * Kx[3 + c_] + Kx[r_ * 3 + 2] * Kx[6 + c_];
+    for (int k = 0; k < 9; ++k) E[k] += sn * Kx[k] + cs * K2[k];
+  }
+  double Rn[9];
+  for (int r_ = 0; r_ < 3; ++r_)
+    for (int c_ = 0; c_ < 3; ++c_)
+      Rn[r_ * 3 + c_] = E[r_ * 3] * from.R[c_] + E[r_ * 3 + 1] * from.R[3 + c_] + E[r_ * 3 + 2] * from.R[6 + c_];
+  for (int k = 0; k < 9; ++k) to.R[k] = Rn[k];
+  for (int k = 0; k < 3; ++k) to.t[k] = from.t[k] + d[3 + k];
+}
+
+// Least squares of the reprojection error over the matches with mask[i] set: up to 10 Gauss-Newton
+// steps (normal equations reduced by the CTA, solved by thread 0) from `cur`.  Every thread calls
+// it; on return `cur` and the shared `sh_pose` hold the result.
+template <class Load>
+__device__ __forceinline__ void least_squares_on_mask(Pose& cur, Pose& sh_pose, const Cam& cam, const Load& load_pt,
+                                                      const unsigned char* mask, int n, double* red, double* Hs,
+                                                      int& flag) {
+  const int tid = threadIdx.x;
+  for (int it = 0; it < 10; ++it) {
+    double acc[27];
+#pragma unroll
+    for (int k = 0; k < 27; ++k) acc[k] = 0.0;
+    for (int i = tid; i < n; i += kPnpThreads) {
+      if (!mask[i]) continue;
+      double p[3], u, v;
+      load_pt(i, p, u, v);
+      gn_terms<false>(cur, cam, p, u, v, acc, nullptr);
+    }
+    for (int k = 0; k < 27; ++k) {
+      const double s = block_sum(acc[k], red);
+      if (tid == 0) Hs[k] = s;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      double d[6];
+      double step = 0.0;
+      const bool okc = solve_damped(Hs, 1e-9, d);
+      if (okc) {
+        apply_step(sh_pose, d, sh_pose);
+        for (int k = 0; k < 6; ++k) step = fmax(step, fabs(d[k]));
+      }
+      flag = (!okc || step < 1e-12) ? 1 : 0;
+    }
+    __syncthreads();
+    cur = sh_pose;
+    const int stop = flag;
+    __syncthreads();
+    if (stop) break;
+  }
+}
+
+// Support of a model in the COLMAP mode: inlier count, then the smaller sum of squared errors of
+// the inliers, then the lower hypothesis id (so that the winner does not depend on scheduling).
+struct Support {
+  int count;
+  double sse;
+  unsigned h;
+};
+__device__ __forceinline__ bool better(const Support& a, const Support& b) {
+  return a.count > b.count || (a.count == b.count && (a.sse < b.sse || (a.sse == b.sse && a.h < b.h)));
+}
+
+// kOpenCv: cv2.solvePnPRansac as the reference's default branch calls it (full K, err < thr, the
+//   3D points multiplied by `scale`), then `refine_rounds` rounds of least squares on the inliers
+//   with the inlier set re-evaluated between rounds.
+// kColmap: pycolmap.absolute_pose_estimation as the reference's use_pycolmap_ransac branch calls it
+//   (metric_utils.py:137-170): SIMPLE_PINHOLE camera (f = K[0][0], fy and skew ignored), inlier =
+//   err <= thr and in front, support = (count, smaller SSE); LO-RANSAC: least squares on the
+//   winner's inliers, kept while the support improves, for at most `refine_rounds` rounds; then the
+//   pose is refined on that fixed inlier set with the Cauchy loss sum log(1 + |r_i|^2) per point
+//   (IRLS Levenberg-Marquardt).  The mask is the RANSAC model's inlier set, before that refinement.
+enum class PnpSolver { kOpenCv, kColmap };
+
+template <PnpSolver kSolver>
 __global__ void __launch_bounds__(kPnpThreads)
 pnp_ransac_kernel(const float* __restrict__ pts3d, const float* __restrict__ pts2d,
                   const long long* __restrict__ m_bids, int M, const float* __restrict__ Kmat,
                   float scale, float thr, int n_hyp, unsigned seed, int refine_rounds,
                   float* __restrict__ pose_out, int* __restrict__ n_inl_out,
                   unsigned char* __restrict__ inl_mask, int* __restrict__ status_out) {
+  constexpr bool kColmap = kSolver == PnpSolver::kColmap;
   pdl_sync();
   __shared__ int seg[2];
   __shared__ unsigned long long best_key[kPnpThreads / 32];
@@ -267,6 +456,7 @@ pnp_ransac_kernel(const float* __restrict__ pts3d, const float* __restrict__ pts
   const int lo = seg[0], n = seg[1] - seg[0];
   const float* K = Kmat + b * 9;
   Cam cam{(double)K[0], (double)K[4], (double)K[2], (double)K[5], (double)K[1]};
+  if constexpr (kColmap) cam = Cam{(double)K[0], (double)K[0], (double)K[2], (double)K[5], 0.0};
   const double thr2 = (double)thr * (double)thr;
   float* pose = pose_out + b * 12;
   auto fail = [&]() {
@@ -292,6 +482,7 @@ pnp_ransac_kernel(const float* __restrict__ pts3d, const float* __restrict__ pts
 
   // ---------------------------------------------------------------- 1+2: hypotheses and scoring
   int my_count = -1;
+  double my_sse = INFINITY;
   unsigned my_h = 0xffffffffu;
   Pose my_pose;
   for (int h = tid; h < n_hyp; h += kPnpThreads) {
@@ -336,169 +527,300 @@ pnp_ransac_kernel(const float* __restrict__ pts3d, const float* __restrict__ pts
     });
     if (!(cand_err < INFINITY)) continue;
     int count = 0;
+    double sse = 0.0;
     for (int i = 0; i < n; ++i) {
       double p[3], u, v;
       load_pt(i, p, u, v);
-      count += reproj_err2(cand, cam, p, u, v) < thr2 ? 1 : 0;
+      const double e = reproj_err2(cand, cam, p, u, v);
+      if constexpr (kColmap) {
+        if (e <= thr2) {
+          ++count;
+          sse += e;
+        }
+      } else {
+        count += e < thr2 ? 1 : 0;
+      }
     }
-    if (count > my_count) {   // strided h is increasing: the first best stays (lowest id on ties)
+    // strided h is increasing: the first best stays (lowest id on ties)
+    if (count > my_count || (kColmap && count == my_count && sse < my_sse)) {
       my_count = count;
+      my_sse = sse;
       my_h = (unsigned)h;
       my_pose = cand;
     }
   }
-  // block argmax of (count, lowest h)
-  unsigned long long key = my_count < 0 ? 0ull
-                                        : (((unsigned long long)(unsigned)my_count + 1ull) << 32) |
-                                              (unsigned long long)(0xffffffffu - my_h);
-  unsigned long long wkey = key;
+  if constexpr (kColmap) {
+    // block argmax of the support (count, smaller sse, lower h)
+    __shared__ Support w_best[kPnpThreads / 32];
+    Support s{my_count, my_sse, my_h};
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const unsigned long long other = __shfl_xor_sync(0xffffffffu, wkey, o);
-    wkey = other > wkey ? other : wkey;
-  }
-  if ((tid & 31) == 0) best_key[tid >> 5] = wkey;
-  __syncthreads();
-  unsigned long long bkey = 0;
+    for (int o = 16; o > 0; o >>= 1) {
+      const Support other{__shfl_xor_sync(0xffffffffu, s.count, o), __shfl_xor_sync(0xffffffffu, s.sse, o),
+                          __shfl_xor_sync(0xffffffffu, s.h, o)};
+      if (better(other, s)) s = other;
+    }
+    if ((tid & 31) == 0) w_best[tid >> 5] = s;
+    __syncthreads();
+    Support best = w_best[0];
 #pragma unroll
-  for (int w = 0; w < kPnpThreads / 32; ++w) bkey = best_key[w] > bkey ? best_key[w] : bkey;
-  if (bkey == 0ull) {   // no admissible hypothesis at all
-    fail();
-    return;
+    for (int w = 1; w < kPnpThreads / 32; ++w)
+      if (better(w_best[w], best)) best = w_best[w];
+    if (best.count < 0) {   // no admissible hypothesis at all
+      fail();
+      return;
+    }
+    if (my_count >= 0 && my_h == best.h) best_pose = my_pose;   // h is unique
+  } else {
+    // block argmax of (count, lowest h)
+    unsigned long long key = my_count < 0 ? 0ull
+                                          : (((unsigned long long)(unsigned)my_count + 1ull) << 32) |
+                                                (unsigned long long)(0xffffffffu - my_h);
+    unsigned long long wkey = key;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long other = __shfl_xor_sync(0xffffffffu, wkey, o);
+      wkey = other > wkey ? other : wkey;
+    }
+    if ((tid & 31) == 0) best_key[tid >> 5] = wkey;
+    __syncthreads();
+    unsigned long long bkey = 0;
+#pragma unroll
+    for (int w = 0; w < kPnpThreads / 32; ++w) bkey = best_key[w] > bkey ? best_key[w] : bkey;
+    if (bkey == 0ull) {   // no admissible hypothesis at all
+      fail();
+      return;
+    }
+    if (key == bkey) best_pose = my_pose;   // keys are unique (h is)
   }
-  if (key == bkey) best_pose = my_pose;   // keys are unique (h is)
   __syncthreads();
   Pose cur = best_pose;
+  unsigned char* mask = inl_mask + lo;
 
-  // ---------------------------------------------------------------- 3: refinement on the inliers
   int n_inl = 0;
-  for (int round = 0; round <= refine_rounds; ++round) {
-    // inlier set under the current pose
-    int cnt = 0;
-    for (int i = tid; i < n; i += kPnpThreads) {
-      double p[3], u, v;
-      load_pt(i, p, u, v);
-      const unsigned char in = reproj_err2(cur, cam, p, u, v) < thr2 ? 1 : 0;
-      inl_mask[lo + i] = in;
-      cnt += in;
+  if constexpr (kColmap) {
+    // ---------------------------------------------------------------- 3: local optimisation
+    // support of `ps` over the CTA (fixed-order sums), its inlier set written to the mask
+    auto score = [&](const Pose& ps, int& cnt_out, double& sse_out) {
+      int cnt = 0;
+      double sse = 0.0;
+      for (int i = tid; i < n; i += kPnpThreads) {
+        double p[3], u, v;
+        load_pt(i, p, u, v);
+        const double e = reproj_err2(ps, cam, p, u, v);
+        const unsigned char in = e <= thr2 ? 1 : 0;
+        mask[i] = in;
+        cnt += in;
+        sse += in ? e : 0.0;
+      }
+      cnt_out = (int)(block_sum((double)cnt, red) + 0.5);
+      sse_out = block_sum(sse, red);
+    };
+    double sse;
+    score(cur, n_inl, sse);
+    for (int round = 0; round < refine_rounds && n_inl >= 4; ++round) {
+      __syncthreads();   // mask written by other threads is read below
+      const Pose prev = cur;
+      least_squares_on_mask(cur, best_pose, cam, load_pt, mask, n, red, Hs, flag);
+      int cnt2;
+      double sse2;
+      score(cur, cnt2, sse2);
+      if (cnt2 > n_inl || (cnt2 == n_inl && sse2 < sse)) {
+        n_inl = cnt2;
+        sse = sse2;
+      } else {   // not better: back to the previous model and its inlier set
+        cur = prev;
+        score(cur, n_inl, sse);
+        break;
+      }
     }
-    n_inl = (int)(block_sum((double)cnt, red) + 0.5);
-    if (round == refine_rounds || n_inl < 4) break;
-    __syncthreads();   // inl_mask written by other threads is read below
-    for (int it = 0; it < 10; ++it) {
-      double acc[27];
+    if (n_inl < 4) {
+      fail();
+      return;
+    }
+    // ---------------------------------------------------------------- 4: Cauchy refinement
+    // weighted normal equations and cost sum log(1 + |r|^2) over the inliers at `ps` -> out[28]
+    __shared__ double Hc[2][28];
+    auto cauchy_terms = [&](const Pose& ps, double* out) {
+      double acc[27], cost = 0.0;
 #pragma unroll
       for (int k = 0; k < 27; ++k) acc[k] = 0.0;
       for (int i = tid; i < n; i += kPnpThreads) {
-        if (!inl_mask[lo + i]) continue;
+        if (!mask[i]) continue;
         double p[3], u, v;
         load_pt(i, p, u, v);
-        const double Y0 = cur.R[0] * p[0] + cur.R[1] * p[1] + cur.R[2] * p[2];
-        const double Y1 = cur.R[3] * p[0] + cur.R[4] * p[1] + cur.R[5] * p[2];
-        const double Y2 = cur.R[6] * p[0] + cur.R[7] * p[1] + cur.R[8] * p[2];
-        const double x = Y0 + cur.t[0], y = Y1 + cur.t[1], z = Y2 + cur.t[2];
-        if (!(z > 1e-9)) continue;
-        const double iz = 1.0 / z, xn = x * iz, yn = y * iz;
-        const double ru = cam.fx * xn + cam.skew * yn + cam.cx - u;
-        const double rv = cam.fy * yn + cam.cy - v;
-        // d(u)/dXc, d(v)/dXc
-        const double gu[3] = {cam.fx * iz, cam.skew * iz, -(cam.fx * xn + cam.skew * yn) * iz};
-        const double gv[3] = {0.0, cam.fy * iz, -cam.fy * yn * iz};
-        // Xc = exp(w) Y + t  ->  dXc/dw = -[Y]x ; J row = (g x ... ) : g^T (-[Y]x) = (Y x g)^T
-        const double Yv[3] = {Y0, Y1, Y2};
-        double ju[6], jv[6];
-        cross3(Yv, gu, ju);
-        cross3(Yv, gv, jv);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          ju[3 + k] = gu[k];
-          jv[3 + k] = gv[k];
-        }
-        int o = 0;
-#pragma unroll
-        for (int r_ = 0; r_ < 6; ++r_) {
-#pragma unroll
-          for (int c_ = r_; c_ < 6; ++c_) acc[o++] += ju[r_] * ju[c_] + jv[r_] * jv[c_];
-        }
-#pragma unroll
-        for (int r_ = 0; r_ < 6; ++r_) acc[21 + r_] += ju[r_] * ru + jv[r_] * rv;
+        gn_terms<true>(ps, cam, p, u, v, acc, &cost);
       }
       for (int k = 0; k < 27; ++k) {
         const double s = block_sum(acc[k], red);
-        if (tid == 0) Hs[k] = s;
+        if (tid == 0) out[k] = s;
       }
+      const double c = block_sum(cost, red);
+      if (tid == 0) out[27] = c;
       __syncthreads();
+    };
+    __syncthreads();   // mask written by other threads is read below
+    int buf = 0;
+    cauchy_terms(cur, Hc[buf]);
+    double cost = Hc[buf][27];
+    double lambda = 1e-4;   // Levenberg-Marquardt damping, relative to diag H
+    for (int it = 0; it < 100; ++it) {
       if (tid == 0) {
-        // solve (H + lambda diag H) d = -g by Cholesky
-        double H[6][6], g[6], L[6][6], d[6];
-        int o = 0;
-        for (int r_ = 0; r_ < 6; ++r_)
-          for (int c_ = r_; c_ < 6; ++c_) {
-            H[r_][c_] = Hs[o];
-            H[c_][r_] = Hs[o];
-            ++o;
-          }
-        for (int r_ = 0; r_ < 6; ++r_) {
-          g[r_] = Hs[21 + r_];
-          H[r_][r_] *= 1.0 + 1e-9;
-        }
-        bool okc = true;
-        for (int r_ = 0; r_ < 6 && okc; ++r_)
-          for (int c_ = 0; c_ <= r_; ++c_) {
-            double s = H[r_][c_];
-            for (int k = 0; k < c_; ++k) s -= L[r_][k] * L[c_][k];
-            if (r_ == c_) {
-              if (!(s > 1e-300)) {
-                okc = false;
-                break;
-              }
-              L[r_][r_] = sqrt(s);
-            } else {
-              L[r_][c_] = s / L[c_][c_];
-            }
-          }
+        double d[6];
         double step = 0.0;
+        const bool okc = solve_damped(Hc[buf], lambda, d);
         if (okc) {
-          double yv[6];
-          for (int r_ = 0; r_ < 6; ++r_) {
-            double s = -g[r_];
-            for (int k = 0; k < r_; ++k) s -= L[r_][k] * yv[k];
-            yv[r_] = s / L[r_][r_];
-          }
-          for (int r_ = 5; r_ >= 0; --r_) {
-            double s = yv[r_];
-            for (int k = r_ + 1; k < 6; ++k) s -= L[k][r_] * d[k];
-            d[r_] = s / L[r_][r_];
-          }
-          // R <- exp(w) R (Rodrigues), t <- t + dt
-          const double th = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-          double E[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-          if (th > 1e-16) {
-            const double kx = d[0] / th, ky = d[1] / th, kz = d[2] / th;
-            const double sn = sin(th), cs = 1.0 - cos(th);
-            const double Kx[9] = {0, -kz, ky, kz, 0, -kx, -ky, kx, 0};
-            double K2[9];
-            for (int r_ = 0; r_ < 3; ++r_)
-              for (int c_ = 0; c_ < 3; ++c_)
-                K2[r_ * 3 + c_] = Kx[r_ * 3] * Kx[c_] + Kx[r_ * 3 + 1] * Kx[3 + c_] + Kx[r_ * 3 + 2] * Kx[6 + c_];
-            for (int k = 0; k < 9; ++k) E[k] += sn * Kx[k] + cs * K2[k];
-          }
-          double Rn[9];
-          for (int r_ = 0; r_ < 3; ++r_)
-            for (int c_ = 0; c_ < 3; ++c_)
-              Rn[r_ * 3 + c_] = E[r_ * 3] * best_pose.R[c_] + E[r_ * 3 + 1] * best_pose.R[3 + c_] +
-                                E[r_ * 3 + 2] * best_pose.R[6 + c_];
-          for (int k = 0; k < 9; ++k) best_pose.R[k] = Rn[k];
-          for (int k = 0; k < 3; ++k) best_pose.t[k] += d[3 + k];
+          apply_step(cur, d, best_pose);
           for (int k = 0; k < 6; ++k) step = fmax(step, fabs(d[k]));
         }
         flag = (!okc || step < 1e-12) ? 1 : 0;
       }
       __syncthreads();
-      cur = best_pose;
-      const int stop = flag;
-      __syncthreads();
-      if (stop) break;
+      if (flag) break;
+      const Pose trial = best_pose;
+      cauchy_terms(trial, Hc[buf ^ 1]);
+      const double c_new = Hc[buf ^ 1][27];
+      if (c_new < cost) {   // accept; the normal equations at the new pose are already there
+        const double rel = (cost - c_new) / cost;
+        cur = trial;
+        cost = c_new;
+        buf ^= 1;
+        lambda = fmax(lambda * 0.1, 1e-12);
+        if (rel < 1e-12) break;
+      } else {
+        lambda *= 10.0;
+        if (lambda > 1e12) break;
+      }
+    }
+  } else {
+    // ---------------------------------------------------------------- 3: refinement on the inliers
+    for (int round = 0; round <= refine_rounds; ++round) {
+      // inlier set under the current pose
+      int cnt = 0;
+      for (int i = tid; i < n; i += kPnpThreads) {
+        double p[3], u, v;
+        load_pt(i, p, u, v);
+        const unsigned char in = reproj_err2(cur, cam, p, u, v) < thr2 ? 1 : 0;
+        inl_mask[lo + i] = in;
+        cnt += in;
+      }
+      n_inl = (int)(block_sum((double)cnt, red) + 0.5);
+      if (round == refine_rounds || n_inl < 4) break;
+      __syncthreads();   // inl_mask written by other threads is read below
+      for (int it = 0; it < 10; ++it) {
+        double acc[27];
+  #pragma unroll
+        for (int k = 0; k < 27; ++k) acc[k] = 0.0;
+        for (int i = tid; i < n; i += kPnpThreads) {
+          if (!inl_mask[lo + i]) continue;
+          double p[3], u, v;
+          load_pt(i, p, u, v);
+          const double Y0 = cur.R[0] * p[0] + cur.R[1] * p[1] + cur.R[2] * p[2];
+          const double Y1 = cur.R[3] * p[0] + cur.R[4] * p[1] + cur.R[5] * p[2];
+          const double Y2 = cur.R[6] * p[0] + cur.R[7] * p[1] + cur.R[8] * p[2];
+          const double x = Y0 + cur.t[0], y = Y1 + cur.t[1], z = Y2 + cur.t[2];
+          if (!(z > 1e-9)) continue;
+          const double iz = 1.0 / z, xn = x * iz, yn = y * iz;
+          const double ru = cam.fx * xn + cam.skew * yn + cam.cx - u;
+          const double rv = cam.fy * yn + cam.cy - v;
+          // d(u)/dXc, d(v)/dXc
+          const double gu[3] = {cam.fx * iz, cam.skew * iz, -(cam.fx * xn + cam.skew * yn) * iz};
+          const double gv[3] = {0.0, cam.fy * iz, -cam.fy * yn * iz};
+          // Xc = exp(w) Y + t  ->  dXc/dw = -[Y]x ; J row = (g x ... ) : g^T (-[Y]x) = (Y x g)^T
+          const double Yv[3] = {Y0, Y1, Y2};
+          double ju[6], jv[6];
+          cross3(Yv, gu, ju);
+          cross3(Yv, gv, jv);
+  #pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            ju[3 + k] = gu[k];
+            jv[3 + k] = gv[k];
+          }
+          int o = 0;
+  #pragma unroll
+          for (int r_ = 0; r_ < 6; ++r_) {
+  #pragma unroll
+            for (int c_ = r_; c_ < 6; ++c_) acc[o++] += ju[r_] * ju[c_] + jv[r_] * jv[c_];
+          }
+  #pragma unroll
+          for (int r_ = 0; r_ < 6; ++r_) acc[21 + r_] += ju[r_] * ru + jv[r_] * rv;
+        }
+        for (int k = 0; k < 27; ++k) {
+          const double s = block_sum(acc[k], red);
+          if (tid == 0) Hs[k] = s;
+        }
+        __syncthreads();
+        if (tid == 0) {
+          // solve (H + lambda diag H) d = -g by Cholesky
+          double H[6][6], g[6], L[6][6], d[6];
+          int o = 0;
+          for (int r_ = 0; r_ < 6; ++r_)
+            for (int c_ = r_; c_ < 6; ++c_) {
+              H[r_][c_] = Hs[o];
+              H[c_][r_] = Hs[o];
+              ++o;
+            }
+          for (int r_ = 0; r_ < 6; ++r_) {
+            g[r_] = Hs[21 + r_];
+            H[r_][r_] *= 1.0 + 1e-9;
+          }
+          bool okc = true;
+          for (int r_ = 0; r_ < 6 && okc; ++r_)
+            for (int c_ = 0; c_ <= r_; ++c_) {
+              double s = H[r_][c_];
+              for (int k = 0; k < c_; ++k) s -= L[r_][k] * L[c_][k];
+              if (r_ == c_) {
+                if (!(s > 1e-300)) {
+                  okc = false;
+                  break;
+                }
+                L[r_][r_] = sqrt(s);
+              } else {
+                L[r_][c_] = s / L[c_][c_];
+              }
+            }
+          double step = 0.0;
+          if (okc) {
+            double yv[6];
+            for (int r_ = 0; r_ < 6; ++r_) {
+              double s = -g[r_];
+              for (int k = 0; k < r_; ++k) s -= L[r_][k] * yv[k];
+              yv[r_] = s / L[r_][r_];
+            }
+            for (int r_ = 5; r_ >= 0; --r_) {
+              double s = yv[r_];
+              for (int k = r_ + 1; k < 6; ++k) s -= L[k][r_] * d[k];
+              d[r_] = s / L[r_][r_];
+            }
+            // R <- exp(w) R (Rodrigues), t <- t + dt
+            const double th = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+            double E[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+            if (th > 1e-16) {
+              const double kx = d[0] / th, ky = d[1] / th, kz = d[2] / th;
+              const double sn = sin(th), cs = 1.0 - cos(th);
+              const double Kx[9] = {0, -kz, ky, kz, 0, -kx, -ky, kx, 0};
+              double K2[9];
+              for (int r_ = 0; r_ < 3; ++r_)
+                for (int c_ = 0; c_ < 3; ++c_)
+                  K2[r_ * 3 + c_] = Kx[r_ * 3] * Kx[c_] + Kx[r_ * 3 + 1] * Kx[3 + c_] + Kx[r_ * 3 + 2] * Kx[6 + c_];
+              for (int k = 0; k < 9; ++k) E[k] += sn * Kx[k] + cs * K2[k];
+            }
+            double Rn[9];
+            for (int r_ = 0; r_ < 3; ++r_)
+              for (int c_ = 0; c_ < 3; ++c_)
+                Rn[r_ * 3 + c_] = E[r_ * 3] * best_pose.R[c_] + E[r_ * 3 + 1] * best_pose.R[3 + c_] +
+                                  E[r_ * 3 + 2] * best_pose.R[6 + c_];
+            for (int k = 0; k < 9; ++k) best_pose.R[k] = Rn[k];
+            for (int k = 0; k < 3; ++k) best_pose.t[k] += d[3 + k];
+            for (int k = 0; k < 6; ++k) step = fmax(step, fabs(d[k]));
+          }
+          flag = (!okc || step < 1e-12) ? 1 : 0;
+        }
+        __syncthreads();
+        cur = best_pose;
+        const int stop = flag;
+        __syncthreads();
+        if (stop) break;
+      }
     }
   }
   if (tid < 9) pose[(tid / 3) * 4 + tid % 3] = (float)cur.R[tid];
@@ -522,9 +844,24 @@ extern "C" int opp_pnp_ransac(const float* pts3d, const float* pts2d, const long
   OPP_REQUIRE(m == 0 || (pts3d && pts2d && m_bids && inlier_mask), "null match lists");
   OPP_REQUIRE(batch > 0 && hypotheses > 0 && scale > 0.f && reproj_thr > 0.f && refine_rounds >= 0,
               "bad pnp arguments");
-  OPP_CHECK_CUDA(opp::launch_pdl(pnp_ransac_kernel, dim3(batch), dim3(kPnpThreads), 0, (cudaStream_t)stream, 
-      pts3d, pts2d, m_bids, m, intrinsics, scale, reproj_thr, hypotheses, seed, refine_rounds, poses,
-      n_inliers, inlier_mask, status));
+  OPP_CHECK_CUDA(opp::launch_pdl(pnp_ransac_kernel<PnpSolver::kOpenCv>, dim3(batch), dim3(kPnpThreads), 0,
+      (cudaStream_t)stream, pts3d, pts2d, m_bids, m, intrinsics, scale, reproj_thr, hypotheses, seed,
+      refine_rounds, poses, n_inliers, inlier_mask, status));
+  OPP_CHECK_CUDA(cudaGetLastError());
+  return OPP_OK;
+}
+
+extern "C" int opp_pnp_ransac_colmap(const float* pts3d, const float* pts2d, const long long* m_bids, int m,
+                                     const float* intrinsics, int batch, float max_error_px, int hypotheses,
+                                     unsigned seed, int lo_rounds, float* poses, int* n_inliers,
+                                     unsigned char* inlier_mask, int* status, opp_stream_t stream) {
+  OPP_REQUIRE(intrinsics && poses && n_inliers && status, "null pointer");
+  OPP_REQUIRE(m == 0 || (pts3d && pts2d && m_bids && inlier_mask), "null match lists");
+  OPP_REQUIRE(batch > 0 && hypotheses > 0 && max_error_px > 0.f && lo_rounds >= 0, "bad pnp arguments");
+  // the points are used as given (scale 1): pycolmap's call has no rescale
+  OPP_CHECK_CUDA(opp::launch_pdl(pnp_ransac_kernel<PnpSolver::kColmap>, dim3(batch), dim3(kPnpThreads), 0,
+      (cudaStream_t)stream, pts3d, pts2d, m_bids, m, intrinsics, 1.0f, max_error_px, hypotheses, seed,
+      lo_rounds, poses, n_inliers, inlier_mask, status));
   OPP_CHECK_CUDA(cudaGetLastError());
   return OPP_OK;
 }

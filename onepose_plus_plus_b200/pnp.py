@@ -30,11 +30,23 @@ __all__ = ["ransac_pnp_batched", "pose_metrics_batched", "ransac_PnP", "compute_
 logger = logging.getLogger(__name__)
 
 
+SOLVERS = ("opencv", "colmap")
+
+
 def ransac_pnp_batched(m_bids, mkpts_3d, mkpts_2d, intrinsics, scale=1.0, reprojection_error=5.0,
-                       hypotheses=1024, seed=0, refine_rounds=3):
+                       hypotheses=1024, seed=0, refine_rounds=3, solver="opencv"):
     """m_bids int64 [M] ascending, mkpts_3d fp32 [M, 3], mkpts_2d fp32 [M, 2], intrinsics fp32
     [B, 3, 3] (all CUDA).  Returns a dict of CUDA tensors: pose [B, 3, 4], pose_homo [B, 4, 4],
-    n_inliers int32 [B], inlier_mask bool [M], state bool [B].  No host synchronisation."""
+    n_inliers int32 [B], inlier_mask bool [M], state bool [B].  No host synchronisation.
+
+    solver="opencv" (``opp_pnp_ransac``) is the reference's cv2.solvePnPRansac branch: full K, the
+    points multiplied by ``scale`` and t divided by it.  solver="colmap" (``opp_pnp_ransac_colmap``)
+    is its ``use_pycolmap_ransac`` branch: a SIMPLE_PINHOLE camera (f = K[0, 0]; K[1, 1] is not
+    read), ``scale`` not applied, LO-RANSAC with ``refine_rounds`` local-optimisation rounds, then
+    the pose refined on the RANSAC inliers under the per-point Cauchy loss; inlier_mask and
+    n_inliers are those of the RANSAC model."""
+    if solver not in SOLVERS:
+        raise ValueError(f"solver must be one of {SOLVERS}, got {solver!r}")
     K = intrinsics
     if not K.is_cuda:
         raise RuntimeError("ransac_pnp_batched has no CPU path: pass CUDA tensors")
@@ -53,10 +65,16 @@ def ransac_pnp_batched(m_bids, mkpts_3d, mkpts_2d, intrinsics, scale=1.0, reproj
         n_inl = torch.empty(B, dtype=torch.int32, device=dev)
         status = torch.empty(B, dtype=torch.int32, device=dev)
         mask = torch.empty(max(M, 1), dtype=torch.uint8, device=dev)
-        _lib.call("opp_pnp_ransac", _lib.ptr(p3), _lib.ptr(p2), _lib.ptr(mb), M, _lib.ptr(K32), B,
-                  float(scale), float(reprojection_error), int(hypotheses), ctypes.c_uint(seed & 0xFFFFFFFF),
-                  int(refine_rounds), _lib.ptr(pose), _lib.ptr(n_inl), _lib.ptr(mask), _lib.ptr(status),
-                  _lib.stream())
+        if solver == "colmap":
+            _lib.call("opp_pnp_ransac_colmap", _lib.ptr(p3), _lib.ptr(p2), _lib.ptr(mb), M, _lib.ptr(K32), B,
+                      float(reprojection_error), int(hypotheses), ctypes.c_uint(seed & 0xFFFFFFFF),
+                      int(refine_rounds), _lib.ptr(pose), _lib.ptr(n_inl), _lib.ptr(mask), _lib.ptr(status),
+                      _lib.stream())
+        else:
+            _lib.call("opp_pnp_ransac", _lib.ptr(p3), _lib.ptr(p2), _lib.ptr(mb), M, _lib.ptr(K32), B,
+                      float(scale), float(reprojection_error), int(hypotheses), ctypes.c_uint(seed & 0xFFFFFFFF),
+                      int(refine_rounds), _lib.ptr(pose), _lib.ptr(n_inl), _lib.ptr(mask), _lib.ptr(status),
+                      _lib.stream())
         homo = torch.zeros((B, 4, 4), dtype=torch.float32, device=dev)
         homo[:, :3] = pose
         homo[:, 3, 3] = 1.0
@@ -171,16 +189,29 @@ def _add_metric_models(image_paths, batch, device):
 def ransac_PnP(K, pts_2d, pts_3d, scale=1, pnp_reprojection_error=5, img_hw=None,
                use_pycolmap_ransac=False):
     """Signature and return values of the reference's ``ransac_PnP`` (metric_utils.py:121-204) for
-    one frame, numpy in / numpy out: (pose [3,4], pose_homo [4,4], inlier indices, state)."""
+    one frame, numpy in / numpy out: (pose [3,4], pose_homo [4,4], inlier indices, state).
+
+    ``use_pycolmap_ransac=True`` runs the pycolmap branch (``ransac_pnp_batched(solver="colmap")``):
+    ``img_hw`` must then be a pair, as the reference asserts (it does not change the estimate),
+    ``scale`` is not applied, and the inliers are 1-D int64 indices.  Otherwise the cv2 branch runs
+    and the inliers are ``[n, 1]`` int32 like cv2's.  A frame that fails returns the identity pose
+    and ``state`` False in both modes; pycolmap itself reports ``success: False`` there and the
+    reference then raises ``KeyError`` on ``ret["qvec"]``."""
+    if use_pycolmap_ransac and (img_hw is None or len(img_hw) != 2):
+        raise ValueError(f"use_pycolmap_ransac needs img_hw = (height, width), got {img_hw!r}")
     dev = torch.device("cuda", torch.cuda.current_device())
     p2 = torch.as_tensor(np.ascontiguousarray(pts_2d), dtype=torch.float32, device=dev).reshape(-1, 2)
     p3 = torch.as_tensor(np.ascontiguousarray(pts_3d), dtype=torch.float32, device=dev).reshape(-1, 3)
     Kt = torch.as_tensor(np.asarray(K), dtype=torch.float32, device=dev).reshape(1, 3, 3)
     r = ransac_pnp_batched(torch.zeros(p2.shape[0], dtype=torch.int64, device=dev), p3, p2, Kt, scale=scale,
-                           reprojection_error=pnp_reprojection_error)
+                           reprojection_error=pnp_reprojection_error,
+                           solver="colmap" if use_pycolmap_ransac else "opencv")
     if not bool(r["state"][0].item()):
         return np.eye(4)[:3], np.eye(4), np.array([]).astype(bool), False
-    inliers = torch.nonzero(r["inlier_mask"]).cpu().numpy().astype(np.int32)   # [n, 1] like cv2
+    if use_pycolmap_ransac:
+        inliers = torch.nonzero(r["inlier_mask"])[:, 0].cpu().numpy()   # np.arange(n)[mask] like the reference
+    else:
+        inliers = torch.nonzero(r["inlier_mask"]).cpu().numpy().astype(np.int32)   # [n, 1] like cv2
     return (r["pose"][0].double().cpu().numpy(), r["pose_homo"][0].double().cpu().numpy(), inliers, True)
 
 
@@ -200,7 +231,10 @@ def compute_query_pose_errors(data, configs, training=False):
     """``compute_query_pose_errors`` (metric_utils.py:207-292) with the PnP stage on the device: all
     frames of the batch are solved by one launch, then ONE device->host copy brings back the poses
     and inlier masks.  Writes R_errs, t_errs, inliers, pose_pred (and the empty *_c lists the
-    reference initialises).
+    reference initialises).  ``configs["use_pycolmap_ransac"]`` true selects the pycolmap solver
+    (``solver="colmap"``, see ``ransac_pnp_batched``; ``point_cloud_rescale`` is then not applied and
+    ``inliers`` holds 1-D index arrays); ``q_hw_i`` / ``query_image_scale``, which the reference
+    reads only to build pycolmap's image size, are not needed.
 
     With ``configs["eval_ADD_metric"]`` true and ``training`` false (the LINEMOD evaluation), also
     writes ``data["ADD"]`` (one bool per frame: ADD, or ADD-S for the symmetric objects 0810 / 0811,
@@ -215,9 +249,11 @@ def compute_query_pose_errors(data, configs, training=False):
     unit = configs["model_unit"] if "model_unit" in configs else "m"
     K = data["query_intrinsic"]
     dev = data["m_bids"].device
+    colmap = bool(configs.get("use_pycolmap_ransac", False))
+    kw = {"solver": "colmap"} if colmap else {}
     r = ransac_pnp_batched(data["m_bids"], data["mkpts_3d_db"], data["mkpts_query_f"], K.to(dev),
                            scale=configs.get("point_cloud_rescale", 1.0),
-                           reprojection_error=configs["pnp_reprojection_error"])
+                           reprojection_error=configs["pnp_reprojection_error"], **kw)
     metrics = None
     if "eval_ADD_metric" in configs and configs["eval_ADD_metric"] and not training:
         models = _add_metric_models(data["query_image_path"], K.shape[0], dev)
@@ -249,5 +285,6 @@ def compute_query_pose_errors(data, configs, training=False):
         R_err, t_err = query_pose_error(poses[b][:3], gt[b], unit=unit)
         data["R_errs"].append(R_err)
         data["t_errs"].append(t_err)
-        data["inliers"].append(np.nonzero(mask[m_bids == b])[0][:, None].astype(np.int32))
+        idx = np.nonzero(mask[m_bids == b])[0]
+        data["inliers"].append(idx if colmap else idx[:, None].astype(np.int32))
     data["pose_pred"] = poses
