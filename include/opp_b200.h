@@ -393,6 +393,36 @@ int opp_pose_metrics(const float* verts, int num_verts, const float* pose_pred, 
  * is not positive). */
 long long opp_pose_metrics_scratch_bytes(int num_verts, int batch);
 
+/* ------------------------------------------------------------------------------------------
+ * Tracking front end — LocalFeatureObjectDetector.crop_img_by_bbox / previous_pose_detect
+ * (src/local_feature_object_detector/local_feature_2D_detector.py:133-159, 200-226: two
+ * cv2.warpAffine(INTER_LINEAR) calls of data_utils.get_image_crop_resize :239-255 per frame)
+ * ---------------------------------------------------------------------------------------- */
+
+/* Per-frame parameters of opp_crop_resize_u8 (64 bytes, 8-byte aligned):
+ *   m: the INVERSE of the forward affine matrix of the warp, as cv2.warpAffine inverts it (fp64,
+ *      row-major 2x3: src = m * (x, y, 1));
+ *   (x0, y0, w, h): the virtual source — pixel (u, v) of the source is frame[v + y0][u + x0] for
+ *      0 <= u < w, 0 <= v < h and inside the frame, else 0. */
+typedef struct opp_crop_params {
+  double m[6];
+  int x0, y0, w, h;
+} opp_crop_params;
+
+/* cv2.warpAffine(src, M, (out_w, out_h), flags=INTER_LINEAR) of uint8 single-channel images, bit for
+ * bit (cv2's fixed-point coordinates and 2^15-scaled bilinear weights, BORDER_CONSTANT 0), with src =
+ * the virtual source of params[b].  For the two warps of crop_img_by_bbox, (x0, y0, w, h) is the box
+ * and m is the inverse of the second (resize) warp: the first warp is the integer shift the virtual
+ * source applies.  For one plain warp of the frame, (x0, y0, w, h) = (0, 0, width, height).
+ *   frames uint8 [batch][height][width]; params [batch]; out uint8 [batch][out_h][out_w];
+ *   status int32 [batch] or NULL: 0 = ok, 1 = w or h < 1 (cv2 raises), 2 = w or h >= 32767 (cv2
+ *   raises) or a box coordinate with |.| >= 2^20 (outside the int32 fixed-point range); the crop of
+ *   such a frame is written as zeros.  The params live on the device (so that the call can be
+ *   captured in a CUDA graph): they are checked there, not on the host. */
+int opp_crop_resize_u8(const unsigned char* frames, int batch, int height, int width,
+                       const opp_crop_params* params, unsigned char* out, int out_h, int out_w, int* status,
+                       opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

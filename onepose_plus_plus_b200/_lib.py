@@ -58,6 +58,7 @@ SIGNATURES = {
     "opp_pnp_ransac": [P, P, P, I, P, I, F, F, I, ctypes.c_uint, I, P, P, P, P, P],
     "opp_pnp_ransac_colmap": [P, P, P, I, P, I, F, I, ctypes.c_uint, I, P, P, P, P, P],
     "opp_pose_metrics": [P, I, P, P, P, P, I, P, L, P, P, P],
+    "opp_crop_resize_u8": [P, I, I, I, P, P, I, I, P, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),

@@ -1000,7 +1000,16 @@ class OnePosePlus_model(_Engine):
             # kernels implement the inference forward only) — see train_path.py
             from . import train_path
             return train_path.forward_train(self, data)
+        return self._forward(data)
+
+    def _forward(self, data, prologue=None):
+        """forward(data); `prologue` (tracking.py) produces query_image on the device first: its
+        `inputs` (tensors, host or device) are copied to the device and `run(inputs, query_image)`
+        enqueues the kernels that write the image — in CUDA-graph mode inside the same graph, with
+        `key` added to the graph's signature."""
         img, img_scale, bank_raw = self._check_inputs(data)
+        if prologue is not None and (img.dtype != torch.uint8 or not img.is_contiguous()):
+            raise ValueError("a prologue writes query_image in place: it must be a contiguous uint8 tensor")
         qmask = data.get("query_image_mask")
         if qmask is not None:
             # OnePosePlusModel.py:158: mask at coarse resolution, flattened to [B, S]; nonzero = valid
@@ -1030,8 +1039,10 @@ class OnePosePlus_model(_Engine):
             if self.use_cuda_graphs:
                 if qmask is not None:
                     raise NotImplementedError("query_image_mask is not supported in CUDA-graph mode")
-                out, M = self._replay(img, img_scale, bank_raw, fine_on)
+                out, M = self._replay(img, img_scale, bank_raw, fine_on, prologue)
             else:
+                if prologue is not None:
+                    prologue.run([t.to(dev) for t in prologue.inputs], img)
                 out, count, cap = self._enqueue(img, img_scale, bank_raw, fine_on, dynamic=False, qmask=qmask)
                 M = out.pop("M")
             self._publish(data, out, M, dev, fine_on)
@@ -1134,7 +1145,7 @@ class OnePosePlus_model(_Engine):
             self._graphs = {}
         return self
 
-    def _replay(self, img, img_scale, bank_raw, fine_on):
+    def _replay(self, img, img_scale, bank_raw, fine_on, prologue=None):
         resident = bank_raw is None
         if resident:
             bkey = ("resident", id(self._bank))
@@ -1145,6 +1156,8 @@ class OnePosePlus_model(_Engine):
             bkey = tuple((tuple(t.shape), t.dtype) for t in bank_raw)
         key = (tuple(img.shape), img.dtype, img_scale is not None, bkey, fine_on, self.conf_matrix_mode,
                self.coarse_colmax, self.coarse_lse_cols, self.kv_single_plane, self.fine_windows)
+        if prologue is not None:
+            key = key + (prologue.key,)
         ent = self._graphs.get(key)
         if ent is not None and ent["ws_epoch"] != self._ws_epoch:
             ent = None            # a workspace buffer was re-allocated: the captured pointers are stale
@@ -1154,9 +1167,15 @@ class OnePosePlus_model(_Engine):
             s_img = torch.empty_like(img)
             s_scale = torch.empty_like(img_scale) if img_scale is not None else None
             s_bank = None if resident else tuple(torch.empty_like(t.contiguous()) for t in bank_raw)
+            s_pro = None if prologue is None else [torch.empty(t.shape, dtype=t.dtype, device=img.device)
+                                                   for t in prologue.inputs]
 
             def load():
-                s_img.copy_(img)
+                if s_pro is None:
+                    s_img.copy_(img)
+                else:
+                    for d, t in zip(s_pro, prologue.inputs):
+                        d.copy_(t)
                 if s_scale is not None:
                     s_scale.copy_(img_scale)
                 if s_bank is not None:
@@ -1164,25 +1183,35 @@ class OnePosePlus_model(_Engine):
                         d.copy_(t)
             load()
             # warm-up outside the capture: sizes the workspace, sets kernel attributes
+            if s_pro is not None:
+                prologue.run(s_pro, s_img)
             self._enqueue(s_img, s_scale, s_bank, fine_on, dynamic=True)
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             count_host = torch.empty(1, dtype=torch.int32, pin_memory=True)
             with torch.cuda.graph(g):
+                if s_pro is not None:
+                    prologue.run(s_pro, s_img)   # first node: query_image from the prologue's inputs
                 out, count, cap = self._enqueue(s_img, s_scale, s_bank, fine_on, dynamic=True)
                 count_host.copy_(count, non_blocking=True)   # last node of the graph: M lands in pinned memory
             out["gt_mask"].zero_()
             ent = {"graph": g, "out": out, "count": count_host, "ws_epoch": self._ws_epoch,
-                   "inputs": (s_img, s_scale, s_bank)}
+                   "inputs": (s_img, s_scale, s_bank, s_pro)}
             self._graphs[key] = ent
-        s_img, s_scale, s_bank = ent["inputs"]
-        s_img.copy_(img)
+        s_img, s_scale, s_bank, s_pro = ent["inputs"]
+        if s_pro is None:
+            s_img.copy_(img)
+        else:
+            for d, t in zip(s_pro, prologue.inputs):
+                d.copy_(t)
         if s_scale is not None:
             s_scale.copy_(img_scale)
         if s_bank is not None:
             for d, t in zip(s_bank, bank_raw):
                 d.copy_(t)
         ent["graph"].replay()
+        if s_pro is not None:
+            img.copy_(s_img)   # the caller's query_image receives what the prologue wrote
         src = ent["out"]
         torch.cuda.current_stream().synchronize()        # the only host sync, after everything is queued
         M = min(int(ent["count"][0]), src["fcap"])
