@@ -423,6 +423,48 @@ int opp_crop_resize_u8(const unsigned char* frames, int batch, int height, int w
                        const opp_crop_params* params, unsigned char* out, int out_h, int out_w, int* status,
                        opp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training, coarse level — Loss.compute_coarse_loss, focal branch (src/lightning_model/
+ * losses.py:18-58) on the dual-softmax confidence, forward and backward, without the [B, L, S]
+ * matrix (opp_train.cu has the formulas).
+ * ---------------------------------------------------------------------------------------- */
+
+/* Row blocks (CTAs per batch element) of both calls below for `rows` 3D points. */
+int opp_coarse_focal_blocks(int rows);
+
+/* Softmax statistics of sim = scale * a b^T, computed from the same fp32 sim the two calls below
+ * recompute (one statistics pass + an in-order merge of the column partials).
+ *   a fp32 [B][rows][k], b fp32 [B][cols][k] (k = 256); col_mask uint8 [B][cols] or NULL (masked
+ *   columns drop out of every row's softmax).  part_c fp32 [B][opp_coarse_focal_blocks(rows)][cols][2]
+ *   workspace.  st_rows fp32 [B][rows][2], st_cols fp32 [B][cols][2]: (m, log s) with m = max of sim
+ *   and s = sum exp(sim - m) over the row / column, so logsumexp = m + log s. */
+int opp_coarse_focal_stats(const float* a, const float* b, const unsigned char* col_mask, int batches, int rows,
+                           int cols, int k, float scale, float* part_c, float* st_rows, float* st_cols,
+                           opp_stream_t stream);
+
+/* Loss and the backward's per-row / per-column sums.
+ *   a, b, col_mask as above; st_rows / st_cols from opp_coarse_focal_stats on the same a, b;
+ *   gt [B][rows][cols], gt_bytes 1 (bool / uint8) or 2 (int16): 1 positive, 0 negative, anything
+ *   else neither.
+ *   Workspace (nb = opp_coarse_focal_blocks(rows)): part_loss fp64 [B*nb][2], part_cnt int64
+ *   [B*nb][2], part_r fp64 [B][rows][2], part_c fp64 [B][nb][cols][2].
+ *   Outputs: loss fp32 [1]; counts int64 [2] = (npos, nneg); wts fp32 [2] = (pos_w / npos,
+ *   neg_w / nneg), 0 for an empty class; r fp64 [B][rows], c fp64 [B][cols] = the weighted sums of
+ *   c dloss/dc over each row / column.  Deterministic (fixed-order sums, no atomics). */
+int opp_coarse_focal_fwd(const float* a, const float* b, const float* st_rows, const float* st_cols,
+                         const void* gt, int gt_bytes, const unsigned char* col_mask, int batches, int rows,
+                         int cols, int k, float scale, float alpha, float gamma, float pos_w, float neg_w,
+                         double* part_loss, long long* part_cnt, double* part_r, double* part_c, float* loss,
+                         long long* counts, float* wts, double* r, double* c, opp_stream_t stream);
+
+/* d loss / d a and d loss / d b times grad[0] (a device scalar: no host synchronisation), from the
+ * statistics and r / c / wts of opp_coarse_focal_fwd.  da fp32 [B][rows][k], db fp32 [B][cols][k]
+ * (overwritten).  Deterministic. */
+int opp_coarse_focal_bwd(const float* a, const float* b, const float* st_rows, const float* st_cols,
+                         const double* r, const double* c, const float* wts, const float* grad, const void* gt,
+                         int gt_bytes, const unsigned char* col_mask, int batches, int rows, int cols, int k,
+                         float scale, float alpha, float gamma, float* da, float* db, opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

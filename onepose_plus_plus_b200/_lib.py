@@ -59,11 +59,15 @@ SIGNATURES = {
     "opp_pnp_ransac_colmap": [P, P, P, I, P, I, F, I, ctypes.c_uint, I, P, P, P, P, P],
     "opp_pose_metrics": [P, I, P, P, P, P, I, P, L, P, P, P],
     "opp_crop_resize_u8": [P, I, I, I, P, P, I, I, P, P],
+    "opp_coarse_focal_stats": [P, P, P, I, I, I, I, F, P, P, P, P],
+    "opp_coarse_focal_fwd": [P, P, P, P, P, I, P, I, I, I, I, F, F, F, F, F] + [P] * 10,
+    "opp_coarse_focal_bwd": [P] * 9 + [I, P, I, I, I, I, F, F, F, P, P, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),
          "opp_kv_chunks_b": ([I, I], c_int),
          "opp_conv_win_pitch": ([I], c_int),
+         "opp_coarse_focal_blocks": ([I], c_int),
          "opp_pose_metrics_scratch_bytes": ([I, I], c_longlong),
          "opp_last_error": ([], ctypes.c_char_p)}
 
@@ -100,7 +104,8 @@ def stream():
 
 
 # kernels launched per entry point (bench.py reports the per-step total as gpu_launches)
-KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_pose_metrics": 3}
+KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_pose_metrics": 3,
+                    "opp_coarse_focal_stats": 2, "opp_coarse_focal_fwd": 3, "opp_coarse_focal_bwd": 2}
 LAUNCHES = 0
 _PROFILE = None
 

@@ -220,6 +220,77 @@ def match_select(pt_val, pt_idx, px_idx, kpts, img_scale, batch, l, hc, wc, thr,
          ptr(i_ids), ptr(j_ids), ptr(mconf), ptr(mkpts3d), ptr(mkpts_c), ptr(count), int(bank_shared), stream())
 
 
+GT_BYTES = {torch.bool: 1, torch.uint8: 1, torch.int16: 2}
+
+
+def _gt_bytes(gt):
+    if gt.dtype not in GT_BYTES:
+        raise TypeError(f"conf_matrix_gt: expected bool, uint8 or int16, got {gt.dtype}")
+    _chk(gt, gt.dtype, "conf_matrix_gt")
+    return GT_BYTES[gt.dtype]
+
+
+def coarse_focal_stats(a, b, col_mask, scale):
+    """Softmax statistics of sim = scale * a b^T over each row / column, from the same fp32 sim the
+    focal kernels recompute: (st_rows [B,L,2], st_cols [B,S,2]) = (max, log sum exp(sim - max))."""
+    _chk(a, torch.float32, "feat3d")
+    _chk(b, torch.float32, "feat2d")
+    _chk(col_mask, torch.uint8, "col_mask")
+    B, L, K = a.shape
+    S = b.shape[1]
+    nb = _lib.load().opp_coarse_focal_blocks(L)
+    dev, f32 = a.device, torch.float32
+    part_c = torch.empty(B, nb, S, 2, dtype=f32, device=dev)
+    st_rows = torch.empty(B, L, 2, dtype=f32, device=dev)
+    st_cols = torch.empty(B, S, 2, dtype=f32, device=dev)
+    call("opp_coarse_focal_stats", ptr(a), ptr(b), ptr(col_mask), B, L, S, K, float(scale), ptr(part_c),
+         ptr(st_rows), ptr(st_cols), stream())
+    return st_rows, st_cols
+
+
+def coarse_focal_fwd(a, b, st_rows, st_cols, gt, col_mask, scale, alpha, gamma, pos_w, neg_w):
+    """Focal loss of the dual-softmax confidence (losses.py:18-58) from fp32 features a [B,L,256],
+    b [B,S,256] and their coarse_focal_stats (st_rows, st_cols); returns (loss [1], counts int64
+    [2] = (npos, nneg), wts [2], r [B,L], c [B,S]) — the last three are what coarse_focal_bwd reads."""
+    _chk(a, torch.float32, "feat3d")
+    _chk(b, torch.float32, "feat2d")
+    _chk(col_mask, torch.uint8, "col_mask")
+    gb = _gt_bytes(gt)
+    B, L, K = a.shape
+    S = b.shape[1]
+    nb = _lib.load().opp_coarse_focal_blocks(L)
+    dev, f32 = a.device, torch.float32
+    part_loss = torch.empty(B * nb, 2, dtype=torch.float64, device=dev)
+    part_cnt = torch.empty(B * nb, 2, dtype=torch.int64, device=dev)
+    part_r = torch.empty(B, L, 2, dtype=torch.float64, device=dev)
+    part_c = torch.empty(B, nb, S, 2, dtype=torch.float64, device=dev)
+    loss = torch.empty((), dtype=f32, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    wts = torch.empty(2, dtype=f32, device=dev)
+    r = torch.empty(B, L, dtype=torch.float64, device=dev)
+    c = torch.empty(B, S, dtype=torch.float64, device=dev)
+    call("opp_coarse_focal_fwd", ptr(a), ptr(b), ptr(st_rows), ptr(st_cols), ptr(gt), gb, ptr(col_mask), B, L,
+         S, K, float(scale), float(alpha), float(gamma), float(pos_w), float(neg_w), ptr(part_loss),
+         ptr(part_cnt), ptr(part_r), ptr(part_c), ptr(loss), ptr(counts), ptr(wts), ptr(r), ptr(c), stream())
+    return loss, counts, wts, r, c
+
+
+def coarse_focal_bwd(a, b, st_rows, st_cols, r, c, wts, grad, gt, col_mask, scale, alpha, gamma):
+    """(d loss / d a, d loss / d b) * grad, grad a device scalar."""
+    _chk(a, torch.float32, "feat3d")
+    _chk(b, torch.float32, "feat2d")
+    _chk(grad, torch.float32, "grad")
+    _chk(col_mask, torch.uint8, "col_mask")
+    gb = _gt_bytes(gt)
+    B, L, K = a.shape
+    S = b.shape[1]
+    da, db = torch.empty_like(a), torch.empty_like(b)
+    call("opp_coarse_focal_bwd", ptr(a), ptr(b), ptr(st_rows), ptr(st_cols), ptr(r), ptr(c), ptr(wts), ptr(grad),
+         ptr(gt), gb, ptr(col_mask), B, L, S, K, float(scale), float(alpha), float(gamma), ptr(da), ptr(db),
+         stream())
+    return da, db
+
+
 def fine_gather(fine, desc3d, b_ids, i_ids, j_ids, x32, x16, m, hf, wf, wc, stride, n, split,
                 bank_shared=False, count=None, windows=False):
     """windows: `fine` is the compact [m, 5, 8, planes*128] window tensor of conv_win."""

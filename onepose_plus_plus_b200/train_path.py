@@ -10,7 +10,11 @@ the same parameters (the module tree of model.py holds ordinary nn.Conv2d / Batc
 LayerNorm modules with the reference's names), evaluated with library PyTorch ops in the
 reference's order, BatchNorm in batch-statistics mode exactly as ``nn.Module.train()`` leaves it.
 This is the slow path by construction (SURVEY §8 f4 "keep the PyTorch path for self.training");
-``.eval()`` always runs the CUDA kernels and never falls back to this module.
+``.eval()`` always runs the CUDA kernels and never falls back to this module.  The one exception is
+the coarse supervision: with ``model.conf_matrix_mode == "lazy"`` on CUDA tensors the L x S
+confidence matrix is not built — the statistics and the match selection run on the inference
+kernels and ``data["conf_matrix"]`` is a TrainConfHandle that ``losses.Loss`` differentiates with
+the opp_coarse_focal kernels (DESIGN §7 f4).
 
 Every function cites the reference lines it follows.
 """
@@ -106,7 +110,6 @@ def _coarse_matches(cm, conf, data, training):
     """CoarseMatching.get_coarse_match (utils/coarse_matching.py:125-242) including the training
     branch: a random subset of the predictions padded with ground-truth matches (:177-217)."""
     hc, wc = data["q_hw_c"]
-    dev = conf.device
     B, L, S = conf.shape
     mask = (conf > cm.thr).view(B, L, hc, wc).clone()
     if cm.border_rm > 0:     # mask_border (:10-20): the `-b:0` slices are empty, only top/left are cleared
@@ -118,6 +121,15 @@ def _coarse_matches(cm, conf, data, training):
     b_ids, i_ids = torch.where(mask_v)
     j_ids = all_j[b_ids, i_ids]
     mconf = conf[b_ids, i_ids, j_ids]
+    return _pad_matches(cm, b_ids, i_ids, j_ids, mconf, (B, L, S), data, training)
+
+
+@torch.no_grad()
+def _pad_matches(cm, b_ids, i_ids, j_ids, mconf, shape, data, training):
+    """get_coarse_match from the predicted matches on: training padding (:177-217), coordinates."""
+    hc, wc = data["q_hw_c"]
+    dev = b_ids.device
+    B, L, S = shape
     tcfg = cm.config["train"]
     if training and tcfg["train_padding"]:
         n_max = int(B * min(L, S) * tcfg["train_coarse_percent"])
@@ -143,17 +155,103 @@ def _coarse_matches(cm, conf, data, training):
             "mconf": mconf[keep]}
 
 
-def coarse_matching(cm, feat3d, feat2d, data, mask_query, training):
-    """CoarseMatching.forward (utils/coarse_matching.py:76-123)"""
+def dual_softmax(cm, feat3d, feat2d, mask_query):
+    """conf_matrix of CoarseMatching.forward (utils/coarse_matching.py:96-119), with autograd"""
     c = feat3d.shape[-1]
     sim = torch.einsum("nlc,nsc->nls", feat3d / c ** 0.5, feat2d / c ** 0.5) / (cm.temperature + 1e-4)
     if mask_query is not None:
         neg = torch.zeros_like(sim)
         neg[~mask_query.bool()[:, None].expand_as(sim)] = -1e9
         sim = sim + neg
-    conf = F.softmax(sim, 1) * F.softmax(sim, 2)
-    data["conf_matrix"] = conf
-    data.update(_coarse_matches(cm, conf, data, training))
+    return F.softmax(sim, 1) * F.softmax(sim, 2)
+
+
+def coarse_matching(cm, feat3d, feat2d, data, mask_query, training, lazy_split=None):
+    """CoarseMatching.forward (utils/coarse_matching.py:76-123).  lazy_split (CUDA, the model's
+    conf_matrix_mode "lazy"): the matrix is not built; data["conf_matrix"] is a TrainConfHandle and
+    the matches come from the inference kernels (split = the model's fp16x3 operand mode)."""
+    if lazy_split is None:
+        conf = dual_softmax(cm, feat3d, feat2d, mask_query)
+        data["conf_matrix"] = conf
+        data.update(_coarse_matches(cm, conf, data, training))
+        return
+    handle, b_ids, i_ids, j_ids, mconf = _lazy_coarse(cm, feat3d, feat2d, data, mask_query, lazy_split)
+    data["conf_matrix"] = handle
+    data.update(_pad_matches(cm, b_ids, i_ids, j_ids, mconf, tuple(handle.shape), data, training))
+
+
+class TrainConfHandle:
+    """data["conf_matrix"] in training with conf_matrix_mode "lazy": the autograd-connected features
+    and the softmax statistics of their fp32 sim (opp_coarse_focal_stats — the same sim the loss
+    kernels recompute), instead of the [B, L, S] matrix.  onepose_plus_plus_b200.losses.Loss
+    evaluates the coarse loss and its backward from it.
+      .shape        torch.Size([B, L, S])
+      .max()        max of the matrix (detached 0-d tensor, from the selection pass's row maxima)
+      .materialize() the matrix the eager mode writes, with autograd (same formula)."""
+
+    def __init__(self, cm, feat3d, feat2d, mask_query, rowmax=None):
+        from . import ops
+        B, L, C = feat3d.shape
+        S = feat2d.shape[1]
+        self.cm, self.feat3d, self.feat2d, self.mask_query = cm, feat3d, feat2d, mask_query
+        self.scale = 1.0 / (C * (cm.temperature + 1e-4))    # (a / sqrt(C)) . (b / sqrt(C)) / (T + 1e-4)
+        self.shape = torch.Size((B, L, S))
+        with torch.no_grad():
+            self.a32 = feat3d.detach().float().contiguous()
+            self.b32 = feat2d.detach().float().contiguous()
+            self.col_mask = (mask_query != 0).to(torch.uint8).reshape(B, S).contiguous() \
+                if mask_query is not None else None
+            self.st_rows, self.st_cols = ops.coarse_focal_stats(self.a32, self.b32, self.col_mask, self.scale)
+        self._rowmax = rowmax
+
+    def max(self):
+        if self._rowmax is None:
+            raise RuntimeError("this handle was built without the selection pass's row maxima")
+        return self._rowmax.max()
+
+    def materialize(self):
+        return dual_softmax(self.cm, self.feat3d, self.feat2d, self.mask_query)
+
+
+@torch.no_grad()
+def _lazy_coarse(cm, feat3d, feat2d, data, mask_query, split):
+    """Match selection with the inference kernels (opp_sim_lse_cols + finalisers on fp16 hi/lo planes,
+    opp_sim_conf_colmax, opp_match_select_colmax): threshold, top/left border, mutual nearest
+    neighbour by value, matches in (b, l) order, mconf = the row maxima.  The loss statistics of the
+    handle are computed separately, from the fp32 features (TrainConfHandle)."""
+    from . import ops
+    B, L, C = feat3d.shape
+    S = feat2d.shape[1]
+    hc, wc = data["q_hw_c"]
+    dev, f32, i32, i64 = feat3d.device, torch.float32, torch.int32, torch.int64
+    scale = 1.0 / (C * (cm.temperature + 1e-4))
+    a16, b16 = ops.to_planes(feat3d.detach().float(), split), ops.to_planes(feat2d.detach().float(), split)
+    col_mask = (mask_query != 0).to(torch.uint8).reshape(B, S).contiguous() if mask_query is not None else None
+    ts, groups = ops.sim_tiles(S), (L + 31) // 32
+    pm, ps = torch.empty(B * L, ts, dtype=f32, device=dev), torch.empty(B * L, ts, dtype=f32, device=dev)
+    lse_rows, lse_cols = torch.empty(B, L, dtype=f32, device=dev), torch.empty(B, S, dtype=f32, device=dev)
+    col_m, col_s = (torch.empty(B, groups, S, dtype=f32, device=dev) for _ in range(2))
+    ops.sim_lse_cols(a16, b16, B, L, S, C, scale, pm, ps, lse_rows, col_m, col_s, lse_cols, split,
+                     col_mask=col_mask)
+    del col_m, col_s, ps
+    pi = torch.empty(B * L, ts, dtype=i32, device=dev)
+    rowmax, rowarg = torch.empty(B, L, dtype=f32, device=dev), torch.empty(B, L, dtype=i32, device=dev)
+    colmax = torch.empty(B, S, dtype=i32, device=dev)
+    ops.sim_conf_colmax(a16, b16, lse_rows, lse_cols, None, B, L, S, C, scale, pm, pi, rowmax, rowarg, colmax,
+                        split)
+    del a16, b16, pm, pi
+    cap = B * L
+    ids = [torch.empty(cap, dtype=i64, device=dev) for _ in range(3)]
+    mconf = torch.empty(cap, dtype=f32, device=dev)
+    count = torch.empty(1, dtype=i32, device=dev)
+    ops.match_select_colmax(rowmax, rowarg, colmax, data["keypoints3d"].detach().float().contiguous(), None, B, L,
+                            hc, wc, cm.thr, cm.border_rm, 1.0,
+                            torch.empty((cap + 1023) // 1024 + 2, dtype=i32, device=dev), *ids, mconf,
+                            torch.empty(cap, 3, dtype=f32, device=dev), torch.empty(cap, 2, dtype=f32, device=dev),
+                            count)
+    n = int(count.item())
+    handle = TrainConfHandle(cm, feat3d, feat2d, mask_query, rowmax)
+    return (handle, *(t[:n] for t in ids), mconf[:n])
 
 
 def fine_preprocess(W, d_model, data, desc3d_db, feat_f):
@@ -195,9 +293,18 @@ def fine_matching(feat3d, feat2d, data, training):
 def forward_train(model, data):
     """OnePosePlus_model.forward (OnePosePlusModel.py:96-201) with autograd, module in train mode."""
     cfg = model.config
+    mode = model.conf_matrix_mode
+    if mode == "skip":
+        raise ValueError('conf_matrix_mode "skip" cannot train: the coarse loss reads data["conf_matrix"] '
+                         '(use "lazy" for the matrix-free handle)')
     if model.loftr_backbone_pretrained and cfg["loftr_backbone"]["pretrained_fix"]:
         model.backbone.eval()                                      # OnePosePlusModel.py:109-113
     img = data["query_image"]
+    lazy_split = model.split if mode == "lazy" and img.is_cuda else None
+    if lazy_split is False:
+        # single fp16 operands would select matches from a sim that differs from the eager fp32 one
+        raise ValueError('conf_matrix_mode "lazy" in train mode needs precision "fp16x3" (the match '
+                         'selection runs on the fp32-grade split operands)')
     data.update({"bs": img.size(0), "q_hw_i": img.shape[2:]})
     feat_c, feat_f = backbone(model.backbone, img)
     data.update({"q_hw_c": feat_c.shape[2:], "q_hw_f": feat_f.shape[2:]})
@@ -208,7 +315,7 @@ def forward_train(model, data):
     d3 = keypoint_encoding(model.kpt_3d_pos_encoding, normalize_3d_keypoints(data["keypoints3d"]), dsel)
     qmask = data["query_image_mask"].flatten(-2) if "query_image_mask" in data else None
     d3, q_c = transformer(model.loftr_coarse, d3, q_c, qmask)
-    coarse_matching(model.coarse_matching, d3, q_c, data, qmask, model.training)
+    coarse_matching(model.coarse_matching, d3, q_c, data, qmask, model.training, lazy_split)
     if not cfg["fine_matching"]["enable"]:
         data.update({"mkpts_query_f": data["mkpts_query_c"]})
         return

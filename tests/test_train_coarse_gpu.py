@@ -1,0 +1,179 @@
+"""The coarse training loss on the device (opp_coarse_focal_fwd / _bwd through losses.Loss) against
+the fp64 oracle (oracle/coarse_loss.py), the stored reference numbers, and the eager training path
+end to end."""
+import os
+import types
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import coarse_loss as cl
+from oracle import make_reference_golden as mrg
+from oracle import workload
+from onepose_plus_plus_b200 import OnePosePlus_model, losses, train_path
+from tests import golden_io
+
+pytestmark = pytest.mark.gpu
+RTOL = 2e-4
+
+
+def _fused(a, b, gt, mask):
+    a = a.cuda().requires_grad_(True)
+    b = b.cuda().requires_grad_(True)
+    mask = mask.cuda() if mask is not None else None
+    h = train_path.TrainConfHandle(types.SimpleNamespace(temperature=cl.TEMPERATURE), a, b, mask)
+    loss, counts = losses.coarse_focal_loss(h, gt.cuda(), 0.5, 2.0, 1.0, 1.0)
+    loss.backward()
+    return loss.detach(), a.grad, b.grad, counts
+
+
+def _close(got, ref, absmax=None):
+    absmax = float(ref.abs().max()) if absmax is None else absmax
+    got, ref = got.double().cpu(), torch.as_tensor(ref).double().cpu()
+    err = (got - ref).abs()
+    tol = RTOL * ref.abs() + 1e-6 + RTOL * absmax
+    assert bool((err <= tol).all()), f"max err {float(err.max()):.3e}, max err/tol {float((err / tol).max()):.3f}"
+    return float((err / (ref.abs() + absmax)).max())
+
+
+@pytest.mark.parametrize("key", list(cl.GOLDEN_CASES))
+def test_kernels_match_oracle_and_reference(key):
+    name, batch, rows, cols = cl.GOLDEN_CASES[key]
+    a, b, gt, mask = cl.make_case(name, batch, rows, cols)
+    loss, da, db, counts = _fused(a, b, gt, mask)
+    r_loss, r_da, r_db = cl.focal_loss_and_grads(a.cuda(), b.cuda(), gt.cuda(), cl.scale_of(),
+                                                 mask.cuda() if mask is not None else None)
+    assert counts.tolist() == [int((gt == 1).sum()), int((gt == 0).sum())]
+    assert abs(loss.item() - r_loss.item()) <= RTOL * abs(r_loss.item())
+    _close(da, r_da)
+    _close(db, r_db)
+    z = np.load(os.path.join(golden_io.GOLDEN_DIR, "reference", "coarse_loss.npz"))
+    assert abs(loss.item() - float(z[key + "_loss"])) <= RTOL * abs(float(z[key + "_loss"]))
+    for nm, t in (("_da", da), ("_db", db)):
+        got = t.flatten().cpu()[torch.from_numpy(z[key + nm + "_idx"])]
+        _close(got, torch.from_numpy(z[key + nm]), float(z[key + nm + "_absmax"]))
+    # deterministic: a second call gives the same bits
+    loss2, da2, db2, _ = _fused(a, b, gt, mask)
+    assert torch.equal(loss, loss2) and torch.equal(da, da2) and torch.equal(db, db2)
+
+
+@pytest.mark.parametrize("name", ["random", "no_pos", "no_neg"])
+def test_kernels_gt_dtypes_and_empty_classes(name):
+    a, b, gt, mask = cl.make_case(name, 2, 70, 90)
+    outs = []
+    dtypes = [torch.uint8, torch.int16] + ([torch.bool] if name == "no_pos" else [])
+    for dt in dtypes:
+        outs.append(_fused(a, b, gt.to(dt), mask))
+    for o in outs[1:]:
+        assert all(torch.equal(x, y) for x, y in zip(o[:3], outs[0][:3]))
+    loss, da, db, _ = outs[0]
+    r_loss, r_da, r_db = cl.focal_loss_and_grads(a.cuda(), b.cuda(), gt.cuda(), cl.scale_of())
+    assert abs(loss.item() - r_loss.item()) <= RTOL * abs(r_loss.item())
+    _close(da, r_da)
+    _close(db, r_db)
+    with pytest.raises(TypeError):
+        _fused(a, b, gt.float(), mask)
+    neither = _fused(a, b, torch.full_like(gt, 2), mask)[0]
+    assert torch.isnan(neither)
+
+
+def _train_shape_case():
+    a, b, gt, _ = cl.make_case("planted", 4, 7000, 4096, seed=1)
+    gt[torch.rand(gt.shape, generator=torch.Generator().manual_seed(2)) < 2e-4] = 1
+    return a, b, gt
+
+
+def test_kernels_at_training_shape():
+    a, b, gt = _train_shape_case()
+    loss, da, db, _ = _fused(a, b, gt, None)
+    r_loss, r_da, r_db = cl.focal_loss_and_grads(a.cuda(), b.cuda(), gt.cuda(), cl.scale_of())
+    assert abs(loss.item() - r_loss.item()) <= RTOL * abs(r_loss.item())
+    m_a, m_b = _close(da, r_da), _close(db, r_db)
+    print(f"training shape: loss rel err {abs(loss.item() / r_loss.item() - 1):.2e}, "
+          f"max |err| / (|ref| + absmax): dA {m_a:.2e}, dB {m_b:.2e}")
+
+
+def test_lazy_step_saves_at_least_one_matrix_at_training_shape():
+    a, b, gt = _train_shape_case()
+    B, L, S = gt.shape
+    gt = gt.cuda()
+    crit = losses.Loss(cl.LOSS_CONFIG)
+    cm = types.SimpleNamespace(temperature=cl.TEMPERATURE)
+    peaks = {}
+    for mode in ("eager", "lazy"):
+        fa, fb = a.cuda().requires_grad_(True), b.cuda().requires_grad_(True)
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        if mode == "eager":
+            conf = train_path.dual_softmax(cm, fa, fb, None)
+        else:
+            conf = train_path.TrainConfHandle(cm, fa, fb, None)
+        loss = crit.compute_coarse_loss(conf, gt)
+        loss.backward()
+        torch.cuda.synchronize()
+        peaks[mode] = torch.cuda.max_memory_allocated() - base
+        del conf, loss, fa, fb
+    print(f"peak above inputs: eager {peaks['eager'] / 2**20:.0f} MiB, lazy {peaks['lazy'] / 2**20:.0f} MiB")
+    assert peaks["eager"] - peaks["lazy"] >= B * L * S * 4
+
+
+@pytest.mark.parametrize("masked", [False, True])
+def test_lazy_training_step_matches_eager(masked):
+    """model.train() on CUDA: eager + the reference loss formula against lazy + the fused loss, and
+    both against "fp64": the lazy forward with the coarse loss evaluated in fp64 (the dual softmax and
+    the reference formula on the handle's features cast to double, through the same autograd graph)."""
+    sd = workload.synthetic_state_dict(0)
+    runs = {}
+    for mode in ("eager", "lazy", "fp64"):
+        m = OnePosePlus_model(mrg.train_config())
+        m.load_state_dict(sd, strict=True)
+        m = m.cuda().train()
+        m.conf_matrix_mode = "eager" if mode == "eager" else "lazy"
+        data = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in mrg.train_batch(sd, masked).items()}
+        torch.manual_seed(11)
+        m(data)
+        if mode == "fp64":
+            h = data["conf_matrix"]
+            data["conf_matrix"] = train_path.dual_softmax(h.cm, h.feat3d.double(), h.feat2d.double(), h.mask_query)
+        M = data["expec_f"].shape[0]
+        data["expec_f_gt"] = (torch.arange(2 * M, device="cuda", dtype=torch.float32).view(M, 2) % 7) / 5 - 0.6
+        losses.Loss(cl.LOSS_CONFIG).train()(data)
+        m.zero_grad()
+        data["loss"].backward()
+        runs[mode] = (m, data)
+    (me, de), (ml, dl), (m64, _) = runs["eager"], runs["lazy"], runs["fp64"]
+    assert isinstance(dl["conf_matrix"], train_path.TrainConfHandle) and torch.is_tensor(de["conf_matrix"])
+    for k in ("b_ids", "i_ids", "j_ids", "gt_mask", "m_bids"):
+        assert torch.equal(de[k], dl[k]), k
+    # 1e-4: the two runs' cuDNN convolutions are not bit-reproducible, and c amplifies sim differences
+    assert torch.allclose(dl["mconf"], de["mconf"], rtol=1e-4, atol=0)
+    assert abs(dl["loss"].item() - de["loss"].item()) <= 1e-5 * abs(de["loss"].item())
+    assert abs(dl["conf_matrix"].max().item() - de["conf_matrix"].max().item()) <= 1e-6
+    assert torch.allclose(dl["conf_matrix"].materialize(), de["conf_matrix"], rtol=1e-6, atol=1e-10)
+    # The yardstick is the fp64 coarse loss: on this batch the eager fp32 formula is itself 2e-3 - 8e-3
+    # of absmax away from it (fp32 sim at |sim| ~ 260 feeding c near 1), so the fused path is asked
+    # to be no further from fp64 than the eager path, with the issue's tolerance as slack.
+    pe, pl, p64 = dict(me.named_parameters()), dict(ml.named_parameters()), dict(m64.named_parameters())
+    bad = []
+    for name in mrg.TRAIN_GRADS:
+        ge, gl, g64 = pe[name].grad, pl[name].grad, p64[name].grad.double()
+        assert gl is not None and torch.isfinite(gl).all(), name
+        amax = float(g64.abs().max())
+        e_lazy, e_eager = float((gl - g64).abs().max()), float((ge - g64).abs().max())
+        print(f"{name}: max |.- fp64| / absmax: lazy {e_lazy / amax:.2e}, eager {e_eager / amax:.2e}")
+        if e_lazy > e_eager + 1e-6 + 2e-4 * amax:
+            bad.append(name)
+    assert not bad, bad
+
+
+def test_lazy_training_needs_split_precision():
+    sd = workload.synthetic_state_dict(0)
+    m = OnePosePlus_model(mrg.train_config(), precision="fp16")
+    m.load_state_dict(sd, strict=True)
+    m = m.cuda().train()
+    m.conf_matrix_mode = "lazy"
+    data = {k: (v.cuda() if torch.is_tensor(v) else v) for k, v in mrg.train_batch(sd, False).items()}
+    with pytest.raises(ValueError, match="fp16x3"):
+        m(data)
