@@ -253,8 +253,8 @@ static void ln_nsplit_cluster(GemmShape& s) {
   s.n_tiles = 1;
 }
 
-// Narrow the N tile until the operand ring, the accumulator tile (token-row epilogues: beside the ring
-// or over it) and the epilogue scratch of Epi fit.  Sets mma_n (the smallest compiled wgmma width
+// Narrow the N tile until the operand ring, the accumulator tile (EpiConvUp: beside the ring or over
+// it) and the epilogue scratch of Epi fit.  Sets mma_n (the smallest compiled wgmma width
 // >= block_n, and >= min_mma_n); call before the W map is built (its box is mma_n / cluster rows).
 template <class Epi>
 static int fit_tile(GemmShape& s, int min_mma_n = 64) {
@@ -639,9 +639,10 @@ int opp_sim_conf_colmax(const void* a, const void* b, const float* lse_own, cons
   return launch<A_ROWS, EpiConfCol>(maps, s, ep, (cudaStream_t)stream);
 }
 
-// partial slots per row written by opp_sim_lse / opp_sim_conf: one per column tile and epilogue warp group
+// partial slots per row written by the dual-softmax passes: one per column tile (a row lives in one
+// quad of one warp, so a tile leaves one (max, sum) / (max, argmax) per row)
 int opp_sim_tiles(int cols) {
-  return EpiLse::kGroups * ((cols + pick_block_n(cols) - 1) / pick_block_n(cols));
+  return (cols + pick_block_n(cols) - 1) / pick_block_n(cols);
 }
 
 }  // extern "C"

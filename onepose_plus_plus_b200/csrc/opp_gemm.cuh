@@ -24,13 +24,14 @@
 // its registers up (setmaxnreg 40) so that the MMA warpgroups can hold 232 each.  Warpgroup g
 // issues one full-width wgmma per K step (m64nNk16, N = the tile's mma_n) for tile rows
 // 64g .. 64g+63 into its registers and then runs the epilogue as epilogue group g, in one of two ways:
-//   * the conv epilogues (EpiConv, EpiWin: per-element math) read the accumulator registers
-//     directly (EpiFromRegs): warp q holds tile rows 64g+16q .. +15 over all N columns.  There is no
-//     accumulator tile in shared memory, so the ring takes its space and the producer never waits
-//     for an epilogue; the two warpgroups run their epilogues independently.
-//   * the token-row epilogues (row / column reductions) write the fp32 accumulator tile to shared
-//     memory: warp w owns accumulator rows 32*(w%4) .. +31, one row per thread, and the two groups
-//     take alternate 32-column chunks.
+//   * the conv epilogues (EpiConv, EpiWin: per-element math) and the token-row epilogues (row /
+//     column reductions: LayerNorm, linear-attention normaliser, dual-softmax statistics) read the
+//     accumulator registers directly (EpiFromRegs): warp q holds tile rows 64g+16q .. +15 over all N
+//     columns.  There is no accumulator tile in shared memory, so the ring takes its space and the
+//     producer never waits for an epilogue; the two warpgroups run their epilogues independently.
+//   * the fused-upsample conv (EpiConvUp) writes the fp32 accumulator tile to shared memory: warp w
+//     owns accumulator rows 32*(w%4) .. +31, one row per thread, and the two groups take alternate
+//     32-column chunks.
 //
 // Reference semantics implemented by the epilogues are cited at each functor
 // (paths relative to the reference repo zju3dv/OnePose_Plus_Plus).
@@ -42,20 +43,6 @@
 
 #ifndef OPP_CONV_GROUPS
 #define OPP_CONV_GROUPS 2
-#endif
-#ifndef OPP_LN_GROUPS
-#define OPP_LN_GROUPS 2
-#endif
-#ifndef OPP_ROW_GROUPS
-#define OPP_ROW_GROUPS 2   // EpiStoreF16 / EpiQ / EpiLse / EpiConf
-#endif
-// Coalesced (warp-staged) global I/O in the LayerNorm epilogue / for the fp32 conf_matrix store
-// instead of row-per-thread 16 B accesses (32 L1 wavefronts per instruction).
-#ifndef OPP_LN_STAGED
-#define OPP_LN_STAGED 1
-#endif
-#ifndef OPP_CONF_STAGED
-#define OPP_CONF_STAGED 1
 #endif
 
 namespace opp {
@@ -132,11 +119,8 @@ struct EpiCtx {
   uint32_t acc;    // shared-memory word address (byte address / 4) of column 0 of this thread's
                    // accumulator row
   int b, m_tile, n_tile;
-  int q;           // row quarter of this warp: rows 32q .. 32q+31 of the tile
+  int q;           // warp within the epilogue group
   int a_mode;
-  int row;         // row within the batch (pixel index within the image for A_CONV)
-  long long grow;  // b*rows + row
-  bool valid;      // row is inside the tensor
   int n0;          // first global column of the tile
   int ncols;       // valid columns in this tile (multiple of 8)
   int etid;        // 0..127 within the epilogue group
@@ -145,9 +129,9 @@ struct EpiCtx {
   uint32_t smem_s, wstage_s;   // the same two regions as 32-bit shared-space addresses
   int group;       // epilogue warp group (0/1); groups take alternate 32-column chunks
   int col_first, col_step;
-  // rows (lane>>2) + 8*i, i = 0..3 of this warp's quarter (EpiFromRegs: i = 0..1, the two rows of
-  // this thread's accumulator fragment): element offset grow*ld is NOT stored, only grow (row index
-  // in the output) and validity, computed once per tile
+  // rows (lane>>2) + 8*i, i = 0..3 of this warp's quarter of the accumulator tile (EpiFromRegs:
+  // i = 0..1, the two rows of this thread's accumulator fragment): element offset grow*ld is NOT
+  // stored, only grow (row index in the output) and validity, computed once per tile
   long long sgrow[4];
   unsigned svalid;
   int next_b, next_m_tile;   // the (batch, M tile) this CTA processes next, or next_b = -1
@@ -229,14 +213,9 @@ __device__ __forceinline__ bool epi_row_at(const GemmShape& s, const EpiCtx& c, 
   grow = (long long)c.b * s.rows + row;
   return ok;
 }
-// (global row, validity) of row `rr` (0..31) of this warp's quarter of the tile
-__device__ __forceinline__ bool epi_row_info(const GemmShape& s, const EpiCtx& c, int rr,
-                                             long long& grow, int& row) {
-  return epi_row_at(s, c, c.q * 32 + rr, grow, row);
-}
 
 // ---------------------------------------------------------------------------------------------
-// Accumulator tile in shared memory: row r, column j at word  r * (mma_n + kAccPad) + j.
+// Accumulator tile in shared memory (EpiConvUp only): row r, column j at word  r * (mma_n + kAccPad) + j.
 // The pad of kAccPad = 4 words puts the 16-byte reads of 8 consecutive rows into distinct banks.
 // ---------------------------------------------------------------------------------------------
 constexpr int kAccPad = 4;
@@ -253,29 +232,17 @@ __device__ __forceinline__ void acc_ld32(uint32_t waddr, float (&v)[32]) {
     v[4 * i + 3] = __uint_as_float(u.w);
   }
 }
-// Walk this thread's accumulator row in 32-column chunks: f(col, v[32]) for col = first,
-// first+step, ... < ncols (warp-uniform).  The two epilogue groups take alternate chunks
-// (first = 32*group, step = 64).
-template <class F>
-__device__ __forceinline__ void acc_foreach32(uint32_t abase, int ncols, int first, int step, F&& f) {
-  float v[32];
-  for (int col = first; col < ncols; col += step) {
-    acc_ld32(abase + col, v);
-    f(col, v);
-  }
-}
 
 // ---------------------------------------------------------------------------------------------
-// Warp-staged, coalesced epilogue I/O.  Accumulator rows live one-per-thread, but global memory
-// wants whole 64/128-byte segments: every 32x32 chunk goes through a per-warp shared-memory
-// transpose buffer (row stride padded by 16 B so both access directions are conflict-light).
+// Warp-staged, coalesced store of one-row-per-thread values (EpiConvUp): global memory wants whole
+// 64/128-byte segments, so every 32x32 chunk goes through a per-warp shared-memory transpose buffer
+// (row stride padded by 16 B so both access directions are conflict-light).
 // ---------------------------------------------------------------------------------------------
 constexpr int kStageRowH = 80;    // 32 fp16 (64 B) + 16 B pad
 constexpr int kWarpStageBytes = 32 * kStageRowH;   // 2560 B
 
 // fp16 planes: v = this lane's 32 values for global columns [gcol, gcol+32); nvalid = valid
 // columns of the chunk (multiple of 8).  Writes hi (and lo when lo_off != 0).
-template <bool kBatch = true>
 __device__ __forceinline__ void staged_store_h32(const GemmShape& s, const EpiCtx& c, __half* out,
                                                  long long ld, int lo_off, int gcol,
                                                  const float* v, int nvalid) {
@@ -308,103 +275,12 @@ __device__ __forceinline__ void staged_store_h32(const GemmShape& s, const EpiCt
     }
     __syncwarp();
     const int seg = lane & 3;
-    // all four shared loads first, then the four global stores: a paired LDS -> STG waits out the
-    // shared-memory latency before every store
-    // (kBatch = false: the conv epilogues are MMA-bound; the paired form holds fewer registers)
-    if constexpr (kBatch) {
-      uint4 t4[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) t4[i] = lds128(st + ((lane >> 2) + 8 * i) * kStageRowH + seg * 16);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        if (((c.svalid >> i) & 1u) && seg * 8 < nvalid)
-          *reinterpret_cast<uint4*>(out + c.sgrow[i] * ld + plane * lo_off + gcol + seg * 8) = t4[i];
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int rr = (lane >> 2) + 8 * i;
-        if (((c.svalid >> i) & 1u) && seg * 8 < nvalid)
-          *reinterpret_cast<uint4*>(out + c.sgrow[i] * ld + plane * lo_off + gcol + seg * 8) =
-              lds128(st + rr * kStageRowH + seg * 16);
-      }
-    }
-    __syncwarp();
-  }
-}
-
-// Inverse of staged_store_h32: r[0..31] = the fp32 value (hi + lo) of this lane's row at global
-// columns [gcol, gcol+32).  Global reads are coalesced (one instruction = 8 rows x 64 B); the
-// row-per-thread form (one instruction = 32 rows x 16 B) costs 32 L1 wavefronts per instruction and
-// made the LayerNorm epilogues wavefront-bound.  Rows / columns outside the tensor read as 0.
-// `pre` holds loads issued earlier by staged_load_issue (so their latency overlaps other work).
-struct StagedRows {
-  uint4 hi[4], lo[4];
-};
-__device__ __forceinline__ void staged_load_issue(const EpiCtx& c, const __half* src, long long ld,
-                                                  int lo_off, int gcol, int nvalid, StagedRows& pre) {
-  const int lane = threadIdx.x & 31;
-  const int seg = lane & 3;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const bool in = ((c.svalid >> i) & 1u) && seg * 8 < nvalid;
-    const __half* row = src + c.sgrow[i] * ld + gcol + seg * 8;
-    pre.hi[i] = in ? *reinterpret_cast<const uint4*>(row) : make_uint4(0, 0, 0, 0);
-    pre.lo[i] = (in && lo_off) ? *reinterpret_cast<const uint4*>(row + lo_off) : make_uint4(0, 0, 0, 0);
-  }
-}
-__device__ __forceinline__ void staged_load_add(const EpiCtx& c, int lo_off, const StagedRows& pre,
-                                                float* v) {
-  const int lane = threadIdx.x & 31;
-  const uint32_t st = c.wstage_s;
-  const uint32_t mine = st + lane * kStageRowH;
-  const int seg = lane & 3;
-#pragma unroll
-  for (int plane = 0; plane < 2; ++plane) {
-    if (plane == 1 && lo_off == 0) break;
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-      sts128(st + ((lane >> 2) + 8 * i) * kStageRowH + seg * 16, plane == 0 ? pre.hi[i] : pre.lo[i]);
-    __syncwarp();
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const uint4 u = lds128(mine + g * 16);
-      const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 f = __half22float2(h[j]);
-        v[8 * g + 2 * j] += f.x;
-        v[8 * g + 2 * j + 1] += f.y;
-      }
-    }
-    __syncwarp();
-  }
-}
-
-// fp32 rows (conf_matrix): v = this lane's 32 values for global columns [gcol, gcol+32), written in
-// two 16-column halves through the same transpose buffer (16 fp32 = 64 B = one staging row), so a
-// store instruction covers 8 rows x 64 B instead of 32 rows x 16 B.  nvalid: multiple of 4.
-__device__ __forceinline__ void staged_store_f32(const EpiCtx& c, float* out, long long ld, int gcol,
-                                                 const float* v, int nvalid) {
-  const int lane = threadIdx.x & 31;
-  const uint32_t st = c.wstage_s;
-  const uint32_t mine = st + lane * kStageRowH;
-  const int seg = lane & 3;
-#pragma unroll
-  for (int half = 0; half < 2; ++half) {
-#pragma unroll
-    for (int g = 0; g < 4; ++g)
-      sts128(mine + g * 16,
-             make_uint4(__float_as_uint(v[16 * half + 4 * g]), __float_as_uint(v[16 * half + 4 * g + 1]),
-                        __float_as_uint(v[16 * half + 4 * g + 2]), __float_as_uint(v[16 * half + 4 * g + 3])));
-    __syncwarp();
-    uint4 t4[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) t4[i] = lds128(st + ((lane >> 2) + 8 * i) * kStageRowH + seg * 16);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      if (((c.svalid >> i) & 1u) && 16 * half + seg * 4 < nvalid)
-        *reinterpret_cast<uint4*>(out + c.sgrow[i] * ld + gcol + 16 * half + seg * 4) = t4[i];
+      const int rr = (lane >> 2) + 8 * i;
+      if (((c.svalid >> i) & 1u) && seg * 8 < nvalid)
+        *reinterpret_cast<uint4*>(out + c.sgrow[i] * ld + plane * lo_off + gcol + seg * 8) =
+            lds128(st + rr * kStageRowH + seg * 16);
     }
     __syncwarp();
   }
@@ -414,252 +290,6 @@ __device__ __forceinline__ void staged_store_f32(const EpiCtx& c, float* out, lo
 // Epilogues.  Outputs that feed later GEMMs are written as (hi|lo) plane pairs when
 // `out_lo` != 0: row layout [hi(n_total) | lo(n_total)], out_lo = n_total.
 // =============================================================================================
-
-// Plain store with an optional activation on the leading `act_cols` columns.
-//   act 1 = ReLU  (transformer.py:41-45 mlp ReLU), act 2 = elu(x)+1 (linear_attention.py:10-11)
-struct EpiStoreF16 {
-  static constexpr int kGroups = OPP_ROW_GROUPS;
-  struct Params {
-    __half* out;
-    long long ld;   // row stride in elements
-    int out_lo;     // 0 or n_total
-    int act;
-    int act_cols;   // multiple of 32
-    // padded positions (query_image_mask, linear_attention.py:49-53): rows with row_mask[grow] == 0
-    // are written as zeros (K' and V of a masked source token), or null
-    const unsigned char* row_mask;
-  };
-  __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    const bool masked = p.row_mask && c.valid && p.row_mask[c.grow] == 0;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-      const int g0 = c.n0 + col;
-      const int act = g0 < p.act_cols ? p.act : 0;
-      if (act == 1) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-      } else if (act == 2) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = elu_plus_one_fast(v[j]);
-      }
-      if (masked) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-      }
-      staged_store_h32(s, c, p.out, p.ld, p.out_lo, g0, v, c.ncols - col);
-    });
-  }
-};
-
-// Query side of linear attention (linear_attention.py:45,58-59): Q = elu(q)+1,
-// Z = 1/(Q . Ksum + eps), output Q * Z * v_length per head of 32 channels.  The matching KV
-// state is pre-divided by v_length (linear_attention.py:55-56), so (Q*Z*v_length) @ (KV/v_length)
-// reproduces the reference product.
-struct EpiQ {
-  static constexpr int kGroups = OPP_ROW_GROUPS;
-  struct Params {
-    __half* out;
-    long long ld;
-    int out_lo;
-    const float* ksum;  // [batches][n_total]
-    float v_len;
-    float eps;
-    const unsigned char* row_mask;   // Q = 0 on padded query positions (linear_attention.py:49-50), or null
-  };
-  __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    epi_sync(c);
-    for (int i = c.etid; i < c.ncols; i += 128)
-      sts32f(c.smem_s + 4 * i, p.ksum[(long long)c.b * s.n_total + c.n0 + i]);
-    epi_sync(c);
-    const bool qmasked = p.row_mask && c.valid && p.row_mask[c.grow] == 0;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-      float dot = 0.f;
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        const uint4 kq = lds128(c.smem_s + 4 * (col + 4 * g));
-        const float kk[4] = {__uint_as_float(kq.x), __uint_as_float(kq.y), __uint_as_float(kq.z),
-                             __uint_as_float(kq.w)};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          v[4 * g + j] = elu_plus_one_fast(v[4 * g + j]);
-          dot = fmaf(v[4 * g + j], kk[j], dot);
-        }
-      }
-      const float z = qmasked ? 0.f : p.v_len / (dot + p.eps);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] *= z;
-      staged_store_h32(s, c, p.out, p.ld, p.out_lo, c.n0 + col, v, 32);
-    });
-  }
-};
-
-// LayerNorm over the full output row (the tile spans all N columns), optional residual add
-// (transformer.py:86-94: norm1 after merge; norm2 then x + msg).
-struct EpiLN {
-  static constexpr int kGroups = OPP_LN_GROUPS;
-  // N-split cluster (GemmShape.pair == 2): 2 x 128 (mean, M2) slots the peer CTA writes into + 2 mbarriers
-  static constexpr int kExtraSmem = 2 * 128 * 8 + 64;
-  struct Params {
-    const float* gamma;
-    const float* beta;
-    float eps;
-    const __half* resid;  // same layout as out16 (ld, out_lo) or null
-    int resid_shared;     // resid is [1][rows][..], shared by every batch element
-    __half* out16;        // or null
-    long long ld;
-    int out_lo;
-    float* out32;         // fp32 [rows][n_total] or null
-  };
-  __device__ static void prefetch(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    if (!p.resid || !c.valid) return;
-    const char* row = reinterpret_cast<const char*>(p.resid + (p.resid_shared ? (long long)c.row : c.grow) * p.ld + c.n0);
-    for (int o = c.group * 128; o < c.ncols * 2; o += 256) {
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(row + o));
-      if (p.out_lo) asm volatile("prefetch.global.L2 [%0];" ::"l"(row + 2 * p.out_lo + o));
-    }
-  }
-  // Two warp groups share every row (alternate 32-column chunks).  Each thread accumulates shifted
-  // sums over its half, the halves are merged with Chan's parallel-variance formula (group 0
-  // first, so both threads of a row compute bit-identical statistics), then each group
-  // normalises and writes its own chunks.  Residual loads and fp16 stores go through the per-warp
-  // transpose buffer (OPP_LN_STAGED): a row-per-thread 16 B access touches 32 cache lines per
-  // instruction = 32 L1 wavefronts.
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    // gamma / beta of this CTA's columns, staged once per CTA: a LayerNorm GEMM has one N tile, or
-    // (N-split cluster) one fixed N half per CTA; the launchers check it
-    if (c.it == 0) {
-      for (int i = c.etid; i < c.ncols; i += 128) {
-        sts32f(c.smem_s + 4 * i, p.gamma[c.n0 + i]);
-        sts32f(c.smem_s + 4 * (256 + i), p.beta[c.n0 + i]);
-      }
-      epi_sync(c);
-    }
-    float x0 = 0.f, s1 = 0.f, s2 = 0.f;
-    int cnt = 0;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-      if (cnt == 0) x0 = v[0];
-      cnt += 32;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const float d = v[j] - x0;
-        s1 += d;
-        s2 = fmaf(d, d, s2);
-      }
-    });
-    // exchange (x0, s1, s2, cnt) with the thread of the other group that owns the same row
-    float4 ga = make_float4(x0, s1, s2, (float)cnt), gb = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (kGroups == 2) {
-      const int lane = threadIdx.x & 31;
-      float4* mine = reinterpret_cast<float4*>(c.wstage) + lane;
-      const float4* other = reinterpret_cast<const float4*>(
-                                c.wstage + (c.group ? -4 : 4) * kWarpStageBytes) + lane;
-      *mine = ga;
-      named_bar_sync(3, 256);
-      const float4 o = *other;
-#if OPP_LN_STAGED
-      named_bar_sync(3, 256);   // the slots live in the transpose buffers the second pass reuses
-#endif
-      if (c.group == 0) {
-        gb = o;
-      } else {
-        gb = ga;
-        ga = o;
-      }
-    }
-    float mean, m2;
-    {
-      const float na = ga.w, nb = gb.w;
-      const float mean_a = na > 0.f ? ga.x + ga.y / na : 0.f;
-      const float m2a = na > 0.f ? fmaxf(ga.z - ga.y * ga.y / na, 0.f) : 0.f;
-      const float mean_b = nb > 0.f ? gb.x + gb.y / nb : mean_a;
-      const float m2b = nb > 0.f ? fmaxf(gb.z - gb.y * gb.y / nb, 0.f) : 0.f;
-      const float n = na + nb;
-      const float delta = mean_b - mean_a;
-      mean = mean_a + delta * (nb / n);
-      m2 = m2a + m2b + delta * delta * (na * nb / n);
-    }
-    if (s.pair == 2) {
-      // N-split cluster: the other half of every row is in the peer CTA of the cluster (same M tile,
-      // same iteration).  Group 0 writes (mean, M2) of this half into the PEER's slot of this tile
-      // parity and arrives (release.cluster) on the peer's mbarrier; everybody waits on the local
-      // one (acquire.cluster) and merges "columns 0..127 first", so both CTAs get bit-identical
-      // statistics.  Two slots / barriers alternate by tile parity: the peer can be one publish
-      // ahead, never two (its next publish needs ours; the 256-thread barrier that ends run()
-      // keeps our group 1 from still reading the slot by then).
-      const int lane = threadIdx.x & 31;
-      const int par = c.it & 1;
-      float2* slot = reinterpret_cast<float2*>(c.extra) + par * 128 + c.q * 32 + lane;
-      uint64_t* xbar = reinterpret_cast<uint64_t*>(c.extra + 2 * 128 * 8) + par;
-      const uint32_t peer = (uint32_t)(c.n_tile ^ 1);
-      if (c.group == 0) {
-        st_cluster_f32x2(slot, peer, mean, m2);
-        mbar_arrive_cluster_release(xbar, peer);
-      }
-      mbar_wait_cluster(xbar, (uint32_t)((c.it >> 1) & 1));
-      const float2 o = *slot;
-      const float mean_a = c.n_tile == 0 ? mean : o.x, m2a = c.n_tile == 0 ? m2 : o.y;
-      const float mean_b = c.n_tile == 0 ? o.x : mean, m2b = c.n_tile == 0 ? o.y : m2;
-      const float delta = mean_b - mean_a;
-      mean = mean_a + delta * 0.5f;                       // both halves have c.ncols columns
-      m2 = m2a + m2b + delta * delta * (0.5f * (float)c.ncols);
-    }
-    const float rstd = 1.f / sqrtf(m2 / (float)s.n_total + p.eps);
-    // a shared residual is indexed by the row inside the batch: rebase the pointer once per tile
-    const __half* resid = p.resid;
-    if (resid && p.resid_shared) resid -= (long long)c.b * s.rows * p.ld;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-#if OPP_LN_STAGED
-      StagedRows pre;
-      if (resid) staged_load_issue(c, resid, p.ld, p.out_lo, c.n0 + col, c.ncols - col, pre);
-#endif
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        const uint4 gq = lds128(c.smem_s + 4 * (col + 4 * g));
-        const uint4 bq = lds128(c.smem_s + 4 * (256 + col + 4 * g));
-        v[4 * g + 0] = (v[4 * g + 0] - mean) * rstd * __uint_as_float(gq.x) + __uint_as_float(bq.x);
-        v[4 * g + 1] = (v[4 * g + 1] - mean) * rstd * __uint_as_float(gq.y) + __uint_as_float(bq.y);
-        v[4 * g + 2] = (v[4 * g + 2] - mean) * rstd * __uint_as_float(gq.z) + __uint_as_float(bq.z);
-        v[4 * g + 3] = (v[4 * g + 3] - mean) * rstd * __uint_as_float(gq.w) + __uint_as_float(bq.w);
-      }
-#if OPP_LN_STAGED
-      // every lane takes part in the warp-staged transposes; row validity is per staged row
-      if (resid) staged_load_add(c, p.out_lo, pre, v);
-      if (p.out32 && c.valid) {
-        float4* o4 = reinterpret_cast<float4*>(p.out32 + c.grow * (long long)s.n_total + c.n0 + col);
-#pragma unroll
-        for (int g = 0; g < 8; ++g)
-          o4[g] = make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-      }
-      if (p.out16) staged_store_h32(s, c, p.out16, p.ld, p.out_lo, c.n0 + col, v, c.ncols - col);
-#else
-      if (!c.valid) return;
-      if (resid) {
-        const __half* rrow = resid + c.grow * p.ld;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float r[8];
-          load_split8(rrow, col + g * 8, r, p.out_lo);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[g * 8 + j] += r[j];
-        }
-      }
-      if (p.out32) {
-        float4* o4 = reinterpret_cast<float4*>(p.out32 + c.grow * (long long)s.n_total + c.n0 + col);
-#pragma unroll
-        for (int g = 0; g < 8; ++g)
-          o4[g] = make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-      }
-      if (p.out16) {
-        __half* row = p.out16 + c.grow * p.ld;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) store_split8(row, col + g * 8, v + g * 8, p.out_lo);
-      }
-#endif
-    });
-    if (kGroups == 2) named_bar_sync(3, 256);   // the exchange slots are reused by the next tile
-  }
-};
 
 // ---------------------------------------------------------------------------------------------
 // Register-fragment epilogue I/O (EpiFromRegs).  Warp q of MMA warpgroup g holds tile rows
@@ -689,12 +319,16 @@ __device__ __forceinline__ float2 lds64f(uint32_t addr) {
   return v;
 }
 
+__device__ __forceinline__ void sts64f(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+
 // the (tile-row) fragment values of slice j: v[4 ii + 2h + e] = d[4 (4j + ii) + 2h + e]; columns
-// past the accumulator width (the second half of the last slice at N = 208) read as 0
+// past the accumulator width (the second half of the last slice at N = 208) read as `fill`
 template <int N>
-__device__ __forceinline__ void frag_slice(const float (&d)[N / 2], int j, float (&v)[16]) {
+__device__ __forceinline__ void frag_slice(const float (&d)[N / 2], int j, float (&v)[16], float fill = 0.f) {
 #pragma unroll
-  for (int k = 0; k < 16; ++k) v[k] = 16 * j + k < N / 2 ? d[16 * j + k] : 0.f;
+  for (int k = 0; k < 16; ++k) v[k] = 16 * j + k < N / 2 ? d[16 * j + k] : fill;
 }
 
 // + the fp32 vector at smem word address `base` (the epilogue group's bias) per fragment column
@@ -739,6 +373,30 @@ __device__ __forceinline__ void frag_store_h(const GemmShape& s, const EpiCtx& c
         *reinterpret_cast<uint4*>(out + c.sgrow[h] * ld + plane * lo_off + gcol + t * 8) =
             lds128(st + plane * kFragPlaneH + (rq + 8 * h) * kFragRowH + 16 * t);
   }
+  __syncwarp();
+}
+
+// fp32 slice columns [gcol, gcol + 32) of this warp's 16 rows (row stride ld floats, 16-byte aligned
+// rows): the slice goes through the stage (row pitch kFragRowF) and leaves it in two 16-column halves,
+// lane moving the 16-byte segment (lane&3) of its two rows: 8 rows x 64 B per instruction.
+// nvalid = valid columns of the slice (multiple of 4).
+__device__ __forceinline__ void frag_store_f32(const EpiCtx& c, float* out, long long ld, int gcol,
+                                               const float (&v)[16], int nvalid) {
+  const int lane = threadIdx.x & 31, t = lane & 3, rq = lane >> 2;
+  const uint32_t st = c.wstage_s;
+#pragma unroll
+  for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      sts64f(st + (rq + 8 * h) * kFragRowF + 4 * (8 * ii + 2 * t), v[4 * ii + 2 * h], v[4 * ii + 2 * h + 1]);
+  __syncwarp();
+#pragma unroll
+  for (int half = 0; half < 2; ++half)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (((c.svalid >> h) & 1u) && 16 * half + 4 * t < nvalid)
+        *reinterpret_cast<uint4*>(out + c.sgrow[h] * ld + gcol + 16 * half + 4 * t) =
+            lds128(st + (rq + 8 * h) * kFragRowF + 64 * half + 16 * t);
   __syncwarp();
 }
 
@@ -1117,7 +775,324 @@ struct EpiConvUp {
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = v[j] > 0.f ? v[j] : v[j] * p.slope;
       }
-      staged_store_h32<false>(s, c, p.out, p.ld, p.out_lo, c.n0 + col, v, c.ncols - col);
+      staged_store_h32(s, c, p.out, p.ld, p.out_lo, c.n0 + col, v, c.ncols - col);
+    }
+  }
+};
+
+// =============================================================================================
+// Token-row epilogues (A_ROWS), on the accumulator registers like the conv epilogues.  Warp q of
+// warpgroup g holds the 16 consecutive token rows 64g + 16q .. +15 of the tile over all N columns, so
+// a row never spans the two warpgroups: this lane holds rows (lane>>2) + 8h (c.sgrow[h], bit h of
+// c.svalid) at columns 8i + 2(lane&3) + {0, 1}.  A row is spread over the 4 lanes of a quad (row
+// reductions: two xor shuffles, every lane ends with the same bits), a column over the two rows of
+// a lane and the 8 quads of the warp (column reductions: in the lane, then three xor levels).
+// =============================================================================================
+__device__ __forceinline__ float quad_sum(float x) {
+  x += __shfl_xor_sync(0xffffffffu, x, 1);
+  return x + __shfl_xor_sync(0xffffffffu, x, 2);
+}
+__device__ __forceinline__ float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+// (value, column) maximum over the quad; the lowest column wins a tie, whatever the lane order
+__device__ __forceinline__ void quad_argmax(float& v, int& idx) {
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, v, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+    if (ov > v || (ov == v && oi < idx)) {
+      v = ov;
+      idx = oi;
+    }
+  }
+}
+
+// Column reductions of a 32-column slice: x[k], k = 2 ii + e, is this lane's value of slice column
+// 8 ii + 2 (lane&3) + e.  col_allreduce8: every lane ends with the reduction of its 8 columns over
+// the warp's 16 rows (xor butterfly over lane bits 2..4).  col_reduce8: at each level a lane keeps
+// one half of its values and trades the other half with lane ^ (4 << lvl) (7 shuffles); lane ends
+// with the reduction of slice column frag_lane_col() only.
+template <class Op>
+__device__ __forceinline__ void col_allreduce8(float (&x)[8], Op op) {
+#pragma unroll
+  for (int o = 4; o <= 16; o <<= 1)
+#pragma unroll
+    for (int k = 0; k < 8; ++k) x[k] = op(x[k], __shfl_xor_sync(0xffffffffu, x[k], o));
+}
+template <class Op>
+__device__ __forceinline__ float col_reduce8(float (&x)[8], Op op) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int lvl = 2; lvl >= 0; --lvl) {
+    const int half = 1 << lvl;
+    const bool up = (lane >> (2 + lvl)) & 1;
+#pragma unroll
+    for (int k = 0; k < half; ++k) {
+      const float keep = up ? x[half + k] : x[k];
+      const float send = up ? x[k] : x[half + k];
+      x[k] = op(keep, __shfl_xor_sync(0xffffffffu, send, 4 << lvl));
+    }
+  }
+  return x[0];   // value k = lane >> 2
+}
+__device__ __forceinline__ int frag_lane_col() {
+  const int lane = threadIdx.x & 31, rq = lane >> 2;
+  return 8 * (rq >> 1) + 2 * (lane & 3) + (rq & 1);
+}
+// element k of x (k warp-uniform at run time, x indexed by compile-time constants only)
+__device__ __forceinline__ float pick8(const float (&x)[8], int k) {
+  float r = x[0];
+#pragma unroll
+  for (int i = 1; i < 8; ++i) r = k == i ? x[i] : r;
+  return r;
+}
+// the two warps of a 32-row group (q = 2k, 2k+1 of the epilogue group) meet here
+__device__ __forceinline__ void pair_sync(const EpiCtx& c) { named_bar_sync(5 + 2 * c.group + (c.q >> 1), 64); }
+
+// fp32 per-column vector of this tile (lse of the other side), staged per tile: it changes with the
+// batch and the N tile
+__device__ __forceinline__ void epi_stage_cols_b(const GemmShape& s, const EpiCtx& c, const float* src) {
+  epi_sync(c);
+  for (int i = c.etid; i < c.ncols; i += 128) sts32f(c.smem_s + 4 * i, src[(long long)c.b * s.n_total + c.n0 + i]);
+  epi_sync(c);
+}
+
+// Plain store with an optional activation on the leading `act_cols` columns.
+//   act 1 = ReLU  (transformer.py:41-45 mlp ReLU), act 2 = elu(x)+1 (linear_attention.py:10-11)
+// Per element exactly the operations of the shared-memory form: the outputs are bit-identical.
+struct EpiStoreF16 {
+  static constexpr int kGroups = 2;
+  static constexpr bool kFromRegs = true;
+  struct Params {
+    __half* out;
+    long long ld;   // row stride in elements
+    int out_lo;     // 0 or n_total
+    int act;
+    int act_cols;   // multiple of 32
+    // padded positions (query_image_mask, linear_attention.py:49-53): rows with row_mask[grow] == 0
+    // are written as zeros (K' and V of a masked source token), or null
+    const unsigned char* row_mask;
+  };
+  __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
+    bool masked[2] = {false, false};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) masked[h] = p.row_mask && ((c.svalid >> h) & 1u) && p.row_mask[c.sgrow[h]] == 0;
+#pragma unroll
+    for (int j = 0; j < (N + 31) / 32; ++j) {
+      const int col = 32 * j;
+      if (col < c.ncols) {
+        const int g0 = c.n0 + col;
+        const int act = g0 < p.act_cols ? p.act : 0;
+        float v[16];
+        frag_slice<N>(d, j, v);
+        if (act == 1) {
+#pragma unroll
+          for (int k = 0; k < 16; ++k) v[k] = fmaxf(v[k], 0.f);
+        } else if (act == 2) {
+#pragma unroll
+          for (int k = 0; k < 16; ++k) v[k] = elu_plus_one_fast(v[k]);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (masked[h]) {
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii) v[4 * ii + 2 * h] = v[4 * ii + 2 * h + 1] = 0.f;
+          }
+        frag_store_h(s, c, p.out, p.ld, p.out_lo, g0, v, c.ncols - col);
+      }
+    }
+  }
+};
+
+// Query side of linear attention (linear_attention.py:45,58-59): Q = elu(q)+1,
+// Z = 1/(Q . Ksum + eps), output Q * Z * v_length per head of 32 channels.  The matching KV
+// state is pre-divided by v_length (linear_attention.py:55-56), so (Q*Z*v_length) @ (KV/v_length)
+// reproduces the reference product.  A head is one 32-column slice: its dot is 8 products per lane
+// and a quad sum.
+struct EpiQ {
+  static constexpr int kGroups = 2;
+  static constexpr bool kFromRegs = true;
+  struct Params {
+    __half* out;
+    long long ld;
+    int out_lo;
+    const float* ksum;  // [batches][n_total]
+    float v_len;
+    float eps;
+    const unsigned char* row_mask;   // Q = 0 on padded query positions (linear_attention.py:49-50), or null
+  };
+  __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
+    epi_stage_cols_b(s, c, p.ksum);
+    const int c0 = 2 * (threadIdx.x & 3);
+    bool qmasked[2] = {false, false};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) qmasked[h] = p.row_mask && ((c.svalid >> h) & 1u) && p.row_mask[c.sgrow[h]] == 0;
+#pragma unroll
+    for (int j = 0; j < (N + 31) / 32; ++j) {
+      const int col = 32 * j;
+      if (col < c.ncols) {
+        float v[16];
+        frag_slice<N>(d, j, v);
+        float dot[2] = {0.f, 0.f};
+#pragma unroll
+        for (int ii = 0; ii < 4; ++ii) {
+          const float2 kk = lds64f(c.smem_s + 4 * (col + 8 * ii + c0));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            v[4 * ii + 2 * h] = elu_plus_one_fast(v[4 * ii + 2 * h]);
+            v[4 * ii + 2 * h + 1] = elu_plus_one_fast(v[4 * ii + 2 * h + 1]);
+            dot[h] = fmaf(v[4 * ii + 2 * h], kk.x, dot[h]);
+            dot[h] = fmaf(v[4 * ii + 2 * h + 1], kk.y, dot[h]);
+          }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float qd = quad_sum(dot[h]);   // every lane shuffles, masked rows included
+          const float z = qmasked[h] ? 0.f : p.v_len / (qd + p.eps);
+#pragma unroll
+          for (int ii = 0; ii < 4; ++ii) {
+            v[4 * ii + 2 * h] *= z;
+            v[4 * ii + 2 * h + 1] *= z;
+          }
+        }
+        frag_store_h(s, c, p.out, p.ld, p.out_lo, c.n0 + col, v, 32);
+      }
+    }
+  }
+};
+
+// LayerNorm over the full output row (the tile spans all N columns), optional residual add
+// (transformer.py:86-94: norm1 after merge; norm2 then x + msg).  A row lives in one quad: mean and
+// M2 are two passes over the registers with a quad sum each.  The tile is the whole row (the
+// launchers check block_n == mma_n == n, or the 128-column halves of the N-split cluster).
+struct EpiLN {
+  static constexpr int kGroups = 2;
+  static constexpr bool kFromRegs = true;
+  // N-split cluster (GemmShape.pair == 2): 2 x 128 (mean, M2) slots the peer CTA writes into + 2 mbarriers
+  static constexpr int kExtraSmem = 2 * 128 * 8 + 64;
+  static constexpr int kExchangeArrivals = 64;   // one writer lane per quad of the 8 MMA warps
+  struct Params {
+    const float* gamma;
+    const float* beta;
+    float eps;
+    const __half* resid;  // same layout as out16 (ld, out_lo) or null
+    int resid_shared;     // resid is [1][rows][..], shared by every batch element
+    __half* out16;        // or null
+    long long ld;
+    int out_lo;
+    float* out32;         // fp32 [rows][n_total] or null
+  };
+  __device__ static void prefetch(const Params& p, const GemmShape& s, const EpiCtx& c) {
+    if (!p.resid) return;
+    const int t = threadIdx.x & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!((c.svalid >> h) & 1u)) continue;
+      const long long r = p.resid_shared ? c.sgrow[h] - (long long)c.b * s.rows : c.sgrow[h];
+      const char* row = reinterpret_cast<const char*>(p.resid + r * p.ld + c.n0);
+      for (int o = 128 * t; o < c.ncols * 2; o += 512) {
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(row + o));
+        if (p.out_lo) asm volatile("prefetch.global.L2 [%0];" ::"l"(row + 2 * p.out_lo + o));
+      }
+    }
+  }
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
+    const int lane = threadIdx.x & 31, c0 = 2 * (lane & 3);
+    // a shared residual is indexed by the row inside the batch: rebase the pointer once per tile
+    const __half* resid = p.resid;
+    if (resid && p.resid_shared) resid -= (long long)c.b * s.rows * p.ld;
+    // the first slice's residual is copied into the stage while the statistics are computed
+    if (resid) frag_load_issue(c, resid, p.ld, p.out_lo, c.n0, c.ncols);
+    // gamma / beta of this CTA's columns, staged once per CTA: a LayerNorm GEMM has one N tile, or
+    // (N-split cluster) one fixed N half per CTA; the launchers check it
+    if (c.it == 0) {
+      for (int i = c.etid; i < c.ncols; i += 128) {
+        sts32f(c.smem_s + 4 * i, p.gamma[c.n0 + i]);
+        sts32f(c.smem_s + 4 * (256 + i), p.beta[c.n0 + i]);
+      }
+      epi_sync(c);
+    }
+    float mean[2], m2[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float s1 = 0.f;
+#pragma unroll
+      for (int i = 0; i < N / 8; ++i) s1 += d[4 * i + 2 * h] + d[4 * i + 2 * h + 1];
+      mean[h] = quad_sum(s1) / (float)c.ncols;
+      float s2 = 0.f;
+#pragma unroll
+      for (int i = 0; i < N / 8; ++i) {
+        const float a = d[4 * i + 2 * h] - mean[h], b = d[4 * i + 2 * h + 1] - mean[h];
+        s2 = fmaf(a, a, s2);
+        s2 = fmaf(b, b, s2);
+      }
+      m2[h] = quad_sum(s2);
+    }
+    if (s.pair == 2) {
+      // N-split cluster: the other half of every row is in the peer CTA of the cluster (same M tile,
+      // same iteration).  Lane 0 of each quad writes (mean, M2) of its two rows into the PEER's slots
+      // of this tile parity and arrives (release.cluster) on the peer's mbarrier; it waits on the
+      // local one (acquire.cluster), reads the peer's values for its rows and hands them to its quad.
+      // Both CTAs merge "columns 0..127 first", so they get bit-identical statistics.  Two slots /
+      // barriers alternate by tile parity: the peer can be one publish ahead, never two (its next
+      // publish needs ours, and a lane publishes only after it has read this tile's slots).
+      const int par = c.it & 1;
+      const int r0 = 64 * c.group + 16 * c.q + (lane >> 2);
+      float2* slot = reinterpret_cast<float2*>(c.extra) + par * 128 + r0;
+      uint64_t* xbar = reinterpret_cast<uint64_t*>(c.extra + 2 * 128 * 8) + par;
+      const uint32_t peer = (uint32_t)(c.n_tile ^ 1);
+      float2 o[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+      if ((lane & 3) == 0) {
+        st_cluster_f32x2(slot, peer, mean[0], m2[0]);
+        st_cluster_f32x2(slot + 8, peer, mean[1], m2[1]);
+        mbar_arrive_cluster_release(xbar, peer);
+        mbar_wait_cluster(xbar, (uint32_t)((c.it >> 1) & 1));
+        o[0] = slot[0];
+        o[1] = slot[8];
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        o[h].x = __shfl_sync(0xffffffffu, o[h].x, lane & ~3);
+        o[h].y = __shfl_sync(0xffffffffu, o[h].y, lane & ~3);
+        const float mean_a = c.n_tile == 0 ? mean[h] : o[h].x, m2a = c.n_tile == 0 ? m2[h] : o[h].y;
+        const float mean_b = c.n_tile == 0 ? o[h].x : mean[h], m2b = c.n_tile == 0 ? o[h].y : m2[h];
+        const float delta = mean_b - mean_a;
+        mean[h] = mean_a + delta * 0.5f;                       // both halves have c.ncols columns
+        m2[h] = m2a + m2b + delta * delta * (0.5f * (float)c.ncols);
+      }
+    }
+    float rstd[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) rstd[h] = 1.f / sqrtf(m2[h] / (float)s.n_total + p.eps);
+#pragma unroll
+    for (int j = 0; j < (N + 31) / 32; ++j) {
+      const int col = 32 * j;
+      if (col < c.ncols) {
+        const int nvalid = c.ncols - col;
+        float v[16];
+        frag_slice<N>(d, j, v);
+#pragma unroll
+        for (int ii = 0; ii < 4; ++ii) {
+          const float2 gq = lds64f(c.smem_s + 4 * (col + 8 * ii + c0));
+          const float2 bq = lds64f(c.smem_s + 4 * (256 + col + 8 * ii + c0));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            v[4 * ii + 2 * h] = (v[4 * ii + 2 * h] - mean[h]) * rstd[h] * gq.x + bq.x;
+            v[4 * ii + 2 * h + 1] = (v[4 * ii + 2 * h + 1] - mean[h]) * rstd[h] * gq.y + bq.y;
+          }
+        }
+        if (resid) frag_load_add(c, p.out_lo, v);
+        if (p.out32) frag_store_f32(c, p.out32, s.n_total, c.n0 + col, v, nvalid);
+        if (p.out16) frag_store_h(s, c, p.out16, p.ld, p.out_lo, c.n0 + col, v, nvalid);
+        if (resid && col + 32 < c.ncols) frag_load_issue(c, resid, p.ld, p.out_lo, c.n0 + col + 32, nvalid - 32);
+      }
     }
   }
 };
@@ -1125,41 +1100,106 @@ struct EpiConvUp {
 // Dual-softmax statistics (coarse_matching.py:102-115): per row, over this tile's columns,
 // (max, sum exp) of sim = acc*scale.  Partials [grow][n_tile] are merged by a finalize kernel.
 struct EpiLse {
-  static constexpr int kGroups = OPP_ROW_GROUPS;   // partial slot = kGroups*n_tile + group
+  static constexpr int kGroups = 2;
+  static constexpr bool kFromRegs = true;
   struct Params {
     float* part_m;
     float* part_s;
     float scale;
   };
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    float m = -INFINITY;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
+    const int c0 = 2 * (threadIdx.x & 3);
 #pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (col + j < c.ncols) m = fmaxf(m, v[j] * p.scale);
-    });
-    float sum = 0.f;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    for (int h = 0; h < 2; ++h) {
+      float m = -INFINITY;
 #pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (col + j < c.ncols) sum += fast_exp(v[j] * p.scale - m);
-    });
-    if (c.valid) {
-      // a group that saw no column of a ragged last tile leaves (m = -inf, s = 0): neutral in the merge
-      p.part_m[c.grow * (kGroups * s.n_tiles) + kGroups * c.n_tile + c.group] = m;
-      p.part_s[c.grow * (kGroups * s.n_tiles) + kGroups * c.n_tile + c.group] = sum;
+      for (int i = 0; i < N / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * i + c0 + e < c.ncols) m = fmaxf(m, d[4 * i + 2 * h + e] * p.scale);
+      m = quad_max(m);
+      float sum = 0.f;
+#pragma unroll
+      for (int i = 0; i < N / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * i + c0 + e < c.ncols) sum += fast_exp(d[4 * i + 2 * h + e] * p.scale - m);
+      sum = quad_sum(sum);
+      if ((threadIdx.x & 3) == 0 && ((c.svalid >> h) & 1u)) {
+        p.part_m[c.sgrow[h] * s.n_tiles + c.n_tile] = m;
+        p.part_s[c.sgrow[h] * s.n_tiles + c.n_tile] = sum;
+      }
     }
   }
 };
 
-// conf = softmax_dim1(sim) * softmax_dim2(sim) = exp((2*sim - lse_pt) - lse_px)
-// (coarse_matching.py:115) evaluated per element, optional fp32 store of conf_matrix, and the
-// per-row (max, first argmax) over this tile's columns for the mutual-nearest test
-// (coarse_matching.py:157-165).  `own_is_pt` says whether rows are 3D points (pass A) or
-// query cells (pass B); the expression is evaluated in the same order in both passes.
+// fp32 conf_matrix store of one slice (row stride n_total): staged when rows are 16-byte aligned,
+// else element by element
+__device__ __forceinline__ void conf_store(const GemmShape& s, const EpiCtx& c, float* conf, int col,
+                                           const float (&v)[16]) {
+  if ((s.n_total & 3) == 0) {
+    frag_store_f32(c, conf, (long long)s.n_total, c.n0 + col, v, c.ncols - col);
+    return;
+  }
+  const int c0 = 2 * (threadIdx.x & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (!((c.svalid >> h) & 1u)) continue;
+    float* dst = conf + c.sgrow[h] * (long long)s.n_total + c.n0 + col;
+#pragma unroll
+    for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+        if (col + 8 * ii + c0 + e < c.ncols) dst[8 * ii + c0 + e] = v[4 * ii + 2 * h + e];
+  }
+}
+
+// conf = softmax_dim1(sim) * softmax_dim2(sim) = exp((2*sim - lse_pt) - lse_px) of one slice
+// (coarse_matching.py:115), and the running per-row (max, first argmax) over the tile's columns
+// (coarse_matching.py:157-165): a lane visits its columns in increasing order.  `own_is_pt` says
+// whether rows are 3D points (pass A) or query cells (pass B); the expression is evaluated in the
+// same order in both passes.
+__device__ __forceinline__ void conf_slice(const EpiCtx& c, int col, float scale, const float (&lown)[2],
+                                           bool own_is_pt, float (&v)[16], float (&best)[2], int (&bidx)[2]) {
+  const int c0 = 2 * (threadIdx.x & 3);
+#pragma unroll
+  for (int ii = 0; ii < 4; ++ii)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int cl = col + 8 * ii + c0 + e;
+      const float lo = lds32f(c.smem_s + 4 * (cl & 255));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float x2 = 2.f * (v[4 * ii + 2 * h + e] * scale);
+        const float x = fast_exp(own_is_pt ? (x2 - lown[h]) - lo : (x2 - lo) - lown[h]);
+        v[4 * ii + 2 * h + e] = x;
+        if (cl < c.ncols && x > best[h]) {
+          best[h] = x;
+          bidx[h] = c.n0 + cl;
+        }
+      }
+    }
+}
+// the per-row (max, argmax) of the tile into partial slot [grow][n_tile]
+__device__ __forceinline__ void conf_best_store(const GemmShape& s, const EpiCtx& c, float* part_val, int* part_idx,
+                                                float (&best)[2], int (&bidx)[2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    quad_argmax(best[h], bidx[h]);
+    if ((threadIdx.x & 3) == 0 && ((c.svalid >> h) & 1u)) {
+      part_val[c.sgrow[h] * s.n_tiles + c.n_tile] = best[h];
+      part_idx[c.sgrow[h] * s.n_tiles + c.n_tile] = bidx[h];
+    }
+  }
+}
+
+// conf per element, optional fp32 store of conf_matrix, and the per-row (max, first argmax) over
+// this tile's columns for the mutual-nearest test (the four-pass flow).
 struct EpiConf {
-  static constexpr int kGroups = OPP_ROW_GROUPS;   // partial slot = kGroups*n_tile + group
+  static constexpr int kGroups = 2;
+  static constexpr bool kFromRegs = true;
   struct Params {
     const float* lse_own;    // [batches*rows]
     const float* lse_other;  // [batches][n_total]
@@ -1170,59 +1210,34 @@ struct EpiConf {
     int* part_idx;
   };
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    epi_sync(c);
-    for (int i = c.etid; i < c.ncols; i += 128)
-      sts32f(c.smem_s + 4 * i, p.lse_other[(long long)c.b * s.n_total + c.n0 + i]);
-    epi_sync(c);
-    const float lown = c.valid ? p.lse_own[c.grow] : 0.f;
-    float best = -1.f;
-    int best_idx = c.n0;
-    const bool vec_ok = (s.n_total & 3) == 0;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
+    epi_stage_cols_b(s, c, p.lse_other);
+    float lown[2], best[2] = {-1.f, -1.f};
+    int bidx[2] = {c.n0, c.n0};
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const float x2 = 2.f * (v[j] * p.scale);
-        const float lo = lds32f(c.smem_s + 4 * ((col + j) & 255));
-        const float e = p.own_is_pt ? (x2 - lown) - lo : (x2 - lo) - lown;
-        v[j] = fast_exp(e);
-        if (col + j < c.ncols && v[j] > best) {
-          best = v[j];
-          best_idx = c.n0 + col + j;
-        }
+    for (int h = 0; h < 2; ++h) lown[h] = ((c.svalid >> h) & 1u) ? p.lse_own[c.sgrow[h]] : 0.f;
+#pragma unroll
+    for (int j = 0; j < (N + 31) / 32; ++j) {
+      const int col = 32 * j;
+      if (col < c.ncols) {
+        float v[16];
+        frag_slice<N>(d, j, v);
+        conf_slice(c, col, p.scale, lown, p.own_is_pt != 0, v, best, bidx);
+        if (p.conf) conf_store(s, c, p.conf, col, v);
       }
-#if OPP_CONF_STAGED
-      if (p.conf && vec_ok) {
-        staged_store_f32(c, p.conf, (long long)s.n_total, c.n0 + col, v, c.ncols - col);
-      } else
-#endif
-      if (p.conf && c.valid) {
-        float* dst = p.conf + c.grow * (long long)s.n_total + c.n0 + col;
-        if (vec_ok) {
-          float4* o4 = reinterpret_cast<float4*>(dst);
-#pragma unroll
-          for (int g = 0; g < 8; ++g)
-            if (col + g * 4 < c.ncols)
-              o4[g] = make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (col + j < c.ncols) dst[j] = v[j];
-        }
-      }
-    });
-    if (c.valid) {
-      p.part_val[c.grow * (kGroups * s.n_tiles) + kGroups * c.n_tile + c.group] = best;
-      p.part_idx[c.grow * (kGroups * s.n_tiles) + kGroups * c.n_tile + c.group] = best_idx;
     }
+    conf_best_store(s, c, p.part_val, p.part_idx, best, bidx);
   }
 };
 
 // lse pass with the COLUMN statistics folded in (replaces the second lse pass): rows are 3D points.
-// Row partials as in EpiLse; in addition every warp reduces each column of its 32x32 chunk over
-// its 32 rows with two butterflies (max, then sum of exp(x - column max of these 32 rows)) and
-// writes the pair to  col_m / col_s [batch][row group][n_total]  (row group = 32 rows; coalesced:
-// lane j owns column j).  opp_lse_col_finalize merges the row groups.
+// Row partials as in EpiLse; in addition every warp reduces each column of a 32-column slice over
+// its 16 rows (the column max with an xor butterfly, then the sum of exp(x - that max) with a halving
+// one, after which lane holds column frag_lane_col()), the two warps of a 32-row group merge their
+// (max, sum) through the odd warp's stage (even warp first), and the even warp writes the pair to
+// col_m / col_s [batch][row group][n_total] (row group = 32 rows).  opp_lse_col_finalize merges the
+// row groups.
 struct EpiLseColParams {
   float* part_m;
   float* part_s;
@@ -1235,80 +1250,107 @@ struct EpiLseColParams {
 };
 template <bool kMask>
 struct EpiLseColT {
-  static constexpr int kGroups = OPP_ROW_GROUPS;   // row partial slot = kGroups*n_tile + group
+  static constexpr int kGroups = 2;
+  static constexpr bool kFromRegs = true;
   // With an n64 mainloop in the same kernel, ptxas serialises every wgmma of it (C7514) next to
   // this epilogue's column butterflies; its GEMMs have >= 4096 columns, so tiles of <= 64 columns
   // (tiny inputs only) run at 128
   static constexpr int kMinMmaN = 128;
   using Params = EpiLseColParams;
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    const int lane = threadIdx.x & 31;
-    const int rg = c.m_tile * 4 + c.q;   // 32-row group of this warp inside the batch
-    const bool rg_ok = rg < p.row_groups;
-    const long long cbase = ((long long)c.b * p.row_groups + rg) * s.n_total + c.n0;
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
+    const int lane = threadIdx.x & 31, c0 = 2 * (lane & 3);
     if constexpr (kMask) {   // additive column bias (0 / -1e9) of this tile, shared by the epilogue group
       epi_sync(c);
       for (int i = c.etid; i < c.ncols; i += 128)
         sts32f(c.smem_s + 4 * i, p.col_mask[(long long)c.b * s.n_total + c.n0 + i] ? 0.f : -1e9f);
       epi_sync(c);
     }
-    float m = -INFINITY;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-      float t[32];
+    // sim (+ column bias) in place; -inf for rows outside the tensor and columns past the tile
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
+    for (int i = 0; i < N / 8; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int cl = 8 * i + c0 + e;
         float cb_ = 0.f;
-        if constexpr (kMask) cb_ = lds32f(c.smem_s + 4 * ((col + j) & 255));
-        v[j] = (c.valid && col + j < c.ncols) ? v[j] * p.scale + cb_ : -INFINITY;
-        m = fmaxf(m, v[j]);
-        t[j] = v[j];
+        if constexpr (kMask) cb_ = lds32f(c.smem_s + 4 * (cl & 255));
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          d[4 * i + 2 * h + e] = (((c.svalid >> h) & 1u) && cl < c.ncols) ? d[4 * i + 2 * h + e] * p.scale + cb_
+                                                                          : -INFINITY;
       }
+    // row partials
 #pragma unroll
-      for (int o = 16; o >= 1; o >>= 1) {
-        const bool up = (lane & o) != 0;
+    for (int h = 0; h < 2; ++h) {
+      float m = -INFINITY;
 #pragma unroll
-        for (int k = 0; k < o; ++k) {
-          const float keep = up ? t[o + k] : t[k];
-          const float send = up ? t[k] : t[o + k];
-          t[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, o));
-        }
+      for (int i = 0; i < N / 8; ++i) m = fmaxf(m, fmaxf(d[4 * i + 2 * h], d[4 * i + 2 * h + 1]));
+      m = quad_max(m);
+      float sum = 0.f;
+#pragma unroll
+      for (int i = 0; i < N / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * i + c0 + e < c.ncols) sum += fast_exp(d[4 * i + 2 * h + e] - m);
+      sum = quad_sum(sum);
+      if ((lane & 3) == 0 && ((c.svalid >> h) & 1u)) {
+        p.part_m[c.sgrow[h] * s.n_tiles + c.n_tile] = m;
+        p.part_s[c.sgrow[h] * s.n_tiles + c.n_tile] = sum;
       }
-      const float cm = t[0];   // max of column col + lane over this warp's valid rows (-inf: none)
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const float cmj = __shfl_sync(0xffffffffu, cm, j);
-        t[j] = v[j] == -INFINITY ? 0.f : fast_exp(v[j] - cmj);
-      }
-#pragma unroll
-      for (int o = 16; o >= 1; o >>= 1) {
-        const bool up = (lane & o) != 0;
-#pragma unroll
-        for (int k = 0; k < o; ++k) {
-          const float keep = up ? t[o + k] : t[k];
-          const float send = up ? t[k] : t[o + k];
-          t[k] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-        }
-      }
-      if (rg_ok && col + lane < c.ncols) {
-        p.col_m[cbase + col + lane] = cm;
-        p.col_s[cbase + col + lane] = t[0];
-      }
-    });
-    float sum = 0.f;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (col + j < c.ncols) {
-          float cb_ = 0.f;
-          if constexpr (kMask) cb_ = lds32f(c.smem_s + 4 * ((col + j) & 255));
-          sum += fast_exp((v[j] * p.scale + cb_) - m);
-        }
-    });
-    if (c.valid) {
-      p.part_m[c.grow * (kGroups * s.n_tiles) + kGroups * c.n_tile + c.group] = m;
-      p.part_s[c.grow * (kGroups * s.n_tiles) + kGroups * c.n_tile + c.group] = sum;
     }
+    // column partials of this warp's 16 rows, one slice at a time
+    constexpr int kSlices = (N + 31) / 32;
+    float cmax[kSlices], csum[kSlices];
+    const int rq = lane >> 2;
+#pragma unroll
+    for (int j = 0; j < kSlices; ++j) {
+      cmax[j] = -INFINITY;
+      csum[j] = 0.f;
+      if (32 * j < c.ncols) {
+        float v[16];
+        frag_slice<N>(d, j, v, -INFINITY);
+        float x[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) x[k] = fmaxf(v[4 * (k >> 1) + (k & 1)], v[4 * (k >> 1) + 2 + (k & 1)]);
+        col_allreduce8(x, [](float a, float b) { return fmaxf(a, b); });
+        cmax[j] = pick8(x, rq);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float a = v[4 * (k >> 1) + (k & 1)], b = v[4 * (k >> 1) + 2 + (k & 1)];
+          x[k] = (a == -INFINITY ? 0.f : fast_exp(a - x[k])) + (b == -INFINITY ? 0.f : fast_exp(b - x[k]));
+        }
+        csum[j] = col_reduce8(x, [](float a, float b) { return a + b; });
+      }
+    }
+    // merge the warp pair of the 32-row group: the odd warp hands its partials over in its stage
+    const bool odd = (c.q & 1) != 0;
+    const uint32_t xs = c.wstage_s + (odd ? 0 : kWarpStageBytes);
+    if (odd) {
+#pragma unroll
+      for (int j = 0; j < kSlices; ++j) sts64f(xs + 8 * (32 * j + lane), cmax[j], csum[j]);
+    }
+    pair_sync(c);
+    if (!odd) {
+      const int rg = c.m_tile * 4 + 2 * c.group + (c.q >> 1);   // 32-row group inside the batch
+      if (rg < p.row_groups) {
+        const long long cbase = ((long long)c.b * p.row_groups + rg) * s.n_total + c.n0;
+        const int lc = frag_lane_col();
+#pragma unroll
+        for (int j = 0; j < kSlices; ++j) {
+          const int cl = 32 * j + lc;
+          if (cl < c.ncols) {
+            const float2 o = lds64f(xs + 8 * (32 * j + lane));
+            const float m = fmaxf(cmax[j], o.x);
+            const float sa = cmax[j] == -INFINITY ? 0.f : csum[j] * fast_exp(cmax[j] - m);
+            const float sb = o.x == -INFINITY ? 0.f : o.y * fast_exp(o.x - m);
+            p.col_m[cbase + cl] = m;
+            p.col_s[cbase + cl] = sa + sb;
+          }
+        }
+      }
+    }
+    pair_sync(c);   // the odd warp's stage is free again
   }
 };
 
@@ -1316,14 +1358,16 @@ using EpiLseCol = EpiLseColT<false>;
 using EpiLseColMasked = EpiLseColT<true>;   // + query_image_mask (-1e9 on the padded query cells)
 
 // conf pass with the column maxima folded in (replaces the second conf pass): rows are 3D points,
-// conf is stored as in EpiConf, and for every 32x32 chunk the warp reduces each COLUMN over its 32
-// rows with a butterfly (at offset o a lane keeps one half of its 2o values and exchanges the other
-// half with lane ^ o: 31 shuffles, lane j ends with the maximum of column j) followed by one
-// atomicMax per lane on colmax[b][column] (conf >= 0, so its float bits order like unsigned ints).
-// The mutual-nearest test (coarse_matching.py:157-165) is then  rowmax(i) == colmax(argmax_j(i)),
-// an exact comparison of two copies of the same register value.
+// conf and the row (max, first argmax) as in EpiConf with own_is_pt.  Every warp reduces each
+// column of a slice over its 16 rows with a halving butterfly (lane ends with column
+// frag_lane_col()), the two warps of a 32-row group merge through the odd warp's stage, and the even
+// warp does one atomicMax per column on colmax[b][column] (conf >= 0, so its float bits order like
+// unsigned ints; an integer max, so the result does not depend on the order).  The mutual-nearest
+// test (coarse_matching.py:157-165) is then  rowmax(i) == colmax(argmax_j(i)), an exact comparison
+// of two copies of the same register value.
 struct EpiConfCol {
-  static constexpr int kGroups = OPP_ROW_GROUPS;   // partial slot = kGroups*n_tile + group
+  static constexpr int kGroups = 2;
+  static constexpr bool kFromRegs = true;
   // With an n64 mainloop in the same kernel, ptxas serialises every wgmma of it (C7514) next to
   // this epilogue's column butterfly; its GEMMs have >= 4096 columns, so tiles of <= 64 columns
   // (tiny inputs only) run at 128
@@ -1333,71 +1377,67 @@ struct EpiConfCol {
     const float* lse_other;  // [batches][n_total] (query cells)
     float scale;
     float* conf;             // [batches*rows][n_total] or null
-    float* part_val;         // [batches*rows][kGroups*n_tiles]
+    float* part_val;         // [batches*rows][n_tiles]
     int* part_idx;
     unsigned* colmax;        // [batches][n_total], zero-initialised
   };
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  __device__ static void run(const Params& p, const GemmShape& s, const EpiCtx& c) {
-    epi_sync(c);
-    for (int i = c.etid; i < c.ncols; i += 128)
-      sts32f(c.smem_s + 4 * i, p.lse_other[(long long)c.b * s.n_total + c.n0 + i]);
-    epi_sync(c);
-    const float lown = c.valid ? p.lse_own[c.grow] : 0.f;
-    float best = -1.f;
-    int best_idx = c.n0;
-    const bool vec_ok = (s.n_total & 3) == 0;
+  template <int N>
+  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
     const int lane = threadIdx.x & 31;
-    unsigned* cm = p.colmax + (long long)c.b * s.n_total + c.n0;
-    acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
+    epi_stage_cols_b(s, c, p.lse_other);
+    float lown[2], best[2] = {-1.f, -1.f};
+    int bidx[2] = {c.n0, c.n0};
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const float x2 = 2.f * (v[j] * p.scale);
-        const float lo = lds32f(c.smem_s + 4 * ((col + j) & 255));
-        v[j] = fast_exp((x2 - lown) - lo);   // same expression order as EpiConf with own_is_pt
-        if (col + j < c.ncols && v[j] > best) {
-          best = v[j];
-          best_idx = c.n0 + col + j;
+    for (int h = 0; h < 2; ++h) lown[h] = ((c.svalid >> h) & 1u) ? p.lse_own[c.sgrow[h]] : 0.f;
+    constexpr int kSlices = (N + 31) / 32;
+    float cmax[kSlices];
+#pragma unroll
+    for (int j = 0; j < kSlices; ++j) {
+      const int col = 32 * j;
+      cmax[j] = 0.f;
+      if (col < c.ncols) {
+        float v[16];
+        frag_slice<N>(d, j, v);
+        conf_slice(c, col, p.scale, lown, true, v, best, bidx);
+        if (p.conf) conf_store(s, c, p.conf, col, v);
+        // column maxima over this warp's 16 rows (rows outside the tensor contribute 0)
+        float x[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float a = (c.svalid & 1u) ? v[4 * (k >> 1) + (k & 1)] : 0.f;
+          const float b = (c.svalid & 2u) ? v[4 * (k >> 1) + 2 + (k & 1)] : 0.f;
+          x[k] = fmaxf(a, b);
         }
+        cmax[j] = col_reduce8(x, [](float a, float b) { return fmaxf(a, b); });
       }
-      if (p.conf && vec_ok) {
-        staged_store_f32(c, p.conf, (long long)s.n_total, c.n0 + col, v, c.ncols - col);
-      } else if (p.conf && c.valid) {
-        float* dst = p.conf + c.grow * (long long)s.n_total + c.n0 + col;
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (col + j < c.ncols) dst[j] = v[j];
-      }
-      // column maxima over this warp's 32 rows (rows outside the tensor contribute 0)
-      if (!c.valid) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
-      }
-#pragma unroll
-      for (int o = 16; o >= 1; o >>= 1) {
-        const bool up = (lane & o) != 0;
-#pragma unroll
-        for (int k = 0; k < o; ++k) {
-          const float keep = up ? v[o + k] : v[k];
-          const float send = up ? v[k] : v[o + k];
-          v[k] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, o));
-        }
-      }
-      if (col + lane < c.ncols && v[0] > 0.f) atomicMax(cm + col + lane, __float_as_uint(v[0]));
-    });
-    if (c.valid) {
-      p.part_val[c.grow * (kGroups * s.n_tiles) + kGroups * c.n_tile + c.group] = best;
-      p.part_idx[c.grow * (kGroups * s.n_tiles) + kGroups * c.n_tile + c.group] = best_idx;
     }
+    conf_best_store(s, c, p.part_val, p.part_idx, best, bidx);
+    // merge the warp pair of the 32-row group: the odd warp hands its maxima over in its stage
+    const bool odd = (c.q & 1) != 0;
+    const uint32_t xs = c.wstage_s + (odd ? 0 : kWarpStageBytes);
+    if (odd) {
+#pragma unroll
+      for (int j = 0; j < kSlices; ++j) sts32f(xs + 4 * (32 * j + lane), cmax[j]);
+    }
+    pair_sync(c);
+    if (!odd) {
+      unsigned* cm = p.colmax + (long long)c.b * s.n_total + c.n0;
+      const int lc = frag_lane_col();
+#pragma unroll
+      for (int j = 0; j < kSlices; ++j) {
+        const int cl = 32 * j + lc;
+        const float m = fmaxf(cmax[j], lds32f(xs + 4 * (32 * j + lane)));
+        if (cl < c.ncols && m > 0.f) atomicMax(cm + cl, __float_as_uint(m));
+      }
+    }
+    pair_sync(c);   // the odd warp's stage is free again
   }
 };
 
 // =============================================================================================
 // The kernel
 // =============================================================================================
-__device__ __forceinline__ void sts64f(uint32_t addr, float a, float b) {
-  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
-}
 // keeps the compiler from moving accesses of in-flight wgmma accumulators across the fences
 template <int R>
 __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
@@ -1436,7 +1476,7 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
   const int ring = s.stages * (a_stage + b_stage);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + s.stages * a_stage;
-  // register-fragment epilogues have no accumulator tile (and acc_alias = 0)
+  // register-fragment epilogues have no accumulator tile (and acc_alias = 0); only EpiConvUp has one
   constexpr bool kAccTile = !EpiFromRegs<Epi>::value;
   uint8_t* smem_acc = s.acc_alias ? smem : smem + ring;
   float* epi_smem = reinterpret_cast<float*>(smem + ring + (kAccTile && !s.acc_alias ? gemm_acc_bytes(s.mma_n) : 0));
@@ -1476,11 +1516,11 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
     // acc_alias: one arrival per epilogue warp of every CTA whose ring the producer writes into
     mbar_init(accfree, 4 * Epi::kGroups * csize);
     if constexpr (EpiExtraSmem<Epi>::value > 0) {
-      // EpiLN's DSMEM exchange: the 128 group-0 threads of the peer CTA arrive once per tile
+      // EpiLN's DSMEM exchange: the writer lanes of the peer CTA arrive once per tile
       uint64_t* xbar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi_smem) + epi_smem_bytes<Epi>() -
                                                    EpiExtraSmem<Epi>::value + 2 * 128 * 8);
-      mbar_init(&xbar[0], 128);
-      mbar_init(&xbar[1], 128);
+      mbar_init(&xbar[0], Epi::kExchangeArrivals);
+      mbar_init(&xbar[1], Epi::kExchangeArrivals);
     }
     fence_mbar_init();
   }
@@ -1699,11 +1739,10 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
       c.it = it;
       c.svalid = 0;
       if constexpr (kAccTile) {
-        c.valid = epi_row_info(s, c, lane, c.grow, c.row);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           int rdummy;
-          if (epi_row_info(s, c, (lane >> 2) + 8 * i, c.sgrow[i], rdummy)) c.svalid |= 1u << i;
+          if (epi_row_at(s, c, q * 32 + (lane >> 2) + 8 * i, c.sgrow[i], rdummy)) c.svalid |= 1u << i;
         }
       } else {
         // the two accumulator-fragment rows of this thread
@@ -1802,16 +1841,7 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
       }
 
       if constexpr (kAccTile) {
-        if (s.debug_skip & 32) {   // bit 5: timing experiment, ONLY the accumulator reads of the epilogue
-          float acc_sink = 0.f;
-          acc_foreach32(c.acc, c.ncols, c.col_first, c.col_step, [&](int col, float* v) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc_sink += v[j];
-          });
-          if (acc_sink == 12345.678f) c.smem[0] = acc_sink;
-        } else if (!(s.debug_skip & 4)) {
-          Epi::run(ep, s, c);   // bit 2: timing experiment, no epilogue at all
-        }
+        if (!(s.debug_skip & 4)) Epi::run(ep, s, c);   // bit 2: timing experiment, no epilogue at all
         if (s.acc_alias) {
           // the producer's next TMA writes land where this warp just read the accumulator
           fence_proxy_async_smem();
@@ -1854,9 +1884,8 @@ gemm_kernel_dyn(const __grid_constant__ TensorMaps maps, const GemmShape s_in,
   gemm_body<A_MODE, Epi>(maps, s, ep);
 }
 
-// Shared memory of a launch with epilogue Epi: operand ring, the accumulator tile (token-row
-// epilogues only: beside the ring, or over it when acc_alias), epilogue scratch, barriers and
-// alignment slack.
+// Shared memory of a launch with epilogue Epi: operand ring, the accumulator tile (EpiConvUp only:
+// beside the ring, or over it when acc_alias), epilogue scratch, barriers and alignment slack.
 inline int gemm_stage_bytes(int mma_n, int split) {
   return (kABytes + mma_n * kBlockK * 2) * (split ? 2 : 1);
 }
