@@ -99,8 +99,11 @@ static int map_rows(CUtensorMap* map, const void* ptr, long long k, long long ro
 }
 
 // $OPP_LOG_TILES=1: print every distinct GEMM tile configuration to stderr once, when it is first
-// launched (which wgmma widths, ring depths and clusters a workload actually uses)
-static void log_tile_once(int a_mode, const GemmShape& s) {
+// launched (which wgmma widths, ring depths and clusters a workload actually uses); every field of
+// the line is an integer.  $OPP_LOG_TILES=2: print the configuration of every launch, followed by
+// "epi <name>" (the epilogue), so that each launch of a test is attributed a line of its own even
+// where launches of the same (n, k) differ only in the epilogue.
+static void log_tile_once(int a_mode, const GemmShape& s, const char* epi) {
   static int on = -1;
   if (on < 0) {
     const char* e = getenv("OPP_LOG_TILES");
@@ -115,6 +118,10 @@ static void log_tile_once(int a_mode, const GemmShape& s) {
            a_mode, s.n_total, s.block_n, s.mma_n, s.k_chunks * kBlockK, s.conv_c, s.stages, s.acc_alias,
            s.cluster, s.pair);
   std::lock_guard<std::mutex> lock(mu);
+  if (on == 2) {
+    fprintf(stderr, "opp gemm tile: %s epi %s\n", key, epi);
+    return;
+  }
   for (int i = 0; i < n_seen; ++i)
     if (!strcmp(seen[i], key)) return;
   if (n_seen < 256) strcpy(seen[n_seen++], key);
@@ -143,7 +150,7 @@ static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Param
                 "GEMM tile N=%d (split %d) does not fit in shared memory", s.block_n, s.split);
   }
   const int smem = gemm_smem_bytes<Epi>(s);
-  log_tile_once(A_MODE, s);
+  log_tile_once(A_MODE, s, Epi::kName);
   const void* kern;
   if constexpr (DYN) kern = (const void*)gemm_kernel_dyn<A_MODE, Epi>;
   else kern = (const void*)gemm_kernel<A_MODE, Epi>;

@@ -507,6 +507,7 @@ struct EpiConvParams {
 };
 struct EpiConv {
   static constexpr int kGroups = OPP_CONV_GROUPS;
+  static constexpr const char* kName = "conv";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   using Params = EpiConvParams;
   // Called before the MMAs of the tile: pull this lane's share of the residual rows towards L2
@@ -570,6 +571,7 @@ struct EpiConv {
 // compact window tensor [matches][tile_h + 2][8][C] of a previous A_WIN launch.
 struct EpiWin {
   static constexpr int kGroups = OPP_CONV_GROUPS;
+  static constexpr const char* kName = "conv_win";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   struct Params {
     __half* out;
@@ -638,6 +640,7 @@ struct EpiWin {
 // math and the stores of chunk i.
 struct EpiConvUp {
   static constexpr int kGroups = OPP_CONV_GROUPS;
+  static constexpr const char* kName = "conv_up";   // $OPP_LOG_TILES
   static constexpr bool kNeedsNext = true;   // EpiCtx::next_b / next_m_tile are filled in
   static constexpr int kWarpStage = 2 * 32 * 80;   // hi and lo windows of a chunk side by side
   using Params = EpiConvParams;
@@ -864,6 +867,7 @@ __device__ __forceinline__ void epi_stage_cols_b(const GemmShape& s, const EpiCt
 // Per element exactly the operations of the shared-memory form: the outputs are bit-identical.
 struct EpiStoreF16 {
   static constexpr int kGroups = 2;
+  static constexpr const char* kName = "store_f16";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   struct Params {
     __half* out;
@@ -915,6 +919,7 @@ struct EpiStoreF16 {
 // and a quad sum.
 struct EpiQ {
   static constexpr int kGroups = 2;
+  static constexpr const char* kName = "q";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   struct Params {
     __half* out;
@@ -973,6 +978,7 @@ struct EpiQ {
 // launchers check block_n == mma_n == n, or the 128-column halves of the N-split cluster).
 struct EpiLN {
   static constexpr int kGroups = 2;
+  static constexpr const char* kName = "ln";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   // N-split cluster (GemmShape.pair == 2): 2 x 128 (mean, M2) slots the peer CTA writes into + 2 mbarriers
   static constexpr int kExtraSmem = 2 * 128 * 8 + 64;
@@ -1101,6 +1107,7 @@ struct EpiLN {
 // (max, sum exp) of sim = acc*scale.  Partials [grow][n_tile] are merged by a finalize kernel.
 struct EpiLse {
   static constexpr int kGroups = 2;
+  static constexpr const char* kName = "lse";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   struct Params {
     float* part_m;
@@ -1199,6 +1206,7 @@ __device__ __forceinline__ void conf_best_store(const GemmShape& s, const EpiCtx
 // this tile's columns for the mutual-nearest test (the four-pass flow).
 struct EpiConf {
   static constexpr int kGroups = 2;
+  static constexpr const char* kName = "conf";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   struct Params {
     const float* lse_own;    // [batches*rows]
@@ -1251,6 +1259,7 @@ struct EpiLseColParams {
 template <bool kMask>
 struct EpiLseColT {
   static constexpr int kGroups = 2;
+  static constexpr const char* kName = "lse_col";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   // With an n64 mainloop in the same kernel, ptxas serialises every wgmma of it (C7514) next to
   // this epilogue's column butterflies; its GEMMs have >= 4096 columns, so tiles of <= 64 columns
@@ -1367,6 +1376,7 @@ using EpiLseColMasked = EpiLseColT<true>;   // + query_image_mask (-1e9 on the p
 // of two copies of the same register value.
 struct EpiConfCol {
   static constexpr int kGroups = 2;
+  static constexpr const char* kName = "conf_col";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   // With an n64 mainloop in the same kernel, ptxas serialises every wgmma of it (C7514) next to
   // this epilogue's column butterfly; its GEMMs have >= 4096 columns, so tiles of <= 64 columns

@@ -1040,6 +1040,11 @@ class OnePosePlus_model(_Engine):
                 if qmask is not None:
                     raise NotImplementedError("query_image_mask is not supported in CUDA-graph mode")
                 out, M = self._replay(img, img_scale, bank_raw, fine_on, prologue)
+                if out is None:
+                    # more matches than the captured fine stage holds (exact ties keep every tied row,
+                    # so the count can exceed B * min(N, S)): this call runs eagerly, the graph stays
+                    out, count, cap = self._enqueue(img, img_scale, bank_raw, fine_on, dynamic=False)
+                    M = out.pop("M")
             else:
                 if prologue is not None:
                     prologue.run([t.to(dev) for t in prologue.inputs], img)
@@ -1214,7 +1219,9 @@ class OnePosePlus_model(_Engine):
             img.copy_(s_img)   # the caller's query_image receives what the prologue wrote
         src = ent["out"]
         torch.cuda.current_stream().synchronize()        # the only host sync, after everything is queued
-        M = min(int(ent["count"][0]), src["fcap"])
+        M = int(ent["count"][0])
+        if M > src["fcap"]:
+            return None, M    # the fine stage ran on the first fcap matches only: the caller re-runs eagerly
         pack = src["pack"]
         out = pack.views(pack.buf.clone(), M)    # one copy kernel
         out["sized"] = True

@@ -342,19 +342,23 @@ def _tile_log():
             for line in f.read().decode(errors="replace").splitlines():
                 if line.startswith(TILE_PREFIX):
                     fl = line[len(TILE_PREFIX):].split()
-                    new.append({fl[i]: int(fl[i + 1]) for i in range(0, len(fl) - 1, 2)})
+                    new.append({fl[i]: int(fl[i + 1]) if fl[i] != "epi" else fl[i + 1]
+                                for i in range(0, len(fl) - 1, 2)})
                 else:
                     sys.stderr.write(line + "\n")
             _TILES_SEEN.extend(new)
 
 
-def _launch_tile(new, mode, n, k, conv_c):
+def _launch_tile(new, mode, n, k, conv_c, epi=None):
     """Tile configuration of the one GEMM launch that ran under _tile_log (`new`).  The engine prints a
-    configuration once per process: a launch that printed nothing has the configuration of an earlier
-    one with the same (mode, n, k, conv_c), which must then be unique."""
-    same = lambda t: (t["mode"], t["n"], t["k"], t["conv_c"]) == (mode, n, k, conv_c)   # noqa: E731
+    configuration once per process ($OPP_LOG_TILES=1): a launch that printed nothing has the
+    configuration of an earlier one with the same (mode, n, k, conv_c), which must then be unique.
+    epi: the epilogue name the engine adds to every launch's line at $OPP_LOG_TILES=2 (None: any)."""
+    same = lambda t: ((t["mode"], t["n"], t["k"], t["conv_c"]) == (mode, n, k, conv_c)   # noqa: E731
+                      and epi in (None, t.get("epi")))
     mine = [t for t in new if same(t)] or [t for t in _TILES_SEEN if same(t)]
-    assert len(mine) == 1, f"no unique tile line for mode {mode} n {n} k {k} conv_c {conv_c}: {mine}"
+    mine = list({tuple((f, v) for f, v in t.items() if epi or f != "epi"): t for t in mine}.values())
+    assert len(mine) == 1, f"no unique tile line for mode {mode} n {n} k {k} conv_c {conv_c} epi {epi}: {mine}"
     return mine[0]
 
 
@@ -1208,6 +1212,512 @@ def check_kv_single_plane():
     _close("kv1 mt", _unplanes(mt, 1), ref_mt, 2e-5, 1e-6)
 
 
+# ------------------------------------------------------------ token-row GEMMs at the forward's launches
+# Every token-row GEMM launch of one forward (model.py _src_state / _encoder_layer on the 2D side,
+# S = 4096 cells of a 512x512 image, and on the 3D side, N = 5000 points, incl. the resident-bank forms
+# of layer 1; _fine at ROW_MATCHES matches per image, 26 rows each, with the row count on the host or
+# on the device), run at bench.py's batch 64 and at batch 1.  epi: "act" (EpiStoreF16), "q" (EpiQ),
+# "ln" (EpiLN); rows per image: "S", "N" or "F" (26 per match).  Options: flat (one launch over
+# batch * rows, as the forward passes B * len), out1 (the K'/V rows: split operands, one fp16 output
+# plane), a0_shared, w_batched (one weight per image: the attention state mt), resid, resid_shared,
+# out32 (fp32 output only: the last fine layer), dyn (row count read on the device, = the capacity).
+ROW_S, ROW_N, ROW_MATCHES = 4096, 5000, 1000
+_FINE_GEMMS = [
+    ("fine wqkv",          "act", "F", 128, 0, 384, dict(flat=1, act=2, act_cols=256)),
+    ("fine merge LN",      "ln",  "F", 128, 0, 128, dict(flat=1)),
+    ("fine mlp0",          "act", "F", 128, 128, 256, dict(flat=1, act=1, act_cols=256)),
+    ("fine mlp2 LN",       "ln",  "F", 256, 0, 128, dict(flat=1, resid=1)),
+    ("fine mlp2 LN out32", "ln",  "F", 256, 0, 128, dict(flat=1, resid=1, out32=1)),
+]
+ROW_GEMMS = [
+    # name                     epi    rows k0   k1   n    options
+    ("wkv 2D",                 "act", "S", 256, 0,   512, dict(flat=1, act=2, act_cols=256, out1=1)),
+    ("wkv 3D",                 "act", "N", 256, 0,   512, dict(flat=1, act=2, act_cols=256, out1=1)),
+    ("linear_q 2D",            "q",   "S", 256, 0,   256, {}),
+    ("linear_q 3D",            "q",   "N", 256, 0,   256, {}),
+    ("linear_q 3D x_shared",   "q",   "N", 256, 0,   256, dict(a0_shared=1)),
+    ("merge LN mt 2D",         "ln",  "S", 256, 0,   256, dict(w_batched=1)),
+    ("merge LN mt 3D",         "ln",  "N", 256, 0,   256, dict(w_batched=1)),
+    ("merge LN bank state 2D", "ln",  "S", 256, 0,   256, {}),
+    ("mlp0 2D",                "act", "S", 256, 256, 512, dict(flat=1, act=1, act_cols=512)),
+    ("mlp0 3D",                "act", "N", 256, 256, 512, dict(flat=1, act=1, act_cols=512)),
+    ("mlp0 3D a0_shared",      "act", "N", 256, 256, 512, dict(act=1, act_cols=512, a0_shared=1)),
+    ("mlp2 2D",                "ln",  "S", 512, 0,   256, dict(flat=1, resid=1)),
+    ("mlp2 3D",                "ln",  "N", 512, 0,   256, dict(flat=1, resid=1)),
+    ("mlp2 3D resid_shared",   "ln",  "N", 512, 0,   256, dict(resid=1, resid_shared=1)),
+] + _FINE_GEMMS + [(name + " dyn", e, r, k0, k1, n, dict(o, dyn=1)) for (name, e, r, k0, k1, n, o) in _FINE_GEMMS]
+_EPI_LOG = {"act": "store_f16", "q": "q", "ln": "ln"}
+
+# The tile configuration each launch runs, (block_n, mma_n, cluster, pair, stages), in the fp16x3
+# mode at batch 64 and batch 1 (fp16: block_n, mma_n, cluster and pair are pinned, the ring is deeper).
+# At batch 1 the 2D side (32 M tiles) takes the latency forms: N tiles halved (split_n_for_latency)
+# and the LayerNorm N-split pair cluster; the 3D side (40 M tiles) halves linear_q only, its
+# N = 512 GEMMs already have 80 super tiles.  The fine GEMMs have no latency forms (the device-count
+# launches are sized at capacity, and the host-count ones have hundreds of M tiles).
+_W256, _W128, _Q64, _PAIR = (256, 256, 2, 0, 2), (128, 128, 2, 0, 3), (64, 64, 2, 0, 4), (128, 128, 2, 2, 3)
+ROW_TILES = {
+    **{(name, 64): _W256 for name in ("wkv 2D", "wkv 3D", "linear_q 2D", "linear_q 3D", "linear_q 3D x_shared",
+                                      "merge LN mt 2D", "merge LN mt 3D", "merge LN bank state 2D", "mlp0 2D",
+                                      "mlp0 3D", "mlp0 3D a0_shared", "mlp2 2D", "mlp2 3D", "mlp2 3D resid_shared")},
+    ("wkv 2D", 1): _W128, ("wkv 3D", 1): _W256,
+    ("linear_q 2D", 1): _Q64, ("linear_q 3D", 1): _W128, ("linear_q 3D x_shared", 1): _W128,
+    ("merge LN mt 2D", 1): _PAIR, ("merge LN mt 3D", 1): _PAIR, ("merge LN bank state 2D", 1): _PAIR,
+    ("mlp0 2D", 1): _W128, ("mlp0 3D", 1): _W256, ("mlp0 3D a0_shared", 1): _W256,
+    ("mlp2 2D", 1): _PAIR, ("mlp2 3D", 1): _PAIR, ("mlp2 3D resid_shared", 1): _PAIR,
+    **{(name + dyn, B): (_W256 if name == "fine mlp0" else _W128)
+       for (name, *_) in _FINE_GEMMS for dyn in ("", " dyn") for B in (64, 1)},
+}
+
+
+def _drand(rows, cols, seed, scale=1.0):
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    return torch.randn(rows, cols, device=DEV, generator=g) * scale
+
+
+def _row_inputs(split, spec, B):
+    """operand planes of one ROW_GEMMS launch at batch B (drawn on the device from fixed seeds)"""
+    _, epi, rk, k0, k1, n, o = spec
+    rows = {"S": ROW_S, "N": ROW_N, "F": 26 * ROW_MATCHES}[rk]
+    inp = {"rows": rows,
+           "a0": _planes(_drand((1 if o.get("a0_shared") else B) * rows, k0, 1), split),
+           "a1": _planes(_drand(B * rows, k1, 2), split) if k1 else None,
+           "w": _planes(_drand((B if o.get("w_batched") else 1) * n, k0 + k1, 3, 0.06 if epi == "q" else 0.05),
+                        split)}
+    if epi == "q":
+        inp["ksum"] = _drand(B, 256, 4).abs() * 100 + 50
+    if epi == "ln":
+        inp["gamma"], inp["beta"] = 1 + 0.1 * _drand(1, n, 5)[0], 0.1 * _drand(1, n, 6)[0]
+        if o.get("resid"):
+            inp["res"] = _planes(_drand((1 if o.get("resid_shared") else B) * rows, n, 7), split)
+    return inp
+
+
+def _row_launch(split, spec, B, inp, out, out32=None, count=None, row_mask=None):
+    """the launch of ROW_GEMMS entry `spec` as the forward makes it; count: device row count in
+    matches (26 rows each); the host row count is the capacity then"""
+    _, epi, _, k0, k1, n, o = spec
+    rows = inp["rows"]
+    nb, lr = (1, B * rows) if o.get("flat") else (B, rows)
+    dyn = {} if count is None else {"count": count, "rows_per_count": 26}
+    if epi == "act":
+        ops.linear_act(inp["a0"], inp["a1"], inp["w"], out, lr, o["act"], o["act_cols"], split,
+                       out_split=False if (split and o.get("out1")) else None, batches=nb,
+                       a0_shared=bool(o.get("a0_shared")), row_mask=row_mask, **dyn)
+    elif epi == "q":
+        ops.linear_q(inp["a0"], inp["w"], inp["ksum"], out, B, rows, ROW_S, split,
+                     x_shared=bool(o.get("a0_shared")), row_mask=row_mask)
+    else:
+        w = inp["w"].view(B if o.get("w_batched") else 1, n, -1)
+        ops.linear_ln(inp["a0"], inp["a1"], w, bool(o.get("w_batched")), inp["gamma"], inp["beta"], nb, lr, split,
+                      resid=inp.get("res"), out16=out, out32=out32, resid_shared=bool(o.get("resid_shared")), **dyn)
+    return nb, lr
+
+
+def _row_outputs(split, spec, B, rows):
+    _, _, _, _, _, n, o = spec
+    pl = 1 if (o.get("out1") or not split) else 2
+    out = None if o.get("out32") else torch.full((B * rows, pl * n), float("nan"), device=DEV, dtype=torch.half)
+    out32 = torch.full((B * rows, n), float("nan"), device=DEV) if o.get("out32") else None
+    return out, out32
+
+
+def _row_check(split, spec, B, inp, out, out32, valid_rows=None):
+    """outputs of one ROW_GEMMS launch against fp64 on the values the stored planes represent, a few
+    images at a time; rows from valid_rows on (a device-side count) must still be NaN"""
+    name, epi, _, k0, k1, n, o = spec
+    rows = inp["rows"]
+    K = k0 + k1
+    out1 = split and o.get("out1")
+    if epi == "act":
+        tol = (6e-4, 1e-4) if out1 else _tol(split, (2e-3, 2e-3), (2e-5, 2e-5))
+    elif epi == "q":
+        tol = _tol(split, (2e-3, 1e-4), (2e-5, 1e-6))
+    else:
+        tol = (_tol(split, (1e-3, 2e-3), (2e-5, 2e-5)) if out32 is not None else
+               _tol(split, (2e-3, 3e-3), (2e-5, 2e-5)))
+    t = _Tally(f"{name} split={split} batch {B}", *tol)
+    W = _unplanes(inp["w"], split).double().view(-1, n, K)
+    total = B * rows if valid_rows is None else valid_rows
+    step = _chunk(rows * max(n, K))
+    for b0 in range(0, B, step):
+        b1 = min(B, b0 + step)
+        sl = slice(b0 * rows, b1 * rows)
+        A = _unplanes(inp["a0"] if o.get("a0_shared") else inp["a0"][sl], split).double()
+        if o.get("a0_shared"):
+            A = A.repeat(b1 - b0, 1)
+        if k1:
+            A = torch.cat([A, _unplanes(inp["a1"][sl], split).double()], 1)
+        Wb = W[b0:b1] if o.get("w_batched") else W.expand(b1 - b0, n, K)
+        y = torch.bmm(A.view(b1 - b0, rows, K), Wb.transpose(1, 2)).reshape(-1, n)
+        if epi == "act":
+            y[:, :o["act_cols"]] = (torch.relu if o["act"] == 1 else _elu1)(y[:, :o["act_cols"]])
+            ref = y
+        elif epi == "q":
+            q = _elu1(y).view(b1 - b0, rows, 8, 32)
+            z = 1.0 / (torch.einsum("blhd,bhd->blh", q, inp["ksum"][b0:b1].double().view(-1, 8, 32)) + 1e-6)
+            ref = (q * z[..., None] * ROW_S).reshape(-1, n)
+        else:
+            ref = F.layer_norm(y, (n,), inp["gamma"].double(), inp["beta"].double(), 1e-5)
+            if o.get("resid"):
+                r = _unplanes(inp["res"] if o.get("resid_shared") else inp["res"][sl], split).double()
+                ref = ref + (r.repeat(b1 - b0, 1) if o.get("resid_shared") else r)
+        got = out32[sl] if out32 is not None else (out[sl].float() if out1 else _unplanes(out[sl], split))
+        r0, r1 = b0 * rows, b1 * rows
+        if r0 < total:
+            v = min(r1, total) - r0
+            t.add(got[:v], ref[:v])
+        if r1 > total:
+            assert torch.isnan(got[max(total - r0, 0):]).all(), f"{name}: rows past the device-side count written"
+    t.check()
+
+
+def _row_cluster_tiles(t, batches, m_tiles):
+    if t["pair"]:     # N-split LayerNorm: one 2-CTA cluster per M tile, both column halves
+        sup = batches * m_tiles
+        clusters = min(sup, _lib.load().opp_num_sms() // 2)
+        return sup // clusters, -(-sup // clusters)
+    return _cluster_tiles(t, batches, m_tiles)
+
+
+def _row_gemm(split, spec, B):
+    """one ROW_GEMMS launch at batch B under the tile log: checked against fp64, returns the tile
+    line and (fewest, most) tiles per cluster"""
+    inp = _row_inputs(split, spec, B)
+    out, out32 = _row_outputs(split, spec, B, inp["rows"])
+    count = None
+    if spec[6].get("dyn"):
+        count = torch.tensor([B * ROW_MATCHES], dtype=torch.int32, device=DEV)
+    with _tile_log() as new:
+        nb, lr = _row_launch(split, spec, B, inp, out, out32, count=count)
+        torch.cuda.synchronize()
+    t = _launch_tile(new, 0, spec[5], spec[3] + spec[4], 0, _EPI_LOG[spec[1]])
+    _row_check(split, spec, B, inp, out, out32)
+    return t, _row_cluster_tiles(t, nb, -(-lr // 128))
+
+
+def _row_layers(split):
+    failed = []
+    for spec in ROW_GEMMS:
+        name = spec[0]
+        for B in (64, 1):
+            try:
+                t, (lo, hi) = _row_gemm(split, spec, B)
+                got = (t["block_n"], t["mma_n"], t["cluster"], t["pair"], t["stages"])
+                print(f"  {name} batch {B}: block_n {got[0]} mma_n {got[1]} cluster {got[2]} pair {got[3]} "
+                      f"stages {got[4]} tiles per cluster {lo}-{hi}")
+                want = ROW_TILES.get((name, B))
+                assert want is not None, f"{name} batch {B}: no pinned tile configuration"
+                if split:
+                    assert got == want, f"{name} batch {B}: tile {got}, expected {want}"
+                else:
+                    assert got[:4] == want[:4], f"{name} batch {B}: tile {got[:4]}, expected {want[:4]}"
+                if B == 64:
+                    assert hi >= 8, f"{name}: only {hi} tiles per cluster at batch 64"
+            except AssertionError as e:   # go on: which launches fail locates a defect
+                print(f"  {name} batch {B}: FAILED: {e}")
+                failed.append(f"{name} batch {B}")
+            torch.cuda.empty_cache()
+    assert not failed, f"split={split}: {failed}"
+
+
+def check_row_gemms():
+    """The token-row GEMMs at the forward's launch configurations against fp64 (ROW_GEMMS), in both
+    operand modes; the tile log shows which configuration each one ran."""
+    for split in (1, 0):
+        _run_child(f"row_gemms_split{split}", OPP_LOG_TILES="2")
+
+
+# row_launch_invariance: EpiStoreF16 and EpiQ compute an element from its own accumulator and (EpiQ)
+# the 32-column head it lies in, so the N tile width (64, 128, 256 columns: the latency split and
+# $OPP_NSPLIT=0) and the batch of the launch must not change its bits.  EpiLN merges the statistics
+# of a row across the two CTAs of the N-split cluster in another order than within one CTA: the pair
+# form is compared with fp64 only (row_gemms at batch 1).
+ROW_VARIANTS = {"default": {}, "nsplit0": {"OPP_NSPLIT": "0"}}
+
+
+def _row_variant(tag):
+    """fixed launches under this process's knobs; image-0 rows saved to $KERNEL_CHECK_DIR/<tag>.pt with
+    the N tile width each ran"""
+    saved = {}
+    q_spec, kv_spec = ROW_GEMMS[2], ("kv", "act", "S", 256, 0, 512, dict(flat=1, act=2, act_cols=256))
+    for split in (1, 0):
+        # EpiQ: image 0 alone and inside a batch of 2 (default: 64- and 128-column tiles)
+        inp2 = _row_inputs(split, q_spec, 2)    # drawn once at batch 2: image 0 is the same in both launches
+        for B in ((1, 2) if tag == "default" else (1,)):
+            inp = dict(inp2, a0=inp2["a0"][:B * ROW_S].contiguous(), ksum=inp2["ksum"][:B].contiguous())
+            out, _ = _row_outputs(split, q_spec, B, ROW_S)
+            with _tile_log() as new:
+                _row_launch(split, q_spec, B, inp, out)
+                torch.cuda.synchronize()
+            t = _launch_tile(new, 0, 256, 256, 0, "q")
+            saved[f"q split={split} batch {B}"] = (t["block_n"], out[:ROW_S].cpu())
+        # EpiStoreF16 (K'/V rows with both planes): 4096 rows, and their first 1024 alone
+        for rows in ((ROW_S, 1024) if tag == "default" else (ROW_S,)):
+            inp = _row_inputs(split, kv_spec, 1)
+            inp["rows"] = rows
+            inp["a0"] = inp["a0"][:rows].contiguous()
+            out, _ = _row_outputs(split, kv_spec, 1, rows)
+            with _tile_log() as new:
+                _row_launch(split, kv_spec, 1, inp, out)
+                torch.cuda.synchronize()
+            t = _launch_tile(new, 0, 512, 256, 0, "store_f16")
+            saved[f"kv split={split} rows {rows}"] = (t["block_n"], out[:1024].cpu())
+    for k, (bn, _) in saved.items():
+        print(f"  [{tag}] {k}: block_n {bn}")
+    torch.save(saved, os.path.join(os.environ["KERNEL_CHECK_DIR"], f"{tag}.pt"))
+
+
+def _row_batch_slices():
+    """Each image of a batch-64 linear_q against a batch-1 launch of the same image, both with
+    256-column tiles ($OPP_NSPLIT=0 keeps the batch-1 tile whole), and each 4-image slice of a batch-64
+    merge LayerNorm with one state mt per image (w_batched) against a batch-4 launch of those images
+    (whole-row tiles in both; batch 1 would take the N-split cluster)."""
+    differ = []
+    for split in (1, 0):
+        for spec, step, tag in ((ROW_GEMMS[2], 1, "q"), (ROW_GEMMS[5], 4, "ln")):
+            B = 64
+            inp = _row_inputs(split, spec, B)
+            out, _ = _row_outputs(split, spec, B, ROW_S)
+            with _tile_log() as new:
+                _row_launch(split, spec, B, inp, out)
+                torch.cuda.synchronize()
+            t64 = _launch_tile(new, 0, 256, 256, 0, tag)
+            assert not torch.isnan(out.float()).any(), f"{spec[0]} batch 64: NaN (unwritten) outputs"
+            pl = out.shape[1] // 256
+            for b0 in range(0, B, step):
+                sl = slice(b0 * ROW_S, (b0 + step) * ROW_S)
+                part = {"rows": ROW_S, "a0": inp["a0"][sl].contiguous(), "a1": None,
+                        "w": inp["w"].view(B, 256, -1)[b0:b0 + step].contiguous() if tag == "ln" else inp["w"]}
+                for k in ("ksum", "gamma", "beta"):
+                    if k in inp:
+                        part[k] = inp[k][b0:b0 + step].contiguous() if k == "ksum" else inp[k]
+                o = torch.full((step * ROW_S, pl * 256), float("nan"), device=DEV, dtype=torch.half)
+                with _tile_log() as new:
+                    _row_launch(split, spec, step, part, o)
+                    torch.cuda.synchronize()
+                t = _launch_tile(new, 0, 256, 256, 0, tag)
+                assert (t["block_n"], t["pair"]) == (t64["block_n"], t64["pair"]) == (256, 0), (t, t64)
+                if not _bits_equal(o, out[sl]):
+                    differ.append(f"{spec[0]} split={split} images {b0}-{b0 + step - 1}: "
+                                  f"{int((o != out[sl]).sum())} elements")
+            print(f"  {spec[0]} split={split}: batch 64 (block_n {t64['block_n']}) against batch-{step} launches")
+    assert not differ, f"batch-64 launches differ from smaller launches of the same images: {differ}"
+
+
+def check_row_launch_invariance():
+    with tempfile.TemporaryDirectory() as d:
+        for tag, env in ROW_VARIANTS.items():
+            _run_child(f"row_variant_{tag}", OPP_LOG_TILES="2", KERNEL_CHECK_DIR=d, **env)
+        saved = {tag: torch.load(os.path.join(d, f"{tag}.pt")) for tag in ROW_VARIANTS}
+    differ = []
+    for kind in ("q split=1", "q split=0", "kv split=1", "kv split=0"):
+        runs = [(f"{tag} {k}", bn, t) for tag, s in saved.items() for k, (bn, t) in s.items() if k.startswith(kind)]
+        widths = sorted({bn for _, bn, _ in runs})
+        print(f"  {kind}: N tile widths {widths}")
+        assert widths == [64, 128, 256], f"{kind}: the variants ran N tiles of {widths}, expected 64, 128 and 256"
+        for what, bn, t in runs[1:]:
+            if not _bits_equal(t, runs[0][2]):
+                differ.append(f"{what} (block_n {bn}) vs {runs[0][0]}: {int((t != runs[0][2]).sum())} elements")
+    _run_child("row_batch_slices", OPP_LOG_TILES="2", OPP_NSPLIT="0")
+    assert not differ, f"token-row outputs depend on the N tile width: {differ}"
+
+
+# ------------------------------------------------------------------ device-side row counts (fine stage)
+def check_row_dyn():
+    """The fine stage launched at capacity with the match count on the device (CUDA-graph path):
+    opp_linear_act_f16_dyn / opp_linear_ln_dyn (26 rows per match) and fine_gather / fine_attention /
+    fine_match, at counts 0, 1, a ragged last 128-row tile, the capacity and past it (clamped).  Rows
+    below count * 26 against fp64 (GEMMs) and bit-identical to the launch with the row count on the
+    host; rows past it untouched (NaN)."""
+    cap = 150
+    for split in (1, 0):
+        pl = 2 if split else 1
+        for spec in _FINE_GEMMS:
+            inp = _row_inputs(split, spec, 1)
+            inp["rows"] = 26 * cap
+            for k in ("a0", "a1", "res"):
+                if inp.get(k) is not None:
+                    inp[k] = inp[k][:26 * cap].contiguous()
+            for c in (0, 1, 37, cap, cap + 5):
+                m = min(c, cap)
+                out, out32 = _row_outputs(split, spec, 1, 26 * cap)
+                _row_launch(split, spec, 1, inp, out, out32, count=torch.tensor([c], dtype=torch.int32, device=DEV))
+                torch.cuda.synchronize()
+                _row_check(split, spec, 1, inp, out, out32, valid_rows=26 * m)
+                if m:
+                    host = {"rows": 26 * m, **{k: (v[:26 * m].contiguous() if k in ("a0", "a1", "res") and
+                                                   v is not None else v) for k, v in inp.items() if k != "rows"}}
+                    ho, ho32 = _row_outputs(split, spec, 1, 26 * m)
+                    _row_launch(split, spec, 1, host, ho, ho32)
+                    torch.cuda.synchronize()
+                    got, want = (out32[:26 * m], ho32) if out32 is not None else (out[:26 * m], ho)
+                    assert torch.equal(got.view(torch.int16), want.view(torch.int16)), \
+                        f"{spec[0]} split={split} count {c}: device-count launch differs from the host-count launch"
+        # fine_gather / fine_attention / fine_match
+        B, hf, wf, N, wc = 2, 64, 80, 500, 20
+        fine = _planes(_rand(B, hf, wf, 128, seed=1), split)
+        desc = _rand(B, 128, N, seed=2)
+        g = torch.Generator().manual_seed(1)
+        b_ids = torch.randint(0, B, (cap,), generator=g).sort().values.to(DEV)
+        i_ids = torch.randint(0, N, (cap,), generator=g).to(DEV)
+        j_ids = torch.randint(0, (hf // 4) * wc, (cap,), generator=g).to(DEV)
+        qkv = _planes(torch.cat([_rand(cap * 26, 256, seed=3).abs() + 0.05, _rand(cap * 26, 128, seed=4)], 1), split)
+        xf = _rand(cap * 26, 128, seed=5)
+        mkc = torch.rand(cap, 2, device=DEV) * 300
+        scale = torch.rand(B, 2, device=DEV) + 0.5
+
+        def run(m, count):
+            o = {"x32": torch.full((m * 26, 128), float("nan"), device=DEV),
+                 "x16": torch.full((m * 26, pl * 128), float("nan"), device=DEV, dtype=torch.half),
+                 "msg": torch.full((m * 26, pl * 128), float("nan"), device=DEV, dtype=torch.half),
+                 "ef": torch.full((m, 3), float("nan"), device=DEV),
+                 "mf": torch.full((m, 2), float("nan"), device=DEV)}
+            ops.fine_gather(fine, desc, b_ids, i_ids, j_ids, o["x32"], o["x16"], m, hf, wf, wc, 4, N, split,
+                            count=count)
+            ops.fine_attention(qkv, o["msg"], m, 1, split, count=count)
+            ops.fine_match(xf, mkc, b_ids, scale, o["ef"], o["mf"], m, 2.0, count=count)
+            torch.cuda.synchronize()
+            return o
+
+        for c in (0, 1, 37, cap, cap + 5):
+            m = min(c, cap)
+            got = run(cap, torch.tensor([c], dtype=torch.int32, device=DEV))
+            host = run(m, None) if m else None
+            for k, v in got.items():
+                per = 26 if v.shape[0] == 26 * cap else 1
+                assert torch.isnan(v[per * m:].float()).all(), f"fine {k} split={split} count {c}: rows past the count"
+                if m:
+                    assert torch.equal(v[:per * m].view(torch.int16) if v.dtype == torch.half else v[:per * m],
+                                       host[k].view(torch.int16) if v.dtype == torch.half else host[k]), \
+                        f"fine {k} split={split} count {c}: device-count launch differs from the host-count launch"
+        print(f"  fine_gather / fine_attention / fine_match split={split}: counts 0, 1, 37, {cap}, {cap + 5}")
+
+
+# --------------------------------------------------------------------------------- masks, colmax selection
+def check_row_masks():
+    """row_mask (query_image_mask) on the K'/V rows (opp_linear_act_f16_b, _out1) and on linear_q (also
+    with the 3D tokens shared): masked rows exactly zero, every other row bit-identical to the launch
+    without a mask."""
+    B = 3
+    g = torch.Generator().manual_seed(9)
+    mask = (torch.rand(B * ROW_S, generator=g) > 0.3).to(torch.uint8).to(DEV)
+    mask[ROW_S:2 * ROW_S] = 0          # one image fully padded
+    kv_spec = ("kv", "act", "S", 256, 0, 512, dict(flat=1, act=2, act_cols=256))
+    for split in (1, 0):
+        cases = [("linear_act_b", kv_spec), ("linear_q", ROW_GEMMS[2]), ("linear_q x_shared", ROW_GEMMS[4])]
+        if split:
+            cases.insert(1, ("linear_act_out1", ROW_GEMMS[0]))
+        for what, spec in cases:
+            spec = (spec[0], spec[1], "S") + spec[3:]
+            inp = _row_inputs(split, spec, B)
+            outs = []
+            for rm in (None, mask):
+                out, _ = _row_outputs(split, spec, B, ROW_S)
+                if spec[1] == "act":     # the forward's masked form: batches = 1 over B * S rows
+                    ops.linear_act(inp["a0"], None, inp["w"], out, B * ROW_S, 2, 256, split,
+                                   out_split=False if what == "linear_act_out1" else None, row_mask=rm)
+                else:
+                    _row_launch(split, spec, B, inp, out, row_mask=rm)
+                outs.append(out)
+            torch.cuda.synchronize()
+            keep = mask.bool()
+            assert not torch.isnan(outs[1].float()).any(), f"{what} split={split}: unwritten rows"
+            assert (outs[1][~keep].view(torch.int16) == 0).all(), f"{what} split={split}: masked rows not zero"
+            assert _bits_equal(outs[1][keep], outs[0][keep]), f"{what} split={split}: unmasked rows changed"
+            print(f"  {what} split={split}: {int((~keep).sum())} masked rows zero, the others unchanged")
+
+
+SCALE_COARSE = 1.0 / (256 * 0.0801)
+
+
+def check_sim_col_mask():
+    """col_mask (query_image_mask) in sim_lse_cols / lse_col_finalize and the conf pass against
+    softmax(sim - 1e9 [masked columns], 1) * softmax(., 2) in fp64 (coarse_matching.py:108-115):
+    lse_cols = +inf and conf exactly 0 in masked columns.  Image 0: a random mask with a whole
+    256-column tile masked; image 1: a single valid column; L = 1000 (a ragged last 32-row group)."""
+    B, L, S, K = 2, 1000, 700, 256
+    for split in (1, 0):
+        af, bf = _rand(B, L, K, scale=0.9, seed=1), _rand(B, S, K, scale=0.9, seed=2)
+        a, b = _planes(af, split), _planes(bf, split)
+        g = torch.Generator().manual_seed(4)
+        cm = (torch.rand(B, S, generator=g) > 0.4).to(torch.uint8)
+        cm[0, 256:512] = 0
+        cm[1] = 0
+        cm[1, 333] = 1
+        cm = cm.to(DEV)
+        ts, groups = ops.sim_tiles(S), (L + 31) // 32
+        lse_rows, lse_cols = torch.full((B, L), float("nan"), device=DEV), torch.full((B, S), float("nan"), device=DEV)
+        ops.sim_lse_cols(a, b, B, L, S, K, SCALE_COARSE, torch.empty(B * L, ts, device=DEV),
+                         torch.empty(B * L, ts, device=DEV), lse_rows, torch.empty(B, groups, S, device=DEV),
+                         torch.empty(B, groups, S, device=DEV), lse_cols, split, col_mask=cm)
+        conf = torch.full((B, L, S), float("nan"), device=DEV)
+        bv, bi = torch.empty(B, L, device=DEV), torch.empty(B, L, device=DEV, dtype=torch.int32)
+        colmax = torch.full((B, S), -1, device=DEV, dtype=torch.int32)
+        ops.sim_conf_colmax(a, b, lse_rows, lse_cols, conf, B, L, S, K, SCALE_COARSE, torch.empty(B * L, ts, device=DEV),
+                            torch.empty(B * L, ts, device=DEV, dtype=torch.int32), bv, bi, colmax, split)
+        torch.cuda.synchronize()
+        sim = torch.einsum("blk,bsk->bls", _q(af, split).double(), _q(bf, split).double()) * SCALE_COARSE
+        sim = sim - 1e9 * (cm == 0).double()[:, None, :]
+        masked = (cm == 0)
+        assert torch.isinf(lse_cols[masked]).all() and (lse_cols[masked] > 0).all(), "masked columns: lse_cols != +inf"
+        _close(f"col_mask split={split} lse_rows", lse_rows, torch.logsumexp(sim, 2).float(), 1e-5, 1e-4)
+        _close(f"col_mask split={split} lse_cols", lse_cols[~masked], torch.logsumexp(sim, 1).float()[~masked],
+               1e-5, 1e-4)
+        assert (conf.transpose(1, 2)[masked] == 0).all(), "masked columns: conf is not exactly 0"
+        _close(f"col_mask split={split} conf", conf, (torch.softmax(sim, 1) * torch.softmax(sim, 2)).float(),
+               5e-4, 1e-7)
+        assert torch.equal(colmax, conf.max(1).values.view(torch.int32)), "column maxima under the mask"
+        assert (bi[1].long() == 333).all(), "image 1: every row's best column is its one valid column"
+
+
+
+def check_match_select_colmax():
+    """opp_match_select_colmax (value-based mutual test against the column maxima) on planted conf maps
+    against the reference's mask expression (coarse_matching.py:142-172): exact ties keep every tied
+    row, the keypoints are one shared [1, N, 3] bank (bank_shared) or one per image."""
+    B, L, hc, wc = 3, 2500, 20, 24
+    S = hc * wc
+    g = torch.Generator().manual_seed(0)
+    conf = torch.rand(B, L, S, generator=g) * 0.3
+    for b in range(B):
+        cols = torch.randperm(S, generator=g)[:200]
+        rows = torch.randperm(L, generator=g)[:200]
+        conf[b, rows, cols] = 0.5 + 0.5 * torch.rand(200, generator=g)
+        # ties: rows 0-29 of the planted ones copied into 30 other rows (same row maxima, tied columns)
+        twins = torch.tensor([r for r in torch.randperm(L, generator=g).tolist() if r not in set(rows.tolist())][:30])
+        conf[b, twins] = conf[b, rows[:30]]
+    conf = conf.to(DEV)
+    pt_val, pt_idx = conf.max(2)
+    colmax = conf.max(1).values.contiguous().view(torch.int32)
+    scale = torch.rand(B, 2, device=DEV) + 0.5
+    for shared in (True, False):
+        kpts = torch.rand(1 if shared else B, L, 3, device=DEV)
+        cap = B * L
+        outs = [torch.full((cap,), -1, device=DEV, dtype=torch.int64) for _ in range(3)]
+        mconf, mk3, mkc = torch.empty(cap, device=DEV), torch.empty(cap, 3, device=DEV), torch.empty(cap, 2, device=DEV)
+        cnt = torch.zeros(1, device=DEV, dtype=torch.int32)
+        ops.match_select_colmax(pt_val.contiguous(), pt_idx.int().contiguous(), colmax, kpts, scale, B, L, hc, wc,
+                                0.4, 2, 8.0, torch.empty((B * L + 1023) // 1024 + 2, device=DEV, dtype=torch.int32),
+                                *outs, mconf, mk3, mkc, cnt, bank_shared=shared)
+        torch.cuda.synchronize()
+        M = int(cnt.item())
+        mask = (conf > 0.4).view(B, L, hc, wc).clone()
+        mask[:, :, :2] = False
+        mask[:, :, :, :2] = False
+        mask = mask.view(B, L, S) * (conf == conf.max(2, keepdim=True)[0]) * (conf == conf.max(1, keepdim=True)[0])
+        mv, aj = mask.max(2)
+        rb, ri = torch.where(mv)
+        rj = aj[rb, ri]
+        tied = int((torch.bincount(rb * S + rj) > 1).sum())
+        print(f"  match_select_colmax bank_shared={shared}: M={M} ref={len(rb)}, {tied} columns matched by tied rows")
+        assert M == len(rb) and M > 100 and tied >= 10, (M, len(rb), tied)
+        assert torch.equal(outs[0][:M], rb) and torch.equal(outs[1][:M], ri) and torch.equal(outs[2][:M], rj)
+        assert torch.equal(mconf[:M], conf[rb, ri, rj])
+        assert torch.equal(mk3[:M], kpts[0, ri] if shared else kpts[rb, ri])
+        _close("match_select_colmax mkpts_c", mkc[:M], torch.stack([rj % wc, rj // wc], 1) * (8.0 * scale[rb][:, [1, 0]]),
+               1e-6, 1e-5)
+
+
 CHECKS = {
     "linear_act": check_linear_act,
     "linear_ln": check_linear_ln,
@@ -1230,6 +1740,12 @@ CHECKS = {
     "sim_colmax": check_sim_colmax,
     "sim_lse_cols": check_sim_lse_cols,
     "kv_single_plane": check_kv_single_plane,
+    "row_gemms": check_row_gemms,
+    "row_launch_invariance": check_row_launch_invariance,
+    "row_dyn": check_row_dyn,
+    "row_masks": check_row_masks,
+    "sim_col_mask": check_sim_col_mask,
+    "match_select_colmax": check_match_select_colmax,
 }
 
 
@@ -1239,7 +1755,11 @@ CHILD_CHECKS = {"conv_up": _conv_up_cases,
                 "conv_layers_split0": functools.partial(_conv_layers, 0),
                 "conv_batch_slices": _conv_batch_slices,
                 "conv_win_production_tiles": _conv_win_production,
-                **{f"conv_variant_{tag}": functools.partial(_conv_variant, tag) for tag in INVARIANCE_VARIANTS}}
+                **{f"conv_variant_{tag}": functools.partial(_conv_variant, tag) for tag in INVARIANCE_VARIANTS},
+                "row_gemms_split1": functools.partial(_row_layers, 1),
+                "row_gemms_split0": functools.partial(_row_layers, 0),
+                "row_batch_slices": _row_batch_slices,
+                **{f"row_variant_{tag}": functools.partial(_row_variant, tag) for tag in ROW_VARIANTS}}
 assert not CHECKS.keys() & CHILD_CHECKS.keys(), "`--one name` must name one function"
 
 
