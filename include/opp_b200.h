@@ -228,6 +228,20 @@ int opp_sim_conf_colmax(const void* a, const void* b, const float* lse_own, cons
                         float* conf, float* part_val, int* part_idx, unsigned* colmax, int batches,
                         int rows, int cols, int k, float scale, int split, opp_stream_t stream);
 
+/* Bank sets (several objects in one forward, rows = the 3D points of each frame's object padded to
+ * a common count): the two calls above with row_count int32 [B] (or NULL = the calls above).
+ * Rows l >= row_count[b] are not rows of the matrix: they drop out of the column statistics and of
+ * colmax, and conf stores 0 for them.  Their row partials (part_m / part_s, part_val / part_idx) are
+ * not meaningful.  A 32-row group with no row below the count leaves (col_m, col_s) = (-inf, 0),
+ * which opp_lse_col_finalize skips.  col_mask and row_count cannot be combined. */
+int opp_sim_lse_cols_rows(const void* a, const void* b, float* part_m, float* part_s, float* col_m,
+                          float* col_s, int batches, int rows, int cols, int k, float scale, int split,
+                          const unsigned char* col_mask, const int* row_count, opp_stream_t stream);
+int opp_sim_conf_colmax_rows(const void* a, const void* b, const float* lse_own, const float* lse_other,
+                             float* conf, float* part_val, int* part_idx, unsigned* colmax, int batches,
+                             int rows, int cols, int k, float scale, int split, const int* row_count,
+                             opp_stream_t stream);
+
 /* best[r] = max over tiles (ties -> lowest index) */
 int opp_best_finalize(const float* part_val, const int* part_idx, float* best_val, int* best_idx,
                       long long rows, int tiles, opp_stream_t stream);
@@ -256,6 +270,16 @@ int opp_match_select_colmax(const float* pt_val, const int* pt_idx, const unsign
                             float* mkpts3d, float* mkpts_c, int* count_out, int bank_shared,
                             opp_stream_t stream);
 
+/* opp_match_select_colmax for a bank set: kpts fp32 [K][l][3] is read at bank_of_batch[b] (int32 [B],
+ * entries in [0, K)), and rows i >= row_count[b] (int32 [B]) never match.  Both NULL = the call
+ * above; one without the other is an error.  The capacity stays batch*l. */
+int opp_match_select_colmax_set(const float* pt_val, const int* pt_idx, const unsigned* colmax,
+                                const float* kpts, const float* img_scale, int batch, int l, int hc,
+                                int wc, float thr, int border, float cell, int* scratch,
+                                long long* b_ids, long long* i_ids, long long* j_ids, float* mconf,
+                                float* mkpts3d, float* mkpts_c, int* count_out, int bank_shared,
+                                const int* bank_of_batch, const int* row_count, opp_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Fine level — FinePreprocess (loftr_module/fine_preprocess.py:32-55), loftr_fine,
  * FineMatching (utils/fine_matching.py:28-110)
@@ -278,6 +302,13 @@ int opp_fine_gather(const void* fine, const float* desc3d, const long long* b_id
                     const long long* i_ids, const long long* j_ids, float* x32, void* x16, int m,
                     int hf, int wf, int wc, int stride, int n, int split, int bank_shared,
                     int windows, const int* count_dev, opp_stream_t stream);
+
+/* opp_fine_gather for a bank set: desc3d fp32 [K][128][n] is read at bank_of_batch[b] (int32 [B]);
+ * NULL = the call above. */
+int opp_fine_gather_set(const void* fine, const float* desc3d, const long long* b_ids,
+                        const long long* i_ids, const long long* j_ids, float* x32, void* x16, int m,
+                        int hf, int wf, int wc, int stride, int n, int split, int bank_shared,
+                        int windows, const int* count_dev, const int* bank_of_batch, opp_stream_t stream);
 
 /* Linear attention for the 1 + 25 tokens of each match (linear_attention.py:29-61 with
  * L,S in {1,25}).  qkv fp16 [26 M][planes*384] = (elu(q)+1 | elu(k)+1 | v), 8 heads of 16.

@@ -46,6 +46,10 @@ SIGNATURES = {
     "opp_match_select": [P, P, P, P, P, I, I, I, I, F, I, F, P, P, P, P, P, P, P, P, I, P],
     "opp_match_select_colmax": [P, P, P, P, P, I, I, I, I, F, I, F, P, P, P, P, P, P, P, P, I, P],
     "opp_fine_gather": [P, P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, P, P],
+    "opp_sim_lse_cols_rows": [P, P, P, P, P, P, I, I, I, I, F, I, P, P, P],
+    "opp_sim_conf_colmax_rows": [P, P, P, P, P, P, P, P, I, I, I, I, F, I, P, P],
+    "opp_match_select_colmax_set": [P, P, P, P, P, I, I, I, I, F, I, F, P, P, P, P, P, P, P, P, I, P, P, P],
+    "opp_fine_gather_set": [P, P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, P, P, P],
     "opp_conv_win": [P, P, P, P, P, P, I, P, I, I, I, I, I, I, I, I, I, I, F, I, P],
     "opp_fine_attention": [P, P, I, I, F, I, P, P],
     "opp_fine_match": [P, P, P, P, P, P, I, F, P, P],
@@ -104,7 +108,8 @@ def stream():
 
 
 # kernels launched per entry point (bench.py reports the per-step total as gpu_launches)
-KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_pose_metrics": 3,
+KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_match_select_colmax_set": 3,
+                    "opp_pose_metrics": 3,
                     "opp_coarse_focal_stats": 2, "opp_coarse_focal_fwd": 3, "opp_coarse_focal_bwd": 2}
 LAUNCHES = 0
 _PROFILE = None

@@ -617,23 +617,36 @@ int opp_sim_conf(const void* a, const void* b, const float* lse_own, const float
   return launch<A_ROWS, EpiConf>(maps, s, ep, (cudaStream_t)stream);
 }
 
-int opp_sim_lse_cols(const void* a, const void* b, float* part_m, float* part_s, float* col_m,
-                     float* col_s, int batches, int rows, int cols, int k, float scale, int split,
-                     const unsigned char* col_mask, opp_stream_t stream) {
+int opp_sim_lse_cols_rows(const void* a, const void* b, float* part_m, float* part_s, float* col_m,
+                          float* col_s, int batches, int rows, int cols, int k, float scale, int split,
+                          const unsigned char* col_mask, const int* row_count, opp_stream_t stream) {
   TensorMaps maps;
   GemmShape s;
   int rc = setup_rows(maps, s, a, k, nullptr, 0, b, 1, batches, rows, cols, split, 1, 0, 0,
                       EpiLseCol::kMinMmaN);
   if (rc) return rc;
   OPP_REQUIRE(part_m && part_s && col_m && col_s, "null pointer");
+  OPP_REQUIRE(!(col_mask && row_count), "col_mask and row_count are not combined");
   EpiLseColParams ep{part_m, part_s, scale, col_m, col_s, (rows + 31) / 32, col_mask};
+  if (row_count) {
+    EpiLseColRowsParams epr{ep, row_count};
+    return launch<A_ROWS, EpiLseColRows>(maps, s, epr, (cudaStream_t)stream);
+  }
   if (col_mask) return launch<A_ROWS, EpiLseColMasked>(maps, s, ep, (cudaStream_t)stream);
   return launch<A_ROWS, EpiLseCol>(maps, s, ep, (cudaStream_t)stream);
 }
 
-int opp_sim_conf_colmax(const void* a, const void* b, const float* lse_own, const float* lse_other,
-                        float* conf, float* part_val, int* part_idx, unsigned* colmax, int batches,
-                        int rows, int cols, int k, float scale, int split, opp_stream_t stream) {
+int opp_sim_lse_cols(const void* a, const void* b, float* part_m, float* part_s, float* col_m,
+                     float* col_s, int batches, int rows, int cols, int k, float scale, int split,
+                     const unsigned char* col_mask, opp_stream_t stream) {
+  return opp_sim_lse_cols_rows(a, b, part_m, part_s, col_m, col_s, batches, rows, cols, k, scale, split,
+                               col_mask, nullptr, stream);
+}
+
+int opp_sim_conf_colmax_rows(const void* a, const void* b, const float* lse_own, const float* lse_other,
+                             float* conf, float* part_val, int* part_idx, unsigned* colmax, int batches,
+                             int rows, int cols, int k, float scale, int split, const int* row_count,
+                             opp_stream_t stream) {
   TensorMaps maps;
   GemmShape s;
   int rc = setup_rows(maps, s, a, k, nullptr, 0, b, 1, batches, rows, cols, split, 1, 0, 0,
@@ -642,8 +655,19 @@ int opp_sim_conf_colmax(const void* a, const void* b, const float* lse_own, cons
   OPP_REQUIRE(lse_own && lse_other && part_val && part_idx && colmax, "null pointer");
   OPP_CHECK_CUDA(cudaMemsetAsync(colmax, 0, (size_t)batches * cols * sizeof(unsigned),
                                  (cudaStream_t)stream));
-  EpiConfCol::Params ep{lse_own, lse_other, scale, conf, part_val, part_idx, colmax};
+  EpiConfColParams ep{lse_own, lse_other, scale, conf, part_val, part_idx, colmax};
+  if (row_count) {
+    EpiConfColRowsParams epr{ep, row_count};
+    return launch<A_ROWS, EpiConfColRows>(maps, s, epr, (cudaStream_t)stream);
+  }
   return launch<A_ROWS, EpiConfCol>(maps, s, ep, (cudaStream_t)stream);
+}
+
+int opp_sim_conf_colmax(const void* a, const void* b, const float* lse_own, const float* lse_other,
+                        float* conf, float* part_val, int* part_idx, unsigned* colmax, int batches,
+                        int rows, int cols, int k, float scale, int split, opp_stream_t stream) {
+  return opp_sim_conf_colmax_rows(a, b, lse_own, lse_other, conf, part_val, part_idx, colmax, batches, rows,
+                                  cols, k, scale, split, nullptr, stream);
 }
 
 // partial slots per row written by the dual-softmax passes: one per column tile (a row lives in one

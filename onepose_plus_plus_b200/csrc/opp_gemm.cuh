@@ -1256,20 +1256,37 @@ struct EpiLseColParams {
   // query_image_mask: columns with col_mask[b][col] == 0 get sim + (-1e9) (coarse_matching.py:108-114), or null
   const unsigned char* col_mask;
 };
-template <bool kMask>
+// + per-batch row counts: rows l >= row_count[b] (the padding of a bank set) are not rows of the matrix
+struct EpiLseColRowsParams : EpiLseColParams {
+  const int* row_count;   // [batches]
+};
+
+// bits h = 0, 1 of c.svalid restricted to the first row_count[c.b] rows of the batch element
+__device__ __forceinline__ unsigned rows_below_count(const GemmShape& s, const EpiCtx& c, const int* row_count) {
+  const long long end = (long long)c.b * s.rows + row_count[c.b];
+  return c.svalid & ((c.sgrow[0] < end ? 1u : 0u) | (c.sgrow[1] < end ? 2u : 0u));
+}
+
+template <bool kMask, bool kRows = false>
 struct EpiLseColT {
+  static_assert(!(kMask && kRows), "query_image_mask and per-batch row counts are not combined");
   static constexpr int kGroups = 2;
-  static constexpr const char* kName = "lse_col";   // $OPP_LOG_TILES
+  static constexpr const char* kName = kRows ? "lse_col_rows" : "lse_col";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   // With an n64 mainloop in the same kernel, ptxas serialises every wgmma of it (C7514) next to
   // this epilogue's column butterflies; its GEMMs have >= 4096 columns, so tiles of <= 64 columns
   // (tiny inputs only) run at 128
   static constexpr int kMinMmaN = 128;
-  using Params = EpiLseColParams;
+  using Params = std::conditional_t<kRows, EpiLseColRowsParams, EpiLseColParams>;
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
   template <int N>
   __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
     const int lane = threadIdx.x & 31, c0 = 2 * (lane & 3);
+    // padded rows are treated like rows outside the tensor: -inf, so they leave the column
+    // statistics alone (a wholly padded 32-row group writes (-inf, 0), which the finaliser skips)
+    // and their row partials are not written (nothing reads them)
+    unsigned valid = c.svalid;
+    if constexpr (kRows) valid = rows_below_count(s, c, p.row_count);
     if constexpr (kMask) {   // additive column bias (0 / -1e9) of this tile, shared by the epilogue group
       epi_sync(c);
       for (int i = c.etid; i < c.ncols; i += 128)
@@ -1286,8 +1303,8 @@ struct EpiLseColT {
         if constexpr (kMask) cb_ = lds32f(c.smem_s + 4 * (cl & 255));
 #pragma unroll
         for (int h = 0; h < 2; ++h)
-          d[4 * i + 2 * h + e] = (((c.svalid >> h) & 1u) && cl < c.ncols) ? d[4 * i + 2 * h + e] * p.scale + cb_
-                                                                          : -INFINITY;
+          d[4 * i + 2 * h + e] = (((valid >> h) & 1u) && cl < c.ncols) ? d[4 * i + 2 * h + e] * p.scale + cb_
+                                                                        : -INFINITY;
       }
     // row partials
 #pragma unroll
@@ -1303,7 +1320,7 @@ struct EpiLseColT {
         for (int e = 0; e < 2; ++e)
           if (8 * i + c0 + e < c.ncols) sum += fast_exp(d[4 * i + 2 * h + e] - m);
       sum = quad_sum(sum);
-      if ((lane & 3) == 0 && ((c.svalid >> h) & 1u)) {
+      if ((lane & 3) == 0 && ((valid >> h) & 1u)) {
         p.part_m[c.sgrow[h] * s.n_tiles + c.n_tile] = m;
         p.part_s[c.sgrow[h] * s.n_tiles + c.n_tile] = sum;
       }
@@ -1365,6 +1382,7 @@ struct EpiLseColT {
 
 using EpiLseCol = EpiLseColT<false>;
 using EpiLseColMasked = EpiLseColT<true>;   // + query_image_mask (-1e9 on the padded query cells)
+using EpiLseColRows = EpiLseColT<false, true>;   // + per-batch row counts (bank sets)
 
 // conf pass with the column maxima folded in (replaces the second conf pass): rows are 3D points,
 // conf and the row (max, first argmax) as in EpiConf with own_is_pt.  Every warp reduces each
@@ -1374,32 +1392,41 @@ using EpiLseColMasked = EpiLseColT<true>;   // + query_image_mask (-1e9 on the p
 // unsigned ints; an integer max, so the result does not depend on the order).  The mutual-nearest
 // test (coarse_matching.py:157-165) is then  rowmax(i) == colmax(argmax_j(i)), an exact comparison
 // of two copies of the same register value.
-struct EpiConfCol {
+struct EpiConfColParams {
+  const float* lse_own;    // [batches*rows]   (3D points)
+  const float* lse_other;  // [batches][n_total] (query cells)
+  float scale;
+  float* conf;             // [batches*rows][n_total] or null
+  float* part_val;         // [batches*rows][n_tiles]
+  int* part_idx;
+  unsigned* colmax;        // [batches][n_total], zero-initialised
+};
+// + per-batch row counts: rows l >= row_count[b] never enter colmax and are stored as conf 0; their
+// row (max, argmax) partials are written but meaningless (the match selection skips those rows)
+struct EpiConfColRowsParams : EpiConfColParams {
+  const int* row_count;    // [batches]
+};
+template <bool kRows>
+struct EpiConfColT {
   static constexpr int kGroups = 2;
-  static constexpr const char* kName = "conf_col";   // $OPP_LOG_TILES
+  static constexpr const char* kName = kRows ? "conf_col_rows" : "conf_col";   // $OPP_LOG_TILES
   static constexpr bool kFromRegs = true;
   // With an n64 mainloop in the same kernel, ptxas serialises every wgmma of it (C7514) next to
   // this epilogue's column butterfly; its GEMMs have >= 4096 columns, so tiles of <= 64 columns
   // (tiny inputs only) run at 128
   static constexpr int kMinMmaN = 128;
-  struct Params {
-    const float* lse_own;    // [batches*rows]   (3D points)
-    const float* lse_other;  // [batches][n_total] (query cells)
-    float scale;
-    float* conf;             // [batches*rows][n_total] or null
-    float* part_val;         // [batches*rows][n_tiles]
-    int* part_idx;
-    unsigned* colmax;        // [batches][n_total], zero-initialised
-  };
+  using Params = std::conditional_t<kRows, EpiConfColRowsParams, EpiConfColParams>;
   __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
   template <int N>
   __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
     const int lane = threadIdx.x & 31;
     epi_stage_cols_b(s, c, p.lse_other);
+    unsigned valid = c.svalid;
+    if constexpr (kRows) valid = rows_below_count(s, c, p.row_count);
     float lown[2], best[2] = {-1.f, -1.f};
     int bidx[2] = {c.n0, c.n0};
 #pragma unroll
-    for (int h = 0; h < 2; ++h) lown[h] = ((c.svalid >> h) & 1u) ? p.lse_own[c.sgrow[h]] : 0.f;
+    for (int h = 0; h < 2; ++h) lown[h] = ((valid >> h) & 1u) ? p.lse_own[c.sgrow[h]] : 0.f;
     constexpr int kSlices = (N + 31) / 32;
     float cmax[kSlices];
 #pragma unroll
@@ -1410,13 +1437,18 @@ struct EpiConfCol {
         float v[16];
         frag_slice<N>(d, j, v);
         conf_slice(c, col, p.scale, lown, true, v, best, bidx);
+        if constexpr (kRows) {
+#pragma unroll
+          for (int k = 0; k < 16; ++k)
+            if (!((valid >> ((k >> 1) & 1)) & 1u)) v[k] = 0.f;
+        }
         if (p.conf) conf_store(s, c, p.conf, col, v);
         // column maxima over this warp's 16 rows (rows outside the tensor contribute 0)
         float x[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
-          const float a = (c.svalid & 1u) ? v[4 * (k >> 1) + (k & 1)] : 0.f;
-          const float b = (c.svalid & 2u) ? v[4 * (k >> 1) + 2 + (k & 1)] : 0.f;
+          const float a = (valid & 1u) ? v[4 * (k >> 1) + (k & 1)] : 0.f;
+          const float b = (valid & 2u) ? v[4 * (k >> 1) + 2 + (k & 1)] : 0.f;
           x[k] = fmaxf(a, b);
         }
         cmax[j] = col_reduce8(x, [](float a, float b) { return fmaxf(a, b); });
@@ -1444,6 +1476,9 @@ struct EpiConfCol {
     pair_sync(c);   // the odd warp's stage is free again
   }
 };
+
+using EpiConfCol = EpiConfColT<false>;
+using EpiConfColRows = EpiConfColT<true>;   // + per-batch row counts (bank sets)
 
 // =============================================================================================
 // The kernel

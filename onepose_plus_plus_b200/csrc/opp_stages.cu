@@ -541,9 +541,16 @@ __device__ __forceinline__ bool match_flag(const float* pt_val, const int* pt_id
 // row maximum IS the column maximum of j (colmax holds the float bits written by EpiConfCol from
 // the very same conf values, so the comparison is exact; coarse_matching.py:157-165 compares
 // conf == conf.max(dim) the same way).
+// kRows (bank sets): rows i >= row_count[b] are the padding of the frame's object and never match.
+template <bool kRows = false>
 __device__ __forceinline__ bool match_flag_colmax(const float* pt_val, const int* pt_idx,
                                                   const unsigned* colmax, long long r, int l, int s,
-                                                  int wc, float thr, int border) {
+                                                  int wc, float thr, int border,
+                                                  const int* row_count = nullptr) {
+  if constexpr (kRows) {
+    const long long b = r / l;
+    if (r - b * l >= row_count[b]) return false;
+  }
   const float v = pt_val[r];
   if (!(v > thr)) return false;
   const int j = pt_idx[r];
@@ -553,15 +560,18 @@ __device__ __forceinline__ bool match_flag_colmax(const float* pt_val, const int
   return colmax[b * s + j] == __float_as_uint(v);
 }
 
+template <bool kRows>
 __global__ void __launch_bounds__(1024) match_count_colmax_kernel(const float* pt_val,
                                                                   const int* pt_idx,
                                                                   const unsigned* colmax,
                                                                   long long rows, int l, int s, int wc,
                                                                   float thr, int border,
-                                                                  int* block_counts) {
+                                                                  int* block_counts,
+                                                                  const int* row_count) {
   pdl_sync();
   const long long r = (long long)blockIdx.x * 1024 + threadIdx.x;
-  const bool f = r < rows && match_flag_colmax(pt_val, pt_idx, colmax, r, l, s, wc, thr, border);
+  const bool f = r < rows && match_flag_colmax<kRows>(pt_val, pt_idx, colmax, r, l, s, wc, thr, border,
+                                                      row_count);
   const int c = __syncthreads_count(f);
   if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
 }
@@ -667,16 +677,19 @@ match_scatter_kernel(const float* pt_val, const int* pt_idx, const int* px_idx, 
   mkpts_c[pos * 2 + 1] = (float)(j / wc) * sy;
 }
 
+// kSet (bank sets): kpts is [K][l][3], read at bank_of_batch[b]; rows past row_count[b] are skipped
+template <bool kSet>
 __global__ void __launch_bounds__(1024)
 match_scatter_colmax_kernel(const float* pt_val, const int* pt_idx, const unsigned* px_idx, const float* kpts,
                      const float* img_scale, long long rows, int l, int s, int wc, float thr,
                      int border, float cell, const int* block_offsets, long long* b_ids,
                      long long* i_ids, long long* j_ids, float* mconf, float* mkpts3d,
-                     float* mkpts_c, int kpts_shared) {
+                     float* mkpts_c, int kpts_shared, const int* bank_of_batch, const int* row_count) {
   pdl_sync();
   __shared__ int warp_sums[32];
   const long long r = (long long)blockIdx.x * 1024 + threadIdx.x;
-  const bool f = r < rows && match_flag_colmax(pt_val, pt_idx, px_idx, r, l, s, wc, thr, border);
+  const bool f = r < rows && match_flag_colmax<kSet>(pt_val, pt_idx, px_idx, r, l, s, wc, thr, border,
+                                                     row_count);
   const unsigned ballot = __ballot_sync(0xffffffffu, f);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (lane == 0) warp_sums[warp] = __popc(ballot);
@@ -701,7 +714,9 @@ match_scatter_colmax_kernel(const float* pt_val, const int* pt_idx, const unsign
   i_ids[pos] = i;
   j_ids[pos] = j;
   mconf[pos] = pt_val[r];
-  const float* kp = kpts + ((kpts_shared ? 0 : b) * l + i) * 3;
+  long long kb = kpts_shared ? 0 : b;
+  if constexpr (kSet) kb = bank_of_batch[b];
+  const float* kp = kpts + (kb * l + i) * 3;
   mkpts3d[pos * 3 + 0] = kp[0];
   mkpts3d[pos * 3 + 1] = kp[1];
   mkpts3d[pos * 3 + 2] = kp[2];
@@ -718,12 +733,14 @@ match_scatter_colmax_kernel(const float* pt_val, const int* pt_idx, const unsign
 // =============================================================================================
 // fine window gather   (loftr_module/fine_preprocess.py:41-55)
 // =============================================================================================
+// kSet (bank sets): desc3d is [K][128][n], read at the frame's object bank_of_batch[b]
+template <bool kSet>
 __global__ void __launch_bounds__(128) fine_gather_kernel(
     const __half* __restrict__ fine, const float* __restrict__ desc3d,
     const long long* __restrict__ b_ids, const long long* __restrict__ i_ids,
     const long long* __restrict__ j_ids, float* __restrict__ x32, __half* __restrict__ x16, int hf,
     int wf, int wc, int stride, int n, int lo_off, int desc_shared, int windows,
-    const int* __restrict__ count_dev) {
+    const int* __restrict__ count_dev, const int* __restrict__ bank_of_batch) {
   pdl_sync();
   const int m = blockIdx.x, c = threadIdx.x;
   if (count_dev && m >= *count_dev) return;   // launched at capacity, match count on the device
@@ -731,7 +748,9 @@ __global__ void __launch_bounds__(128) fine_gather_kernel(
   const int jy = (int)(j / wc), jx = (int)(j - (long long)jy * wc);
   const long long row0 = (long long)m * 26;
   const int ld = lo_off ? 256 : 128;
-  const float d = desc3d[((desc_shared ? 0 : b) * 128 + c) * n + i];
+  long long db = desc_shared ? 0 : b;
+  if constexpr (kSet) db = bank_of_batch[b];
+  const float d = desc3d[(db * 128 + c) * n + i];
   if (x32) x32[row0 * 128 + c] = d;
   store_split1(x16 + row0 * ld, c, d, lo_off);
   // windows (= row pitch P, 8 or 5): `fine` holds the compact per-match windows of opp_conv_win, [m][5][P][ld]
@@ -1410,23 +1429,65 @@ int opp_match_select(const float* pt_val, const int* pt_idx, const int* px_idx, 
   return OPP_OK;
 }
 
+int opp_match_select_colmax_set(const float* pt_val, const int* pt_idx, const unsigned* colmax,
+                                const float* kpts, const float* img_scale, int batch, int l, int hc,
+                                int wc, float thr, int border, float cell, int* scratch,
+                                long long* b_ids, long long* i_ids, long long* j_ids, float* mconf,
+                                float* mkpts3d, float* mkpts_c, int* count_out, int bank_shared,
+                                const int* bank_of_batch, const int* row_count, opp_stream_t stream) {
+  OPP_REQUIRE(pt_val && pt_idx && colmax && kpts && scratch && count_out, "null pointer");
+  OPP_REQUIRE((bank_of_batch == nullptr) == (row_count == nullptr),
+              "bank_of_batch and row_count come together (bank sets)");
+  const long long rows = (long long)batch * l;
+  const int nblocks = (int)((rows + 1023) / 1024);
+  const int s = hc * wc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (bank_of_batch) {
+    OPP_CHECK_CUDA(opp::launch_pdl(match_count_colmax_kernel<true>, dim3(nblocks), dim3(1024), 0, st, pt_val, pt_idx,
+                                   colmax, rows, l, s, wc, thr, border, scratch, row_count));
+  } else {
+    OPP_CHECK_CUDA(opp::launch_pdl(match_count_colmax_kernel<false>, dim3(nblocks), dim3(1024), 0, st, pt_val, pt_idx,
+                                   colmax, rows, l, s, wc, thr, border, scratch, row_count));
+  }
+  OPP_CHECK_CUDA(opp::launch_pdl(match_scan_kernel, dim3(1), dim3(1024), 0, st, scratch, nblocks, count_out));
+  if (bank_of_batch) {
+    OPP_CHECK_CUDA(opp::launch_pdl(match_scatter_colmax_kernel<true>, dim3(nblocks), dim3(1024), 0, st, pt_val, pt_idx,
+                                   colmax, kpts, img_scale, rows, l, s, wc, thr, border, cell, scratch, b_ids,
+                                   i_ids, j_ids, mconf, mkpts3d, mkpts_c, bank_shared, bank_of_batch, row_count));
+  } else {
+    OPP_CHECK_CUDA(opp::launch_pdl(match_scatter_colmax_kernel<false>, dim3(nblocks), dim3(1024), 0, st, pt_val, pt_idx,
+                                   colmax, kpts, img_scale, rows, l, s, wc, thr, border, cell, scratch, b_ids,
+                                   i_ids, j_ids, mconf, mkpts3d, mkpts_c, bank_shared, bank_of_batch, row_count));
+  }
+  OPP_CHECK_CUDA(cudaGetLastError());
+  return OPP_OK;
+}
+
 int opp_match_select_colmax(const float* pt_val, const int* pt_idx, const unsigned* colmax,
                             const float* kpts, const float* img_scale, int batch, int l, int hc,
                             int wc, float thr, int border, float cell, int* scratch,
                             long long* b_ids, long long* i_ids, long long* j_ids, float* mconf,
                             float* mkpts3d, float* mkpts_c, int* count_out, int bank_shared,
                             opp_stream_t stream) {
-  OPP_REQUIRE(pt_val && pt_idx && colmax && kpts && scratch && count_out, "null pointer");
-  const long long rows = (long long)batch * l;
-  const int nblocks = (int)((rows + 1023) / 1024);
-  const int s = hc * wc;
-  cudaStream_t st = (cudaStream_t)stream;
-  OPP_CHECK_CUDA(opp::launch_pdl(match_count_colmax_kernel, dim3(nblocks), dim3(1024), 0, st, pt_val, pt_idx, colmax, rows, l, s, wc, thr,
-                                                      border, scratch));
-  OPP_CHECK_CUDA(opp::launch_pdl(match_scan_kernel, dim3(1), dim3(1024), 0, st, scratch, nblocks, count_out));
-  OPP_CHECK_CUDA(opp::launch_pdl(match_scatter_colmax_kernel, dim3(nblocks), dim3(1024), 0, st, pt_val, pt_idx, colmax, kpts, img_scale, rows,
-                                                        l, s, wc, thr, border, cell, scratch, b_ids,
-                                                        i_ids, j_ids, mconf, mkpts3d, mkpts_c, bank_shared));
+  return opp_match_select_colmax_set(pt_val, pt_idx, colmax, kpts, img_scale, batch, l, hc, wc, thr, border, cell,
+                                     scratch, b_ids, i_ids, j_ids, mconf, mkpts3d, mkpts_c, count_out, bank_shared,
+                                     nullptr, nullptr, stream);
+}
+
+int opp_fine_gather_set(const void* fine, const float* desc3d, const long long* b_ids,
+                        const long long* i_ids, const long long* j_ids, float* x32, void* x16, int m,
+                        int hf, int wf, int wc, int stride, int n, int split, int bank_shared,
+                        int windows, const int* count_dev, const int* bank_of_batch, opp_stream_t stream) {
+  if (m == 0) return OPP_OK;
+  OPP_REQUIRE(fine && desc3d && b_ids && i_ids && j_ids && x16, "null pointer");
+  if (bank_of_batch)
+    OPP_CHECK_CUDA(opp::launch_pdl(fine_gather_kernel<true>, dim3(m), dim3(128), 0, (cudaStream_t)stream,
+                                   (const __half*)fine, desc3d, b_ids, i_ids, j_ids, x32, (__half*)x16, hf, wf,
+                                   wc, stride, n, split ? 128 : 0, bank_shared, windows, count_dev, bank_of_batch));
+  else
+    OPP_CHECK_CUDA(opp::launch_pdl(fine_gather_kernel<false>, dim3(m), dim3(128), 0, (cudaStream_t)stream,
+                                   (const __half*)fine, desc3d, b_ids, i_ids, j_ids, x32, (__half*)x16, hf, wf,
+                                   wc, stride, n, split ? 128 : 0, bank_shared, windows, count_dev, bank_of_batch));
   OPP_CHECK_CUDA(cudaGetLastError());
   return OPP_OK;
 }
@@ -1435,14 +1496,8 @@ int opp_fine_gather(const void* fine, const float* desc3d, const long long* b_id
                     const long long* i_ids, const long long* j_ids, float* x32, void* x16, int m,
                     int hf, int wf, int wc, int stride, int n, int split, int bank_shared,
                     int windows, const int* count_dev, opp_stream_t stream) {
-  if (m == 0) return OPP_OK;
-  OPP_REQUIRE(fine && desc3d && b_ids && i_ids && j_ids && x16, "null pointer");
-  OPP_CHECK_CUDA(opp::launch_pdl(fine_gather_kernel, dim3(m), dim3(128), 0, (cudaStream_t)stream, (const __half*)fine, desc3d, b_ids,
-                                                          i_ids, j_ids, x32, (__half*)x16, hf, wf,
-                                                          wc, stride, n, split ? 128 : 0, bank_shared,
-                                                          windows, count_dev));
-  OPP_CHECK_CUDA(cudaGetLastError());
-  return OPP_OK;
+  return opp_fine_gather_set(fine, desc3d, b_ids, i_ids, j_ids, x32, x16, m, hf, wf, wc, stride, n, split,
+                             bank_shared, windows, count_dev, nullptr, stream);
 }
 
 int opp_fine_attention(const void* qkv, void* msg, int m, int cross, float eps, int split,

@@ -516,10 +516,11 @@ class _Engine(nn.Module):
         2 (3) windows per 128-row tile against hf*wf/128 tiles per image."""
         return M * (208 / 2 + 128 / 3) < 0.85 * B * (hf * wf / 128) * (208 + 128)
 
-    def _src_state(self, L, tag, src, B, ls, src_mask=None):
+    def _src_state(self, L, tag, src, B, ls, src_mask=None, v_len=None):
         """Source side of linear attention for one layer (linear_attention.py:46,55-57 +
         transformer.py:78-79,85): K' = elu(Wk src)+1, V = Wv src, per-head KV / Ksum, with `merge`
-        folded in -> (Mt [B, 256, pl*256] fp16, Ksum [B, 256] fp32)."""
+        folded in -> (Mt [B, 256, pl*256] fp16, Ksum [B, 256] fp32).  v_len (default ls): the
+        length the query side multiplies back by (linear_attention.py:55,61)."""
         dev = src.device
         f16 = torch.float16
         split = self.split
@@ -531,15 +532,17 @@ class _Engine(nn.Module):
         part = self._buf(tag + "part", (B, ops.kv_chunks(ls, B), 8, 33, 32), torch.float32, dev)
         mt = self._buf(tag + "mt", (B, 256, pl * 256), f16, dev)
         ksum = self._buf(tag + "ksum", (B, 256), torch.float32, dev)
-        ops.kv_state(kv16, part, L["merge32"], mt, ksum, B, ls, 256, ls, split, kv_split=kv_split)
+        ops.kv_state(kv16, part, L["merge32"], mt, ksum, B, ls, 256, ls if v_len is None else v_len, split,
+                     kv_split=kv_split)
         return mt, ksum
 
     def _encoder_layer(self, L, tag, x, src, B, lx, ls, out, x_shared=False, state=None, x_mask=None,
-                       src_mask=None):
+                       src_mask=None, state_batched=False):
         """LoFTREncoderLayer.forward (transformer.py:65-94) with linear attention
         (linear_attention.py:29-61) for d_model 256.  x, src, out: fp16 planes [B, len, pl*256].
         x_shared: x is [1, lx, ..] — one object's tokens, the same for every image of the batch.
-        state = (Mt [1, ...], Ksum [B, 256]): precomputed source state shared by the batch.
+        state = (Mt [1, ...], Ksum [B, 256]): precomputed source state shared by the batch
+        (state_batched: Mt is [B, ...], one per image).
         x_mask / src_mask (uint8 [B * len]): padded positions of query_image_mask — Q rows resp.
         K', V rows are zeroed (linear_attention.py:49-53)."""
         dev = x.device
@@ -566,7 +569,7 @@ class _Engine(nn.Module):
                 mt_batched = True
             else:
                 mt, ksum = state
-                mt_batched = False
+                mt_batched = state_batched
             qz = self._buf(tag + "qz", (B * lx, pl * 256), f16, dev)
             ops.linear_q(x, L["wq"], ksum, qz, B, lx, ls, split, x_shared=x_shared, row_mask=x_mask)
             ops.linear_ln(qz, None, mt, mt_batched, *L["n1"], B, lx, split, out16=msg)
@@ -639,6 +642,7 @@ class OnePosePlus_model(_Engine):
                 for p in self.backbone.parameters():
                     p.requires_grad = False
         self._bank = None
+        self._bank_set = None
         self._side_stream = None
         self._fwd_count = 0
         self.use_cuda_graphs = os.environ.get("OPP_B200_GRAPHS", "0") == "1"
@@ -661,6 +665,7 @@ class OnePosePlus_model(_Engine):
         st = self.__dict__.copy()
         st["_plan"], st["_plan_sig"], st["_ws"], st["_sig_tensors"] = None, None, {}, None
         st["_bank"], st["_graphs"], st["_side_stream"] = None, {}, None
+        st["_bank_set"] = None
         st.pop("_aux", None)
         st.pop("_aux_fpn", None)
         return st
@@ -668,17 +673,19 @@ class OnePosePlus_model(_Engine):
     def __setstate__(self, st):
         self.__dict__.update(st)
         for k, v in (("_sig_tensors", None), ("_apply_epoch", 0), ("_ws_epoch", 0), ("_bank", None),
+                     ("_bank_set", None),
                      ("_graphs", {}), ("_fwd_count", 0), ("use_cuda_graphs", False), ("_side_stream", None),
                      ("fine_windows", "auto")):
             self.__dict__.setdefault(k, v)
 
     # ------------------------------------------------------------------ descriptor bank
-    def _encode_bank(self, kpts, dcoarse, dfine, persistent):
+    def _encode_bank(self, kpts, dcoarse, dfine, persistent, l1_v_len=None):
         """Image-independent part of the forward for one descriptor bank (SURVEY §8e/f2): keypoint
         normalisation + encoding (normalize.py:16-26, position_encoding.py:54-60) and — when the
         bank is ONE object ([1, N, .]) and the coarse transformer starts with (self, cross) — the
         3D side of the first self layer plus the 3D-as-source attention state of the first cross
-        layer (transformer.py:148-159: both read only 3D tokens)."""
+        layer (transformer.py:148-159: both read only 3D tokens).  l1_v_len: the v_len that layer-1
+        state is divided by (default N; a bank set pads to N_max and its forward queries with N_max)."""
         dev = kpts.device
         f16 = torch.float16
         pl = 2 if self.split else 1
@@ -695,7 +702,7 @@ class OnePosePlus_model(_Engine):
         if Bb == 1 and linear and len(names) >= 2 and names[0] == "self" and names[1] == "cross":
             d3_l0 = alloc("d3_l0", (1, N, pl * 256), f16)
             self._encoder_layer(self._plan["coarse"][0], "c3s_", d3, d3, 1, N, N, d3_l0)
-            mt, ksum = self._src_state(self._plan["coarse"][1], "c3s_", d3_l0, 1, N)
+            mt, ksum = self._src_state(self._plan["coarse"][1], "c3s_", d3_l0, 1, N, v_len=l1_v_len)
             st["d3_l0"] = d3_l0
             st["l1_mt"] = alloc("l1_mt", mt.shape, f16).copy_(mt)
             st["l1_ksum"] = alloc("l1_ksum", ksum.shape, torch.float32).copy_(ksum)
@@ -709,11 +716,18 @@ class OnePosePlus_model(_Engine):
         [1, 128, N], descriptors3d_coarse_db [1, 256, N].  Afterwards `forward(data)` uses this bank
         whenever `data` carries no "keypoints3d"; the keypoint encoding, the 3D side of the first
         self layer and the 3D source state of the first cross layer are computed once per object."""
+        self._bank = {"raw": self._prep_bank(keypoints3d, descriptors3d_db, descriptors3d_coarse_db),
+                      "state": None}
+        self._bank_set = None
+        return self
+
+    def _prep_bank(self, keypoints3d, descriptors3d_db, descriptors3d_coarse_db=None):
+        """One object's bank on the model's device: (kpts [1,N,3], coarse [1,256,N], fine [1,128,N]) fp32."""
         dev = next(self.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("set_bank: move the model to a CUDA device first (there is no CPU path)")
 
-        def prep(t, c):
+        def prep(t):
             t = torch.as_tensor(t)
             if t.dim() == 2:
                 t = t[None]
@@ -721,25 +735,119 @@ class OnePosePlus_model(_Engine):
                 raise ValueError(f"set_bank expects ONE object ([1, ...] tensors), got {tuple(t.shape)}")
             return t.to(device=dev, dtype=torch.float32).contiguous()
 
-        kp = prep(keypoints3d, 3)
-        fine = prep(descriptors3d_db, 128)
-        coarse = prep(descriptors3d_coarse_db, 256) if descriptors3d_coarse_db is not None else fine
+        kp = prep(keypoints3d)
+        fine = prep(descriptors3d_db)
+        coarse = prep(descriptors3d_coarse_db) if descriptors3d_coarse_db is not None else fine
         N = kp.shape[1]
         if kp.shape[2] != 3 or fine.shape[2] != N or coarse.shape[2] != N or coarse.shape[1] != 256:
             raise ValueError("set_bank: expected keypoints3d [1,N,3], descriptors3d_db [1,128,N], "
                              f"descriptors3d_coarse_db [1,256,N]; got {tuple(kp.shape)}, {tuple(fine.shape)}, "
                              f"{tuple(coarse.shape)}")
-        self._bank = {"raw": (kp, coarse, fine), "state": None}
+        return kp, coarse, fine
+
+    def set_banks(self, banks):
+        """Make a SET of K objects' descriptor banks resident (extension with no counterpart in the
+        reference, which matches every frame of a batch against one object).  `banks`: a list of K
+        (keypoints3d, descriptors3d_db, descriptors3d_coarse_db=None) tuples shaped as for
+        set_bank; the point counts N_k may differ.  Afterwards `forward(data)` reads
+        data["object_ids"] (int [B], entries in [0, K); CPU avoids a read-back: a CUDA tensor is
+        copied to the host to be validated before any launch) and matches frame b against
+        object object_ids[b]: every output equals that of set_bank(*banks[object_ids[b]]) and a
+        forward of frame b alone (each object's keypoints normalised by its own extents), with the
+        frames' matches in the usual ascending (b, i) order; i_ids index the frame's own object and
+        mkpts_3d_db come from it.  conf_matrix is [B, N_max, S] with rows >= N_k of a frame exactly 0.
+        Replaces a bank of set_bank; clear_bank() drops both.  Not built: query_image_mask with a
+        set (NotImplementedError) and training (train() raises while a set is resident)."""
+        names = self.loftr_coarse.layer_names
+        if self.config["loftr_coarse"]["attention"] != "linear" or names[:2] != ["self", "cross"]:
+            raise NotImplementedError("bank sets are built for linear coarse attention starting with (self, cross)")
+        if self.training:
+            raise NotImplementedError("bank sets are built for inference: call eval() first")
+        banks = list(banks)
+        if not banks:
+            raise ValueError("set_banks: empty list of banks")
+        raw = []
+        for bk in banks:
+            if not isinstance(bk, (tuple, list)) or len(bk) not in (2, 3):
+                raise ValueError("set_banks: every bank is (keypoints3d, descriptors3d_db[, descriptors3d_coarse_db])")
+            raw.append(self._prep_bank(*bk))
+            if raw[-1][0].shape[1] < 1:
+                raise ValueError("set_banks: an object without keypoints")
+        if len({r[2].shape[1] for r in raw}) != 1:
+            raise ValueError("set_banks: descriptors3d_db channel counts differ between objects")
+        self._bank = None
+        self._bank_set = {"raw": raw, "state": None}
         return self
 
     def clear_bank(self):
         self._bank = None
+        self._bank_set = None
+
+    def train(self, mode=True):
+        if mode and getattr(self, "_bank_set", None) is not None:
+            raise NotImplementedError("training with a resident bank set is not built: clear_bank() first")
+        return super().train(mode)
 
     def _resident_bank_state(self):
         b = self._bank
         if b["state"] is None or b["state"]["sig"] != self._plan_sig:
             b["state"] = self._encode_bank(*b["raw"], persistent=True)
         return b["state"]
+
+    def _encode_bank_set(self, raw):
+        """Image-independent state of a bank set: every object encoded once, unpadded, by the
+        one-object code (_encode_bank: its own keypoint extents, the first (self, cross) cache), then
+        stored padded to N_max = max N_k.  Rows >= n_rows[k] of kpts / d3_l0 and columns >= n_rows[k]
+        of fine are padding: the forward masks them (row_mask, row_count) and no output reads them,
+        whatever they hold."""
+        dev = raw[0][0].device
+        n = [r[0].shape[1] for r in raw]
+        K, Nm = len(raw), max(n)
+        pl = 2 if self.split else 1
+        st = {"K": K, "N": Nm, "sig": self._plan_sig,
+              "kpts": torch.zeros(K, Nm, 3, device=dev),
+              "fine": torch.zeros(K, raw[0][2].shape[1], Nm, device=dev),
+              "d3_l0": torch.zeros(K, Nm, pl * 256, dtype=torch.float16, device=dev),
+              "l1_mt": torch.empty(K, 256, pl * 256, dtype=torch.float16, device=dev),
+              "l1_ksum": torch.empty(K, 256, dtype=torch.float32, device=dev),
+              "n_rows": torch.tensor(n, dtype=torch.int32, device=dev),
+              "rows": torch.arange(Nm, dtype=torch.int32, device=dev)}
+        for k, (kp, coarse, fine) in enumerate(raw):
+            # the forward's layer-1 query multiplies by v_len = N_max (_coarse_transformer), so the
+            # cached state divides by N_max: KV/N_max * N_max is the one-object KV/N_k * N_k
+            one = self._encode_bank(kp, coarse, fine, persistent=False, l1_v_len=Nm)
+            st["kpts"][k, :n[k]] = kp[0]
+            st["fine"][k, :, :n[k]] = fine[0]
+            st["d3_l0"][k, :n[k]] = one["d3_l0"][0]
+            st["l1_mt"][k] = one["l1_mt"][0]
+            st["l1_ksum"][k] = one["l1_ksum"][0]
+        return st
+
+    def _resident_set_state(self):
+        s = self._bank_set
+        if s["state"] is None or s["state"]["sig"] != self._plan_sig:
+            s["state"] = self._encode_bank_set(s["raw"])
+        return s["state"]
+
+    def _set_frame_state(self, oid, B):
+        """The bank state of a forward with a bank set: per-frame copies of the cached first-layer
+        state (index_select on the device-side object ids, so a CUDA graph captures the gather and
+        serves every assignment of objects to frames), the frames' row counts and the uint8 row
+        mask [B * N_max] (0 on padding).  kpts / fine stay [K, ...] and are read through
+        bank_of_batch."""
+        st = self._resident_set_state()
+        dev, Nm = oid.device, st["N"]
+
+        def gather(name, src):
+            return torch.index_select(src, 0, oid, out=self._buf(name, (B,) + tuple(src.shape[1:]), src.dtype, dev))
+
+        n_b = gather("set_n_rows", st["n_rows"])
+        mask = self._buf("set_row_mask", (B, Nm), torch.bool, dev)
+        torch.lt(st["rows"][None], n_b[:, None], out=mask)
+        return {"Bb": B, "N": Nm, "kpts": st["kpts"], "fine": st["fine"],
+                "d3_l0": gather("set_d3_l0", st["d3_l0"]), "l1_mt": gather("set_l1_mt", st["l1_mt"]),
+                "l1_ksum": gather("set_l1_ksum", st["l1_ksum"]), "row_count": n_b,
+                "row_mask": mask.view(torch.uint8).view(-1), "bank_of_batch": oid}
 
     def _coarse_transformer(self, q2, bank, B, S, N, qmask=None):
         """LocalFeatureTransformer.forward (transformer.py:133-171): self layers update each
@@ -752,7 +860,12 @@ class OnePosePlus_model(_Engine):
         pl = 2 if self.split else 1
         names = self.loftr_coarse.layer_names
         shared = bank["Bb"] == 1 and B > 1
-        cur2, cur3 = q2, bank["d3_in"]
+        cur2, cur3 = q2, bank.get("d3_in")
+        # bank set (_set_frame_state): uint8 [B*N], 0 on the padding of each frame's object.  As a
+        # source its K'/V rows are zero, as a query its rows stay finite; v_len = N (padded) cancels
+        # between the KV state (/v_len) and the query (*v_len), the cached layer-1 state included
+        # (_encode_bank_set builds it with v_len = N)
+        rmask = bank.get("row_mask")
         first = 0
         both = self._both
         if "d3_l0" in bank:
@@ -762,13 +875,18 @@ class OnePosePlus_model(_Engine):
             o2 = self._buf("q2_1", (B, S, pl * 256), f16, dev)
             self._encoder_layer(L0, "c2_", cur2, cur2, B, S, S, o2, x_mask=qmask, src_mask=qmask)
             d3 = bank["d3_l0"]
-            ksum_b = self._buf("l1_ksum_b", (B, 256), torch.float32, dev)
-            ksum_b.copy_(bank["l1_ksum"].expand(B, -1))
+            if rmask is None:
+                ksum_b = self._buf("l1_ksum_b", (B, 256), torch.float32, dev)
+                ksum_b.copy_(bank["l1_ksum"].expand(B, -1))
+                state = (bank["l1_mt"], ksum_b)
+            else:   # bank set: per-frame states and tokens, gathered already
+                state = (bank["l1_mt"], bank["l1_ksum"])
             o2b = self._buf("q2_0", (B, S, pl * 256), f16, dev)
             o3 = self._buf("d3_0", (B, N, pl * 256), f16, dev)
-            both(lambda: self._encoder_layer(L1, "c2_", o2, None, B, S, N, o2b, state=(bank["l1_mt"], ksum_b),
-                                             x_mask=qmask),
-                 lambda: self._encoder_layer(L1, "c3_", d3, o2, B, N, S, o3, x_shared=True, src_mask=qmask))
+            both(lambda: self._encoder_layer(L1, "c2_", o2, None, B, S, N, o2b, state=state, x_mask=qmask,
+                                             state_batched=rmask is not None),
+                 lambda: self._encoder_layer(L1, "c3_", d3, o2, B, N, S, o3, x_shared=rmask is None, src_mask=qmask,
+                                             x_mask=rmask))
             cur2, cur3 = o2b, o3
             first = 2
         elif shared:
@@ -782,9 +900,10 @@ class OnePosePlus_model(_Engine):
             self_layer = names[i] == "self"
             both(lambda: self._encoder_layer(L, "c2_", cur2, cur2 if self_layer else cur3, B, S,
                                              S if self_layer else N, o2, x_mask=qmask,
-                                             src_mask=qmask if self_layer else None),
+                                             src_mask=qmask if self_layer else rmask),
                  lambda: self._encoder_layer(L, "c3_", cur3, cur3 if self_layer else cur2, B, N,
-                                             N if self_layer else S, o3, src_mask=None if self_layer else qmask))
+                                             N if self_layer else S, o3, x_mask=rmask,
+                                             src_mask=rmask if self_layer else qmask))
             cur2, cur3 = o2, o3
         return cur2, cur3
 
@@ -823,12 +942,17 @@ class OnePosePlus_model(_Engine):
         if qmask is not None and not (self.coarse_lse_cols and self.coarse_colmax):
             raise NotImplementedError("query_image_mask is built for the one-pass dual softmax "
                                       "(coarse_lse_cols and coarse_colmax on)")
+        # bank set: rows >= row_count[b] are the padding of frame b's object
+        rows_b, bank_of_batch = bank.get("row_count"), bank.get("bank_of_batch")
+        if rows_b is not None and not (self.coarse_lse_cols and self.coarse_colmax):
+            raise NotImplementedError("bank sets are built for the one-pass dual softmax "
+                                      "(coarse_lse_cols and coarse_colmax on)")
         if self.coarse_lse_cols:
             groups = (N + 31) // 32
             col_m = self._buf("lse_col_m", (B, groups, S), f32, dev)
             col_s = self._buf("lse_col_s", (B, groups, S), f32, dev)
             ops.sim_lse_cols(d3, q2, B, N, S, 256, scale, pm_pt, ps_pt, lse_pt, col_m, col_s, lse_px, split,
-                             col_mask=qmask, side_stream=side)
+                             col_mask=qmask, side_stream=side, row_count=rows_b)
         else:
             pm_px = self._buf("pm_px", (B * S, tl), f32, dev)
             ps_px = self._buf("ps_px", (B * S, tl), f32, dev)
@@ -857,10 +981,11 @@ class OnePosePlus_model(_Engine):
         if self.coarse_colmax:
             colmax = self._buf("colmax", (B, S), i32, dev)
             ops.sim_conf_colmax(d3, q2, lse_pt, lse_px, conf, B, N, S, 256, scale, pm_pt, pi_pt,
-                                pt_val, pt_idx, colmax, split)
+                                pt_val, pt_idx, colmax, split, row_count=rows_b)
             ops.match_select_colmax(pt_val, pt_idx, colmax, bank["kpts"], img_scale, B, N, hc, wc,
                                     cm.thr, cm.border_rm, cell, scratch, b_ids, i_ids, j_ids, mconf,
-                                    mk3, mkc, count, bank_shared=kshared)
+                                    mk3, mkc, count, bank_shared=kshared, bank_of_batch=bank_of_batch,
+                                    row_count=rows_b)
         else:
             pi_px = self._buf("pi_px", (B * S, tl), i32, dev)
             pm_px = self._buf("pm_px", (B * S, tl), f32, dev)
@@ -874,21 +999,24 @@ class OnePosePlus_model(_Engine):
                              cm.thr, cm.border_rm, cell, scratch, b_ids, i_ids, j_ids, mconf, mk3, mkc,
                              count, bank_shared=kshared)
         if mode == "lazy":
-            conf = LazyConfMatrix(self, d3, q2, lse_pt, lse_px, B, N, S, scale)
+            conf = LazyConfMatrix(self, d3, q2, lse_pt, lse_px, B, N, S, scale, rows_b)
         out.update({"conf_matrix": conf, "b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids, "mconf": mconf,
                     "mkpts_3d_db": mk3, "mkpts_query_c": mkc})
         return count, cap
 
-    def _materialize_conf(self, d3, q2, lse_pt, lse_px, B, N, S, scale):
-        """conf_matrix on demand (LazyConfMatrix): re-runs the conf pass with the fp32 store."""
+    def _materialize_conf(self, d3, q2, lse_pt, lse_px, B, N, S, scale, rows_b=None):
+        """conf_matrix on demand (LazyConfMatrix): re-runs the conf pass with the fp32 store (for a
+        bank set the colmax pass, which stores 0 on the padded rows)."""
         dev = q2.device
         ts = ops.sim_tiles(S)
         conf = torch.empty((B, N, S), dtype=torch.float32, device=dev)
-        ops.sim_conf(d3, q2, lse_pt, lse_px, True, conf, B, N, S, 256, scale,
-                     self._buf("lz_pv", (B * N, ts), torch.float32, dev),
-                     self._buf("lz_pi", (B * N, ts), torch.int32, dev),
-                     self._buf("lz_bv", (B, N), torch.float32, dev),
-                     self._buf("lz_bi", (B, N), torch.int32, dev), self.split)
+        part = (self._buf("lz_pv", (B * N, ts), torch.float32, dev), self._buf("lz_pi", (B * N, ts), torch.int32, dev),
+                self._buf("lz_bv", (B, N), torch.float32, dev), self._buf("lz_bi", (B, N), torch.int32, dev))
+        if rows_b is not None:
+            ops.sim_conf_colmax(d3, q2, lse_pt, lse_px, conf, B, N, S, 256, scale, *part,
+                                self._buf("lz_colmax", (B, S), torch.int32, dev), self.split, row_count=rows_b)
+        else:
+            ops.sim_conf(d3, q2, lse_pt, lse_px, True, conf, B, N, S, 256, scale, *part, self.split)
         return conf
 
     def _fine(self, fine_map, bank, ids, M, img_scale, hc, wc, q_hw_i, out, count=None, pack=None, windows_hw=None):
@@ -914,7 +1042,7 @@ class OnePosePlus_model(_Engine):
         dyn26 = {} if count is None else {"count": count, "rows_per_count": 26}
         ops.fine_gather(fine_map, bank["fine"], b_ids, i_ids, j_ids, None if fine_layers else x32, x[0], M,
                         hf, wf, wc, stride, bank["N"], split, bank_shared=bank["Bb"] == 1,
-                        windows=windows_hw is not None, **dyn)
+                        windows=windows_hw is not None, bank_of_batch=bank.get("bank_of_batch"), **dyn)
         cur = 0
         if fine_layers:
             qkv = self._buf("f_qkv", (rows, pl * 384), f16, dev)
@@ -962,8 +1090,12 @@ class OnePosePlus_model(_Engine):
         scale = data.get("query_image_scale")
         if scale is not None and tuple(scale.shape) != (B, 2):
             raise ValueError(f"query_image_scale must be [B, 2] = [{B}, 2], got {tuple(scale.shape)}")
+        if self._bank_set is not None:
+            given = [k for k in ("keypoints3d", "descriptors3d_db", "descriptors3d_coarse_db") if k in data]
+            if given:
+                raise ValueError(f"a bank set is resident (set_banks): data must not carry {given}")
         if "keypoints3d" not in data:
-            if self._bank is None:
+            if self._bank is None and self._bank_set is None:
                 raise KeyError("data has no 'keypoints3d' and no bank is resident (set_bank)")
             return img, scale, None
         kp, dfine = data["keypoints3d"], data["descriptors3d_db"]
@@ -985,6 +1117,28 @@ class OnePosePlus_model(_Engine):
         if len({kp.shape[0], dfine.shape[0], dco.shape[0]}) != 1:
             raise ValueError("keypoints3d / descriptors3d_db / descriptors3d_coarse_db disagree on the batch size")
         return img, scale, (kp, dco, dfine)
+
+    def _check_object_ids(self, data, B):
+        """data["object_ids"] of a forward with a bank set, validated on the host (a CUDA tensor is
+        read back once): int [B], entries in [0, K).  Returns it as int32 on the host, or None
+        without a bank set."""
+        oid = data.get("object_ids")
+        if self._bank_set is None:
+            if oid is not None:
+                raise ValueError("data has 'object_ids' but no bank set is resident (set_banks)")
+            return None
+        if oid is None:
+            raise ValueError("a bank set is resident (set_banks): data needs 'object_ids' (int [B])")
+        oid = torch.as_tensor(oid)
+        if oid.dtype not in (torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64):
+            raise ValueError(f"object_ids must be an integer tensor, got {oid.dtype}")
+        if tuple(oid.shape) != (B,):
+            raise ValueError(f"object_ids must be [B] = [{B}], got {tuple(oid.shape)}")
+        oid = oid.cpu()
+        K = len(self._bank_set["raw"])
+        if int(oid.min()) < 0 or int(oid.max()) >= K:
+            raise ValueError(f"object_ids entries must be in [0, {K}), got {oid.tolist()}")
+        return oid.to(torch.int32)
 
     # ------------------------------------------------------------------ forward
     def forward(self, data):
@@ -1008,9 +1162,12 @@ class OnePosePlus_model(_Engine):
         enqueues the kernels that write the image — in CUDA-graph mode inside the same graph, with
         `key` added to the graph's signature."""
         img, img_scale, bank_raw = self._check_inputs(data)
+        oid = self._check_object_ids(data, img.shape[0])
         if prologue is not None and (img.dtype != torch.uint8 or not img.is_contiguous()):
             raise ValueError("a prologue writes query_image in place: it must be a contiguous uint8 tensor")
         qmask = data.get("query_image_mask")
+        if qmask is not None and oid is not None:
+            raise NotImplementedError("query_image_mask together with a bank set is not built")
         if qmask is not None:
             # OnePosePlusModel.py:158: mask at coarse resolution, flattened to [B, S]; nonzero = valid
             B_, H_, W_ = img.shape[0], img.shape[2], img.shape[3]
@@ -1030,6 +1187,8 @@ class OnePosePlus_model(_Engine):
             img = img.contiguous()
             if img_scale is not None:
                 img_scale = img_scale.to(device=dev, dtype=torch.float32).contiguous()
+            if oid is not None:   # pinned: the upload does not wait for the stream
+                oid = oid.pin_memory().to(dev, non_blocking=True)
             B, _, H, W = img.shape
             fine_on = self.config["fine_matching"]["enable"]
             data.update({"bs": B, "q_hw_i": img.shape[2:], "q_hw_c": torch.Size((H // 8, W // 8)),
@@ -1039,20 +1198,21 @@ class OnePosePlus_model(_Engine):
             if self.use_cuda_graphs:
                 if qmask is not None:
                     raise NotImplementedError("query_image_mask is not supported in CUDA-graph mode")
-                out, M = self._replay(img, img_scale, bank_raw, fine_on, prologue)
+                out, M = self._replay(img, img_scale, bank_raw, fine_on, prologue, oid=oid)
                 if out is None:
                     # more matches than the captured fine stage holds (exact ties keep every tied row,
                     # so the count can exceed B * min(N, S)): this call runs eagerly, the graph stays
-                    out, count, cap = self._enqueue(img, img_scale, bank_raw, fine_on, dynamic=False)
+                    out, count, cap = self._enqueue(img, img_scale, bank_raw, fine_on, dynamic=False, oid=oid)
                     M = out.pop("M")
             else:
                 if prologue is not None:
                     prologue.run([t.to(dev) for t in prologue.inputs], img)
-                out, count, cap = self._enqueue(img, img_scale, bank_raw, fine_on, dynamic=False, qmask=qmask)
+                out, count, cap = self._enqueue(img, img_scale, bank_raw, fine_on, dynamic=False, qmask=qmask,
+                                                oid=oid)
                 M = out.pop("M")
             self._publish(data, out, M, dev, fine_on)
 
-    def _enqueue(self, img, img_scale, bank_raw, fine_on, dynamic, qmask=None):
+    def _enqueue(self, img, img_scale, bank_raw, fine_on, dynamic, qmask=None, oid=None):
         """The whole forward as kernel launches on the current stream.  dynamic=False: one host
         sync reads the match count M between the coarse and the fine stage (the reference syncs in
         torch.where, coarse_matching.py:170) and the fine stage runs on exactly M matches.
@@ -1070,7 +1230,9 @@ class OnePosePlus_model(_Engine):
         q2, fine_in, (hc, wc) = self._backbone(img, defer_fine=True, fpn_stream=fpn_stream)
         fstride = fine_in.shape[1] // hc
         win_ok = win_ok and fstride == 4
-        if bank_raw is None:
+        if oid is not None:
+            bank = self._set_frame_state(oid, B)
+        elif bank_raw is None:
             bank = self._resident_bank_state()
         else:
             kp, dco, dfine = bank_raw
@@ -1144,15 +1306,20 @@ class OnePosePlus_model(_Engine):
         Python, one host sync at the END (to size the outputs) instead of one in the middle.  The
         results are the same bits as the eager path.  Returned tensors are copies (the graph owns
         its buffers); conf_matrix_mode "eager" therefore costs an extra copy of the matrix —
-        prefer "lazy"/"skip" here."""
+        prefer "lazy"/"skip" here.  With a bank set, pass object_ids as a CPU tensor: a CUDA one
+        is read back to validate it before any launch, which waits for the work queued before the
+        forward (a second host sync)."""
         self.use_cuda_graphs = bool(on)
         if not on:
             self._graphs = {}
         return self
 
-    def _replay(self, img, img_scale, bank_raw, fine_on, prologue=None):
+    def _replay(self, img, img_scale, bank_raw, fine_on, prologue=None, oid=None):
         resident = bank_raw is None
-        if resident:
+        if oid is not None:
+            # object_ids is a graph input: one graph per bank set serves every assignment
+            bkey = ("set", id(self._bank_set))
+        elif resident:
             bkey = ("resident", id(self._bank))
         else:
             one = bank_raw[0].shape[0] == 1 or (img.shape[0] > 1 and all(t.stride(0) == 0 for t in bank_raw))
@@ -1187,21 +1354,25 @@ class OnePosePlus_model(_Engine):
                     for d, t in zip(s_bank, bank_raw):
                         d.copy_(t)
             load()
+            s_oid = None if oid is None else oid.clone()
             # warm-up outside the capture: sizes the workspace, sets kernel attributes
             if s_pro is not None:
                 prologue.run(s_pro, s_img)
-            self._enqueue(s_img, s_scale, s_bank, fine_on, dynamic=True)
+            self._enqueue(s_img, s_scale, s_bank, fine_on, dynamic=True, oid=s_oid)
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             count_host = torch.empty(1, dtype=torch.int32, pin_memory=True)
             with torch.cuda.graph(g):
                 if s_pro is not None:
                     prologue.run(s_pro, s_img)   # first node: query_image from the prologue's inputs
-                out, count, cap = self._enqueue(s_img, s_scale, s_bank, fine_on, dynamic=True)
+                out, count, cap = self._enqueue(s_img, s_scale, s_bank, fine_on, dynamic=True, oid=s_oid)
                 count_host.copy_(count, non_blocking=True)   # last node of the graph: M lands in pinned memory
             out["gt_mask"].zero_()
             ent = {"graph": g, "out": out, "count": count_host, "ws_epoch": self._ws_epoch,
-                   "inputs": (s_img, s_scale, s_bank, s_pro)}
+                   "inputs": (s_img, s_scale, s_bank, s_pro), "oid": s_oid,
+                   # the key holds id() of the resident bank / set: holding the object keeps that id
+                   # from being reused by a later set_bank / set_banks while this graph exists
+                   "bank_ref": self._bank_set if oid is not None else (self._bank if resident else None)}
             self._graphs[key] = ent
         s_img, s_scale, s_bank, s_pro = ent["inputs"]
         if s_pro is None:
@@ -1214,6 +1385,8 @@ class OnePosePlus_model(_Engine):
         if s_bank is not None:
             for d, t in zip(s_bank, bank_raw):
                 d.copy_(t)
+        if oid is not None:
+            ent["oid"].copy_(oid)
         ent["graph"].replay()
         if s_pro is not None:
             img.copy_(s_img)   # the caller's query_image receives what the prologue wrote
@@ -1259,8 +1432,8 @@ class LazyConfMatrix:
     somebody asks (`.materialize()` / `torch.as_tensor(handle.materialize())`).  Valid until the
     model's next forward (it reads the model's workspace)."""
 
-    def __init__(self, model, d3, q2, lse_pt, lse_px, B, N, S, scale):
-        self._model, self._args = model, (d3, q2, lse_pt, lse_px, B, N, S, scale)
+    def __init__(self, model, d3, q2, lse_pt, lse_px, B, N, S, scale, rows_b=None):
+        self._model, self._args = model, (d3, q2, lse_pt, lse_px, B, N, S, scale, rows_b)
         self._epoch = model._fwd_count
         self.shape = torch.Size((B, N, S))
         self._value = None

@@ -174,15 +174,22 @@ def sim_conf(a, b, lse_own, lse_other, own_is_pt, conf, batches, rows, cols, k, 
 
 
 def sim_lse_cols(a, b, batches, rows, cols, k, scale, part_m, part_s, lse_rows, col_m, col_s, lse_cols,
-                 split, col_mask=None, side_stream=None):
+                 split, col_mask=None, side_stream=None, row_count=None):
     """lse over columns for every row (as sim_lse) AND lse over rows for every column, one GEMM pass.
     col_mask uint8 [batches, cols]: masked columns (0) get sim - 1e9 and lse_cols = +inf (conf = 0).
+    row_count int32 [batches] (bank sets): rows past the count drop out of lse_cols; their lse_rows
+    are not meaningful.
     side_stream (latency mode): the two independent finalisers run side by side."""
     _chk(col_mask, torch.uint8, "col_mask")
+    _chk(row_count, torch.int32, "row_count")
     tiles = sim_tiles(cols)
     groups = (rows + 31) // 32
-    call("opp_sim_lse_cols", ptr(a), ptr(b), ptr(part_m), ptr(part_s), ptr(col_m), ptr(col_s), batches,
-         rows, cols, k, float(scale), int(split), ptr(col_mask), stream())
+    if row_count is not None:
+        call("opp_sim_lse_cols_rows", ptr(a), ptr(b), ptr(part_m), ptr(part_s), ptr(col_m), ptr(col_s), batches,
+             rows, cols, k, float(scale), int(split), ptr(col_mask), ptr(row_count), stream())
+    else:
+        call("opp_sim_lse_cols", ptr(a), ptr(b), ptr(part_m), ptr(part_s), ptr(col_m), ptr(col_s), batches,
+             rows, cols, k, float(scale), int(split), ptr(col_mask), stream())
     if side_stream is not None:
         cur = torch.cuda.current_stream()
         side_stream.wait_stream(cur)
@@ -197,17 +204,34 @@ def sim_lse_cols(a, b, batches, rows, cols, k, scale, part_m, part_s, lse_rows, 
 
 
 def sim_conf_colmax(a, b, lse_own, lse_other, conf, batches, rows, cols, k, scale, part_val, part_idx,
-                    best_val, best_idx, colmax, split):
-    """conf pass over rows = 3D points that also leaves max_l conf[b, l, s] (float bits) in colmax."""
+                    best_val, best_idx, colmax, split, row_count=None):
+    """conf pass over rows = 3D points that also leaves max_l conf[b, l, s] (float bits) in colmax.
+    row_count int32 [batches] (bank sets): rows past the count stay out of colmax and store conf 0."""
+    _chk(row_count, torch.int32, "row_count")
     tiles = sim_tiles(cols)
-    call("opp_sim_conf_colmax", ptr(a), ptr(b), ptr(lse_own), ptr(lse_other), ptr(conf), ptr(part_val),
-         ptr(part_idx), ptr(colmax), batches, rows, cols, k, float(scale), int(split), stream())
+    if row_count is not None:
+        call("opp_sim_conf_colmax_rows", ptr(a), ptr(b), ptr(lse_own), ptr(lse_other), ptr(conf), ptr(part_val),
+             ptr(part_idx), ptr(colmax), batches, rows, cols, k, float(scale), int(split), ptr(row_count), stream())
+    else:
+        call("opp_sim_conf_colmax", ptr(a), ptr(b), ptr(lse_own), ptr(lse_other), ptr(conf), ptr(part_val),
+             ptr(part_idx), ptr(colmax), batches, rows, cols, k, float(scale), int(split), stream())
     call("opp_best_finalize", ptr(part_val), ptr(part_idx), ptr(best_val), ptr(best_idx),
          batches * rows, tiles, stream())
 
 
 def match_select_colmax(pt_val, pt_idx, colmax, kpts, img_scale, batch, l, hc, wc, thr, border, cell,
-                        scratch, b_ids, i_ids, j_ids, mconf, mkpts3d, mkpts_c, count, bank_shared=False):
+                        scratch, b_ids, i_ids, j_ids, mconf, mkpts3d, mkpts_c, count, bank_shared=False,
+                        bank_of_batch=None, row_count=None):
+    """bank_of_batch / row_count int32 [batch] (bank sets, both or neither): kpts is [K, l, 3], read at
+    the frame's object, and rows past the frame's count never match."""
+    if bank_of_batch is not None or row_count is not None:
+        _chk(bank_of_batch, torch.int32, "bank_of_batch")
+        _chk(row_count, torch.int32, "row_count")
+        call("opp_match_select_colmax_set", ptr(pt_val), ptr(pt_idx), ptr(colmax), ptr(kpts), ptr(img_scale),
+             batch, l, hc, wc, float(thr), int(border), float(cell), ptr(scratch), ptr(b_ids),
+             ptr(i_ids), ptr(j_ids), ptr(mconf), ptr(mkpts3d), ptr(mkpts_c), ptr(count), int(bank_shared),
+             ptr(bank_of_batch), ptr(row_count), stream())
+        return
     call("opp_match_select_colmax", ptr(pt_val), ptr(pt_idx), ptr(colmax), ptr(kpts), ptr(img_scale),
          batch, l, hc, wc, float(thr), int(border), float(cell), ptr(scratch), ptr(b_ids),
          ptr(i_ids), ptr(j_ids), ptr(mconf), ptr(mkpts3d), ptr(mkpts_c), ptr(count), int(bank_shared), stream())
@@ -292,12 +316,19 @@ def coarse_focal_bwd(a, b, st_rows, st_cols, r, c, wts, grad, gt, col_mask, scal
 
 
 def fine_gather(fine, desc3d, b_ids, i_ids, j_ids, x32, x16, m, hf, wf, wc, stride, n, split,
-                bank_shared=False, count=None, windows=False):
-    """windows: `fine` is the compact [m, 5, 8, planes*128] window tensor of conv_win."""
+                bank_shared=False, count=None, windows=False, bank_of_batch=None):
+    """windows: `fine` is the compact [m, 5, 8, planes*128] window tensor of conv_win.
+    bank_of_batch int32 [B] (bank sets): desc3d is [K, 128, n], read at the frame's object."""
     _chk(desc3d, torch.float32, "descriptors3d_db")
+    win = conv_win_pitch(5) if windows is True else int(windows)
+    if bank_of_batch is not None:
+        _chk(bank_of_batch, torch.int32, "bank_of_batch")
+        call("opp_fine_gather_set", ptr(fine), ptr(desc3d), ptr(b_ids), ptr(i_ids), ptr(j_ids), ptr(x32),
+             ptr(x16), m, hf, wf, wc, stride, n, int(split), int(bank_shared), win, ptr(count),
+             ptr(bank_of_batch), stream())
+        return
     call("opp_fine_gather", ptr(fine), ptr(desc3d), ptr(b_ids), ptr(i_ids), ptr(j_ids), ptr(x32),
-         ptr(x16), m, hf, wf, wc, stride, n, int(split), int(bank_shared),
-         (conv_win_pitch(5) if windows is True else int(windows)), ptr(count), stream())
+         ptr(x16), m, hf, wf, wc, stride, n, int(split), int(bank_shared), win, ptr(count), stream())
 
 
 def conv_win_pitch(win):

@@ -338,7 +338,9 @@ class PoseTracker:
 
     model: an eval-mode OnePosePlus_model on the GPU with the object's 3D bank resident
     (``model.set_bank``); K: the original intrinsics [3, 3] (shared) or [B, 3, 3]; bbox3d: the
-    8 corners [8, 3] of the object's 3D box.
+    8 corners [8, 3] of the object's 3D box.  With a bank set (``model.set_banks``, several objects
+    in one forward): bbox3d is [K_obj, 8, 3], one box per object, and object_ids (int [B]) gives each
+    sequence's object; its crop uses its object's box and its frame is matched against its object.
 
     ``step(frames_u8, init_bbox=None)``: frames uint8 [B, H, W] (CUDA, host array, or a list of
     arrays / paths); init_bbox: None, or B entries of None or (x0, y0, x1, y1).  A sequence whose
@@ -349,9 +351,12 @@ class PoseTracker:
     [4, 4], inliers (int64 indices into the frame's matches, as ransac_PnP returns them), state,
     mkpts_3d_db and mkpts_query_f (the frame's matches, CUDA)."""
 
-    def __init__(self, model, K, bbox3d, reprojection_error=7, crop_size=512):
-        if getattr(model, "_bank", None) is None:
+    def __init__(self, model, K, bbox3d, reprojection_error=7, crop_size=512, object_ids=None):
+        bank_set = getattr(model, "_bank_set", None)
+        if getattr(model, "_bank", None) is None and bank_set is None:
             raise ValueError("PoseTracker needs the object's 3D bank resident: call model.set_bank(...) first")
+        if (bank_set is None) != (object_ids is None):
+            raise ValueError("object_ids goes with a bank set (model.set_banks) and only with one")
         _check_side(crop_size, "crop_size")
         if crop_size % 8 or crop_size < 16:
             raise ValueError(f"crop_size must be a multiple of 8 (>= 16) for the matcher, got {crop_size}")
@@ -359,7 +364,19 @@ class PoseTracker:
         self.K = np.asarray(K, dtype=np.float64)
         if self.K.shape[-2:] != (3, 3) or self.K.ndim not in (2, 3):
             raise ValueError(f"K must be [3, 3] or [B, 3, 3], got {self.K.shape}")
-        self.bbox3d = np.asarray(bbox3d, dtype=np.float64).reshape(-1, 3)
+        self.object_ids = None
+        if bank_set is None:
+            self.bbox3d = np.asarray(bbox3d, dtype=np.float64).reshape(-1, 3)
+        else:
+            n_obj = len(bank_set["raw"])
+            self.bbox3d = np.asarray(bbox3d, dtype=np.float64)
+            if self.bbox3d.shape != (n_obj, 8, 3):
+                raise ValueError(f"bbox3d must be [K_obj, 8, 3] = [{n_obj}, 8, 3] with a bank set, "
+                                 f"got {self.bbox3d.shape}")
+            self.object_ids = np.asarray(object_ids)
+            if self.object_ids.ndim != 1 or self.object_ids.dtype.kind not in "iu" \
+                    or self.object_ids.min(initial=0) < 0 or self.object_ids.max(initial=0) >= n_obj:
+                raise ValueError(f"object_ids must be ints in [0, {n_obj}), got {object_ids}")
         self.reprojection_error = float(reprojection_error)
         self.crop_size = int(crop_size)
         self._pose = None
@@ -379,12 +396,22 @@ class PoseTracker:
     def _K(self, b):
         return self.K if self.K.ndim == 2 else self.K[b]
 
+    def _box3d(self, b):
+        return self.bbox3d if self.object_ids is None else self.bbox3d[self.object_ids[b]]
+
     def step(self, frames_u8, init_bbox=None):
+        if self.object_ids is not None:
+            bank_set = getattr(self.model, "_bank_set", None)   # set_banks may have run since __init__
+            if bank_set is None or len(bank_set["raw"]) != len(self.bbox3d):
+                raise ValueError(f"PoseTracker was built for a set of {len(self.bbox3d)} objects; the model "
+                                 f"now holds {'no set' if bank_set is None else len(bank_set['raw'])}")
         frames = _frames(frames_u8, device=torch.device("cuda", torch.cuda.current_device())
                          if not (torch.is_tensor(frames_u8) and frames_u8.is_cuda) else None)
         B = frames.shape[0]
         if self.K.ndim == 3 and self.K.shape[0] != B:
             raise ValueError(f"K holds {self.K.shape[0]} cameras for {B} sequences")
+        if self.object_ids is not None and len(self.object_ids) != B:
+            raise ValueError(f"object_ids holds {len(self.object_ids)} objects for {B} sequences")
         if self._pose is None:
             self._pose, self._n_inliers = [None] * B, [0] * B
         if len(self._pose) != B:
@@ -402,7 +429,7 @@ class PoseTracker:
                     raise ValueError(f"init_bbox[{b}] must be (x0, y0, x1, y1), got shape {box.shape}")
                 box = box.astype(np.int32) if box.dtype.kind == "f" else box
             elif self._pose[b] is not None and self._n_inliers[b] >= MIN_INLIERS:
-                box = bbox_from_pose(self._K(b), self._pose[b], self.bbox3d)
+                box = bbox_from_pose(self._K(b), self._pose[b], self._box3d(b))
             else:
                 continue
             active.append(b)
@@ -417,6 +444,8 @@ class PoseTracker:
         with torch.cuda.device(dev):
             crops = torch.empty((n, 1, self.crop_size, self.crop_size), dtype=torch.uint8, device=dev)
             data = {"query_image": crops}
+            if self.object_ids is not None:
+                data["object_ids"] = torch.as_tensor(self.object_ids[active], dtype=torch.int32)
             self.model._forward(data, prologue=_CropPrologue(sel, rec))
             Kc = torch.as_tensor(np.stack(K_crop), dtype=torch.float32).to(dev)
             r = pnp.ransac_pnp_batched(data["m_bids"], data["mkpts_3d_db"], data["mkpts_query_f"], Kc,
