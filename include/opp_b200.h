@@ -496,6 +496,51 @@ int opp_coarse_focal_bwd(const float* a, const float* b, const float* st_rows, c
                          int gt_bytes, const unsigned char* col_mask, int batches, int rows, int cols, int k,
                          float scale, float alpha, float gamma, float* da, float* db, opp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training, sparse ground truth — the positives of conf_matrix_gt as a list (b_ids, i_ids, j_ids
+ * int64 [g], ascending in (b, i, j), no duplicates: the order of torch.where on the dense matrix)
+ * with their fine locations fine_xy fp32 [g][2], instead of the [B, L, S] and [B, L, S, 2] tensors.
+ * ---------------------------------------------------------------------------------------- */
+
+/* Index of the list by 3D point and by query cell.
+ *   row_ptr int32 [B*rows + 1]: entries of row b*rows + i are [row_ptr[r], row_ptr[r + 1]).
+ *   col_ptr int32 [B*cols + 1], col_rows int32 [g]: the i of the entries of column b*cols + j,
+ *   ascending, at [col_ptr[c], col_ptr[c + 1]).  fill int32 [B*cols]: workspace.
+ *   Several j per i and several i per j are legal; entries out of range are left out of the column
+ *   view.  The result does not depend on launch order (integer atomics hand out slots, each
+ *   bucket is then sorted; one thread sorts one bucket by insertion, which is quadratic in the
+ *   number of 3D points of one cell). */
+int opp_gt_index(const long long* b_ids, const long long* i_ids, const long long* j_ids, int g, int batches,
+                 int rows, int cols, int* row_ptr, int* col_ptr, int* col_rows, int* fill, opp_stream_t stream);
+
+/* opp_coarse_focal_fwd / _bwd with the class of an element taken from the list: 1 for a listed
+ * (b, i, j), 0 for every other element.  row_ptr / col_ptr / col_rows from opp_gt_index of the same
+ * list.  The arithmetic is that of the dense entry points, instruction for instruction: every output
+ * has the bits the dense call gives on the dense form of the list. */
+int opp_coarse_focal_fwd_sparse(const float* a, const float* b, const float* st_rows, const float* st_cols,
+                                const int* row_ptr, const long long* j_ids, const unsigned char* col_mask,
+                                int batches, int rows, int cols, int k, float scale, float alpha, float gamma,
+                                float pos_w, float neg_w, double* part_loss, long long* part_cnt, double* part_r,
+                                double* part_c, float* loss, long long* counts, float* wts, double* r, double* c,
+                                opp_stream_t stream);
+
+int opp_coarse_focal_bwd_sparse(const float* a, const float* b, const float* st_rows, const float* st_cols,
+                                const double* r, const double* c, const float* wts, const float* grad,
+                                const int* row_ptr, const long long* j_ids, const int* col_ptr, const int* col_rows,
+                                const unsigned char* col_mask, int batches, int rows, int cols, int k, float scale,
+                                float alpha, float gamma, float* da, float* db, opp_stream_t stream);
+
+/* fine_supervision (src/models/OnePosePlus/utils/fine_supervision.py) from the list: for each of
+ * the m matches (m_b, m_i, m_j int64) the fine location of (b, i, j), (-50, -50) when it is not in
+ * the list, minus the cell's origin (j % w_c, j / w_c) * coarse scale, over the fine scale and the
+ * window radius.  resolution = (coarse_res, fine_res).  img_scale fp32 [B][2] (query_image_scale,
+ * (h, w) order) multiplies both scales; with img_scale NULL the coarse scale is fine_res, as in the
+ * reference.  out fp32 [m][2]: the bits PyTorch's fp32 evaluation of the reference gives on the device. */
+int opp_fine_supervision(const long long* b_ids, const long long* i_ids, const long long* j_ids,
+                         const float* fine_xy, int g, int batches, int rows, int cols, const long long* m_b,
+                         const long long* m_i, const long long* m_j, int m, int w_c, int coarse_res, int fine_res,
+                         int radius, const float* img_scale, float* out, opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

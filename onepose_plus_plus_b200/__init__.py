@@ -8,5 +8,6 @@ from .model import LazyConfMatrix, OnePosePlus_model, build_backbone  # noqa: F4
 from .loftr import LoFTR_for_OnePose_Plus  # noqa: F401  (2D-2D matcher of the SfM / demo stages)
 from . import pnp  # noqa: F401  (device-side RANSAC-PnP front end: metric_utils.ransac_PnP)
 from . import tracking  # noqa: F401  (demo tracking step: bbox crop on the device, PoseTracker)
+from .train_gt import SparseGT, SparseGTDataset, collate_sparse_gt, sparse_gt_sample  # noqa: F401  (training: sparse ground truth)
 
 __version__ = "0.2.0"

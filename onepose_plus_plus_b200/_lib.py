@@ -66,6 +66,10 @@ SIGNATURES = {
     "opp_coarse_focal_stats": [P, P, P, I, I, I, I, F, P, P, P, P],
     "opp_coarse_focal_fwd": [P, P, P, P, P, I, P, I, I, I, I, F, F, F, F, F] + [P] * 10,
     "opp_coarse_focal_bwd": [P] * 9 + [I, P, I, I, I, I, F, F, F, P, P, P],
+    "opp_gt_index": [P, P, P, I, I, I, I, P, P, P, P, P],
+    "opp_coarse_focal_fwd_sparse": [P] * 7 + [I, I, I, I, F, F, F, F, F] + [P] * 10,
+    "opp_coarse_focal_bwd_sparse": [P] * 13 + [I, I, I, I, F, F, F, P, P, P],
+    "opp_fine_supervision": [P, P, P, P, I, I, I, I, P, P, P, I, I, I, I, I, P, P, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),
@@ -110,7 +114,8 @@ def stream():
 # kernels launched per entry point (bench.py reports the per-step total as gpu_launches)
 KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_match_select_colmax_set": 3,
                     "opp_pose_metrics": 3,
-                    "opp_coarse_focal_stats": 2, "opp_coarse_focal_fwd": 3, "opp_coarse_focal_bwd": 2}
+                    "opp_coarse_focal_stats": 2, "opp_coarse_focal_fwd": 3, "opp_coarse_focal_bwd": 2,
+                    "opp_gt_index": 5, "opp_coarse_focal_fwd_sparse": 3, "opp_coarse_focal_bwd_sparse": 2}
 LAUNCHES = 0
 _PROFILE = None
 

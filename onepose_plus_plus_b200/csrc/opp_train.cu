@@ -9,6 +9,9 @@
 //   Backward: w = pos_w / npos or neg_w / nneg, gc = w c dl/dc (0 where the clamp is active),
 //   R_i = sum_j gc_ij, C_j = sum_i gc_ij, dsim = go (2 gc - p C - q R), dA = s dsim B, dB = s dsim^T A.
 //   Masked query columns (query_image_mask) have c = p = q = 0 and dsim = 0.
+//   The ground truth is the dense [B, L, S] class matrix or, in the _sparse entry points, the sorted
+//   list of its positives (opp_gt_index); the arithmetic is the same instructions either way.  The
+//   fine level's ground truth offsets (fine_supervision) are looked up in the same list.
 //
 // One kernel shape serves every pass: a CTA keeps 64 "own" feature rows in shared memory and
 // streams the other side in 64-row tiles; each tile's 64 x 64 block of sim is recomputed in fp32
@@ -28,6 +31,7 @@
 // Every sum runs in a fixed order (no atomics), so results are bit-reproducible.
 #include <cmath>
 #include <cstdint>
+#include <type_traits>
 
 #include "../../include/opp_b200.h"
 #include "opp_common.cuh"
@@ -41,6 +45,7 @@ constexpr int kFP = kFT + 4;       // shared pitch (floats) of the [k][row] tile
 constexpr int kFThreads = 256;
 constexpr size_t kFSmem = (2 * (size_t)kFK * kFP + (size_t)kFT * kFP + 6 * kFT) * sizeof(float) +
                           2 * kFT * sizeof(double);
+constexpr size_t kFSmemSparse = kFSmem + kFT * sizeof(unsigned long long);   // + the tile's class bits
 
 enum FocalPass { kStats = 0, kFwd = 1, kBwd = 2 };
 
@@ -74,6 +79,16 @@ __device__ __forceinline__ int gt_class(const void* gt, int gt_bytes, long long 
                               : (int)static_cast<const unsigned char*>(gt)[idx];
   return v == 1 ? 1 : (v == 0 ? 0 : -1);
 }
+
+// The ground truth of a launch.  Dense: the [B][L][S] class matrix.  Sparse: the positives as a
+// list — per own row a bucket [ptr[r], ptr[r + 1]) of `ids`, ascending along the streamed side
+// (own = 3D points: ptr = row_ptr, ids = the list's int64 j_ids; own = query cells: ptr = col_ptr,
+// ids = int32 col_rows of opp_gt_index); every element outside the list is a negative.
+typedef const void* __restrict__ DenseGt;
+struct SparseGt {
+  const int* ptr;
+  const void* ids;
+};
 
 // running (max, sum exp(x - max)); m = -inf, s = 0 is the empty set
 __device__ __forceinline__ void lse_add(float& m, float& s, float x) {
@@ -113,17 +128,20 @@ __device__ __forceinline__ void load_tile_t(float* xs, const float* __restrict__
 // kPass kStats / kFwd (own = rows = 3D points) or kBwd (own = rows when kOwnRows, else query cells).
 // grid (ceil(n_own / 64), B).  st_own / st_oth: (m, log s) statistics of the own / other side (the
 // softmax of an own row runs over the other side).  gt [B][L][S] (1 or 2 bytes), col_mask [B][S] or NULL.
-template <int kPass, bool kOwnRows>
+// kSparse: gt is a SparseGt; per tile, thread r < 64 writes the 64 class bits of own row r from its
+// bucket, which it walks once over the whole launch (the streamed index only grows).
+template <int kPass, bool kOwnRows, bool kSparse>
 __global__ void __launch_bounds__(kFThreads, 1)
 coarse_focal_kernel(const float* __restrict__ own, const float* __restrict__ oth,
                     const float2* __restrict__ st_own, const float2* __restrict__ st_oth,
                     const double* __restrict__ stat_own, const double* __restrict__ stat_oth,
                     const float* __restrict__ wts, const float* __restrict__ grad,
-                    const void* __restrict__ gt, int gt_bytes, const unsigned char* __restrict__ col_mask,
-                    int n_own, int n_oth, float scale, FocalCfg f,
+                    typename std::conditional<kSparse, SparseGt, DenseGt>::type gt, int gt_bytes,
+                    const unsigned char* __restrict__ col_mask, int n_own, int n_oth, float scale, FocalCfg f,
                     double* __restrict__ part_loss, long long* __restrict__ part_cnt,
                     void* __restrict__ part_r_, void* __restrict__ part_c_, float* __restrict__ d_own) {
   static_assert(kPass == kBwd || kOwnRows, "statistics and forward run with the 3D points as own rows");
+  static_assert(kPass != kStats || !kSparse, "the statistics read no ground truth");
   extern __shared__ __align__(16) float smem[];
   float* xs = smem;                          // [256][kFP] own rows, transposed
   float* ys = xs + kFK * kFP;                // [256][kFP] other tile, transposed
@@ -136,6 +154,7 @@ coarse_focal_kernel(const float* __restrict__ own, const float* __restrict__ oth
   float* s_mask_oth = s_mask_own + kFT;      // [64]
   double* s_stat_own = reinterpret_cast<double*>(s_mask_oth + kFT);   // [64] R or C of the own rows (bwd)
   double* s_stat_oth = s_stat_own + kFT;     // [64]
+  unsigned long long* s_bits = reinterpret_cast<unsigned long long*>(s_stat_oth + kFT);   // [64] (kSparse)
   // statistics: part_r = (m, log s) per row, part_c = (m, s) per (CTA, column), fp32;
   // forward: part_r = (pos, neg) R per row, part_c = (pos, neg) C per (CTA, column), fp64
   float2* st_part_r = static_cast<float2*>(part_r_);
@@ -160,6 +179,14 @@ coarse_focal_kernel(const float* __restrict__ own, const float* __restrict__ oth
     s_l_own[tid] = st.y;
     s_stat_own[tid] = (kPass == kBwd && in) ? stat_own[(long long)b * n_own + o] : 0.0;
     s_mask_own[tid] = (kOwnRows || !mask || (in && mask[o])) ? 1.f : 0.f;
+  }
+  // sparse ground truth: the unread rest [cur, end) of own row tid's bucket (threads tid < 64)
+  int cur = 0, end = 0;
+  if constexpr (kSparse) {
+    if (tid < kFT && o0 + tid < n_own) {
+      cur = gt.ptr[(long long)b * n_own + o0 + tid];
+      end = gt.ptr[(long long)b * n_own + o0 + tid + 1];
+    }
   }
   float go = 0.f, wpos = 0.f, wneg = 0.f;
   if (kPass == kBwd) {
@@ -195,6 +222,16 @@ coarse_focal_kernel(const float* __restrict__ own, const float* __restrict__ oth
       s_l_oth[tid] = st.y;
       s_stat_oth[tid] = (kPass == kBwd && in) ? stat_oth[(long long)b * n_oth + o] : 0.0;
       s_mask_oth[tid] = (!kOwnRows || !mask || (in && mask[o])) ? 1.f : 0.f;
+      if constexpr (kSparse) {
+        unsigned long long bits = 0;
+        for (; cur < end; ++cur) {
+          const long long id = kOwnRows ? static_cast<const long long*>(gt.ids)[cur]
+                                        : (long long)static_cast<const int*>(gt.ids)[cur];
+          if (id >= t0 + kFT) break;
+          if (id >= t0) bits |= 1ull << (int)(id - t0);
+        }
+        s_bits[tid] = bits;
+      }
     }
     __syncthreads();
 
@@ -259,8 +296,13 @@ coarse_focal_kernel(const float* __restrict__ own, const float* __restrict__ oth
         const float p_row = expf(lp_row), p_col = expf(lp_col);
         const float conf = p_row * p_col;
         const float om = kept ? -expm1f(lp_row + lp_col) : 1.f;
-        const long long gi = kOwnRows ? gt0 + (long long)o * S + j : gt0 + (long long)j * S + o;
-        const int cls = gt_class(gt, gt_bytes, gi);
+        int cls;
+        if constexpr (kSparse) {
+          cls = (int)((s_bits[ro] >> rc) & 1ull);
+        } else {
+          const long long gi = kOwnRows ? gt0 + (long long)o * S + j : gt0 + (long long)j * S + o;
+          cls = gt_class(gt, gt_bytes, gi);
+        }
         float l, gc;
         focal_term(conf, om, cls, f, l, gc);
         if (kPass == kFwd) {
@@ -476,18 +518,154 @@ __global__ void coarse_focal_rc_kernel(const double2* __restrict__ part_r, const
   }
 }
 
-template <int kPass, bool kOwnRows>
+template <int kPass, bool kOwnRows, bool kSparse>
 cudaError_t launch_focal(dim3 grid, cudaStream_t st, const float* own, const float* oth, const float2* st_own,
                          const float2* st_oth, const double* stat_own, const double* stat_oth,
-                         const float* wts, const float* grad, const void* gt, int gt_bytes, const unsigned char* mask,
-                         int n_own, int n_oth, float scale, FocalCfg f, double* pl, long long* pc, void* pr, void* pcc,
-                         float* d_own) {
-  auto kern = coarse_focal_kernel<kPass, kOwnRows>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFSmem);
+                         const float* wts, const float* grad,
+                         typename std::conditional<kSparse, SparseGt, const void*>::type gt, int gt_bytes,
+                         const unsigned char* mask, int n_own, int n_oth, float scale, FocalCfg f, double* pl,
+                         long long* pc, void* pr, void* pcc, float* d_own) {
+  auto kern = coarse_focal_kernel<kPass, kOwnRows, kSparse>;
+  constexpr size_t smem = kSparse ? kFSmemSparse : kFSmem;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return e;
-  kern<<<grid, kFThreads, kFSmem, st>>>(own, oth, st_own, st_oth, stat_own, stat_oth, wts, grad, gt, gt_bytes,
-                                        mask, n_own, n_oth, scale, f, pl, pc, pr, pcc, d_own);
+  kern<<<grid, kFThreads, smem, st>>>(own, oth, st_own, st_oth, stat_own, stat_oth, wts, grad, gt, gt_bytes, mask,
+                                      n_own, n_oth, scale, f, pl, pc, pr, pcc, d_own);
   return cudaGetLastError();
+}
+
+// ---- sparse ground truth: the positives as a list sorted by (b, i, j) ----------------------------
+
+// row_ptr[r] = first entry whose row b L + i is >= r (r = 0 .. B L): one thread per row
+__global__ void gt_row_ptr_kernel(const long long* __restrict__ b_ids, const long long* __restrict__ i_ids, int g,
+                                  int rows, long long n_rows, int* __restrict__ row_ptr) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r > n_rows) return;
+  int lo = 0, hi = g;
+  while (lo < hi) {
+    const int mid = lo + (hi - lo) / 2;
+    if (b_ids[mid] * rows + i_ids[mid] < r) lo = mid + 1;
+    else hi = mid;
+  }
+  row_ptr[r] = lo;
+}
+
+__device__ __forceinline__ bool gt_in_range(long long b, long long i, long long j, int batches, int rows, int cols) {
+  return b >= 0 && b < batches && i >= 0 && i < rows && j >= 0 && j < cols;
+}
+
+// col_ptr[1 + b S + j] += 1 per entry (col_ptr zeroed before)
+__global__ void gt_col_count_kernel(const long long* __restrict__ b_ids, const long long* __restrict__ i_ids,
+                                    const long long* __restrict__ j_ids, int g, int batches, int rows, int cols,
+                                    int* __restrict__ col_ptr) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= g || !gt_in_range(b_ids[e], i_ids[e], j_ids[e], batches, rows, cols)) return;
+  atomicAdd(col_ptr + 1 + b_ids[e] * cols + j_ids[e], 1);
+}
+
+// in-place inclusive scan of x[0 .. n) by one CTA, 1024 elements per round with a running carry
+__global__ void __launch_bounds__(1024) gt_scan_kernel(int* __restrict__ x, long long n) {
+  __shared__ int warp_sum[32];
+  __shared__ int carry_s;
+  const int tid = threadIdx.x, lane = tid % 32, warp = tid / 32;
+  if (tid == 0) carry_s = 0;
+  __syncthreads();
+  for (long long base = 0; base < n; base += 1024) {
+    const long long idx = base + tid;
+    int v = idx < n ? x[idx] : 0;
+    for (int d = 1; d < 32; d <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, v, d);
+      if (lane >= d) v += u;
+    }
+    if (lane == 31) warp_sum[warp] = v;
+    __syncthreads();
+    if (warp == 0) {
+      int w = warp_sum[lane];
+      for (int d = 1; d < 32; d <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, w, d);
+        if (lane >= d) w += u;
+      }
+      warp_sum[lane] = w;
+    }
+    __syncthreads();
+    const int carry = carry_s;
+    v += carry + (warp ? warp_sum[warp - 1] : 0);
+    if (idx < n) x[idx] = v;
+    __syncthreads();
+    if (tid == 1023) carry_s = v;
+    __syncthreads();
+  }
+}
+
+// col_rows[col_ptr[c] + slot] = i, slot handed out by an integer atomic (fill zeroed before); the
+// order inside a bucket is settled by gt_col_sort_kernel
+__global__ void gt_col_scatter_kernel(const long long* __restrict__ b_ids, const long long* __restrict__ i_ids,
+                                      const long long* __restrict__ j_ids, int g, int batches, int rows, int cols,
+                                      const int* __restrict__ col_ptr, int* __restrict__ fill,
+                                      int* __restrict__ col_rows) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= g || !gt_in_range(b_ids[e], i_ids[e], j_ids[e], batches, rows, cols)) return;
+  const long long c = b_ids[e] * cols + j_ids[e];
+  col_rows[col_ptr[c] + atomicAdd(fill + c, 1)] = (int)i_ids[e];
+}
+
+// each column's bucket ascending in i (insertion sort, one thread per column: a bucket holds the 3D
+// points of one query cell, a handful at most), so the result does not depend on the scatter's order
+__global__ void gt_col_sort_kernel(const int* __restrict__ col_ptr, long long n_cols, int* __restrict__ col_rows) {
+  const long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_cols) return;
+  const int lo = col_ptr[c], hi = col_ptr[c + 1];
+  for (int x = lo + 1; x < hi; ++x) {
+    const int v = col_rows[x];
+    int y = x - 1;
+    for (; y >= lo && col_rows[y] > v; --y) col_rows[y + 1] = col_rows[y];
+    col_rows[y + 1] = v;
+  }
+}
+
+// fine_supervision (src/models/OnePosePlus/utils/fine_supervision.py:18-28) for one match per
+// thread: (b, i, j) looked up in the sorted list -> its fine location, or (-50, -50) when it is not
+// ground truth.  Every operation is a separately rounded fp32 one in the reference's order; the
+// scalar divisions are multiplications by the fp32 reciprocal, as PyTorch evaluates tensor / scalar
+// on the device.
+__global__ void fine_supervision_kernel(const long long* __restrict__ gb, const long long* __restrict__ gi,
+                                        const long long* __restrict__ gj, const float* __restrict__ fine_xy, int g,
+                                        const long long* __restrict__ mb, const long long* __restrict__ mi,
+                                        const long long* __restrict__ mj, int m, int w_c, int coarse_res,
+                                        int fine_res, float inv_fine, float inv_radius,
+                                        const float* __restrict__ img_scale, float* __restrict__ out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= m) return;
+  const long long b = mb[t], i = mi[t], j = mj[t];
+  int lo = 0, hi = g;
+  while (lo < hi) {
+    const int mid = lo + (hi - lo) / 2;
+    const long long b2 = gb[mid], i2 = gi[mid];
+    const bool less = b2 != b ? b2 < b : (i2 != i ? i2 < i : gj[mid] < j);
+    if (less) lo = mid + 1;
+    else hi = mid;
+  }
+  float x = -50.f, y = -50.f;
+  if (lo < g && gb[lo] == b && gi[lo] == i && gj[lo] == j) {
+    x = fine_xy[2 * lo];
+    y = fine_xy[2 * lo + 1];
+  }
+  const long long jx = j % w_c, jy = j / w_c;
+  float ex, ey;
+  if (img_scale) {
+    // (x, y) scales = query_image_scale[b][[1, 0]]
+    const float sx = img_scale[2 * b + 1], sy = img_scale[2 * b];
+    const float qx = __fmul_rn((float)jx, __fmul_rn((float)coarse_res, sx));
+    const float qy = __fmul_rn((float)jy, __fmul_rn((float)coarse_res, sy));
+    ex = __fdiv_rn(__fsub_rn(x, qx), __fmul_rn((float)fine_res, sx));
+    ey = __fdiv_rn(__fsub_rn(y, qy), __fmul_rn((float)fine_res, sy));
+  } else {
+    // fine_supervision.py:18: without query_image_scale the coarse scale is the fine one
+    ex = __fmul_rn(__fsub_rn(x, (float)(jx * fine_res)), inv_fine);
+    ey = __fmul_rn(__fsub_rn(y, (float)(jy * fine_res)), inv_fine);
+  }
+  out[2 * t] = __fmul_rn(ex, inv_radius);
+  out[2 * t + 1] = __fmul_rn(ey, inv_radius);
 }
 
 }  // namespace
@@ -516,7 +694,7 @@ extern "C" int opp_coarse_focal_stats(const float* a, const float* b, const unsi
   OPP_REQUIRE(part_c && st_rows && st_cols, "opp_coarse_focal_stats: null output");
   const cudaStream_t st = (cudaStream_t)stream;
   const int blocks = opp_coarse_focal_blocks(rows);
-  OPP_CHECK_CUDA((launch_focal<kStats, true>(dim3(blocks, batches), st, a, b, nullptr, nullptr, nullptr, nullptr,
+  OPP_CHECK_CUDA((launch_focal<kStats, true, false>(dim3(blocks, batches), st, a, b, nullptr, nullptr, nullptr, nullptr,
                                              nullptr, nullptr, nullptr, 1, col_mask, rows, cols, scale,
                                              FocalCfg{0.f, 0.f}, nullptr, nullptr, st_rows, part_c, nullptr)));
   const long long n = (long long)batches * cols;
@@ -538,7 +716,7 @@ extern "C" int opp_coarse_focal_fwd(const float* a, const float* b, const float*
   const cudaStream_t st = (cudaStream_t)stream;
   const int blocks = opp_coarse_focal_blocks(rows);
   const FocalCfg f{alpha, gamma};
-  OPP_CHECK_CUDA((launch_focal<kFwd, true>(dim3(blocks, batches), st, a, b, reinterpret_cast<const float2*>(st_rows),
+  OPP_CHECK_CUDA((launch_focal<kFwd, true, false>(dim3(blocks, batches), st, a, b, reinterpret_cast<const float2*>(st_rows),
                                            reinterpret_cast<const float2*>(st_cols), nullptr, nullptr, nullptr,
                                            nullptr, gt, gt_bytes, col_mask, rows, cols, scale, f, part_loss,
                                            part_cnt, part_r, part_c, nullptr)));
@@ -564,11 +742,112 @@ extern "C" int opp_coarse_focal_bwd(const float* a, const float* b, const float*
   const FocalCfg f{alpha, gamma};
   const float2* sr = reinterpret_cast<const float2*>(st_rows);
   const float2* sc = reinterpret_cast<const float2*>(st_cols);
-  OPP_CHECK_CUDA((launch_focal<kBwd, true>(dim3(opp_coarse_focal_blocks(rows), batches), st, a, b, sr, sc, r, c,
+  OPP_CHECK_CUDA((launch_focal<kBwd, true, false>(dim3(opp_coarse_focal_blocks(rows), batches), st, a, b, sr, sc, r, c,
                                            wts, grad, gt, gt_bytes, col_mask, rows, cols, scale, f, nullptr, nullptr,
                                            nullptr, nullptr, da)));
-  OPP_CHECK_CUDA((launch_focal<kBwd, false>(dim3(opp_coarse_focal_blocks(cols), batches), st, b, a, sc, sr, c, r,
+  OPP_CHECK_CUDA((launch_focal<kBwd, false, false>(dim3(opp_coarse_focal_blocks(cols), batches), st, b, a, sc, sr, c, r,
                                             wts, grad, gt, gt_bytes, col_mask, cols, rows, scale, f, nullptr,
                                             nullptr, nullptr, nullptr, db)));
+  return OPP_OK;
+}
+
+#define OPP_GT_LIST(name)                                                                                   \
+  OPP_REQUIRE(g >= 0 && (g == 0 || (b_ids && i_ids && j_ids)), name ": bad list (g=%d)", g);                \
+  OPP_REQUIRE(batches > 0 && rows > 0 && cols > 0 && (long long)batches * rows < INT32_MAX &&               \
+                  (long long)batches * cols < INT32_MAX,                                                    \
+              name ": bad shape B=%d L=%d S=%d", batches, rows, cols)
+
+extern "C" int opp_gt_index(const long long* b_ids, const long long* i_ids, const long long* j_ids, int g,
+                            int batches, int rows, int cols, int* row_ptr, int* col_ptr, int* col_rows, int* fill,
+                            opp_stream_t stream) {
+  OPP_GT_LIST("opp_gt_index");
+  OPP_REQUIRE(row_ptr && col_ptr && fill && (g == 0 || col_rows), "opp_gt_index: null output");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const long long n_rows = (long long)batches * rows, n_cols = (long long)batches * cols;
+  gt_row_ptr_kernel<<<(unsigned)((n_rows + 256) / 256), 256, 0, st>>>(b_ids, i_ids, g, rows, n_rows, row_ptr);
+  OPP_CHECK_CUDA(cudaGetLastError());
+  OPP_CHECK_CUDA(cudaMemsetAsync(col_ptr, 0, (n_cols + 1) * sizeof(int), st));
+  if (g == 0) return OPP_OK;
+  OPP_CHECK_CUDA(cudaMemsetAsync(fill, 0, n_cols * sizeof(int), st));
+  const unsigned eb = (unsigned)((g + 255) / 256);
+  gt_col_count_kernel<<<eb, 256, 0, st>>>(b_ids, i_ids, j_ids, g, batches, rows, cols, col_ptr);
+  OPP_CHECK_CUDA(cudaGetLastError());
+  gt_scan_kernel<<<1, 1024, 0, st>>>(col_ptr, n_cols + 1);
+  OPP_CHECK_CUDA(cudaGetLastError());
+  gt_col_scatter_kernel<<<eb, 256, 0, st>>>(b_ids, i_ids, j_ids, g, batches, rows, cols, col_ptr, fill, col_rows);
+  OPP_CHECK_CUDA(cudaGetLastError());
+  gt_col_sort_kernel<<<(unsigned)((n_cols + 255) / 256), 256, 0, st>>>(col_ptr, n_cols, col_rows);
+  OPP_CHECK_CUDA(cudaGetLastError());
+  return OPP_OK;
+}
+
+extern "C" int opp_coarse_focal_fwd_sparse(const float* a, const float* b, const float* st_rows,
+                                           const float* st_cols, const int* row_ptr, const long long* j_ids,
+                                           const unsigned char* col_mask, int batches, int rows, int cols, int k,
+                                           float scale, float alpha, float gamma, float pos_w, float neg_w,
+                                           double* part_loss, long long* part_cnt, double* part_r, double* part_c,
+                                           float* loss, long long* counts, float* wts, double* r, double* c,
+                                           opp_stream_t stream) {
+  OPP_FOCAL_SHAPE("opp_coarse_focal_fwd_sparse");
+  OPP_REQUIRE(st_rows && st_cols && row_ptr, "opp_coarse_focal_fwd_sparse: null pointer");
+  OPP_REQUIRE(part_loss && part_cnt && part_r && part_c && loss && counts && wts && r && c,
+              "opp_coarse_focal_fwd_sparse: null output");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int blocks = opp_coarse_focal_blocks(rows);
+  const FocalCfg f{alpha, gamma};
+  OPP_CHECK_CUDA((launch_focal<kFwd, true, true>(dim3(blocks, batches), st, a, b,
+                                                 reinterpret_cast<const float2*>(st_rows),
+                                                 reinterpret_cast<const float2*>(st_cols), nullptr, nullptr, nullptr,
+                                                 nullptr, SparseGt{row_ptr, j_ids}, 0, col_mask, rows, cols, scale, f,
+                                                 part_loss, part_cnt, part_r, part_c, nullptr)));
+  coarse_focal_scalar_kernel<<<1, 256, 0, st>>>(part_loss, part_cnt, batches * blocks, pos_w, neg_w, loss, counts,
+                                               wts);
+  OPP_CHECK_CUDA(cudaGetLastError());
+  const long long n = (long long)batches * (rows + cols);
+  coarse_focal_rc_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+      reinterpret_cast<const double2*>(part_r), reinterpret_cast<const double2*>(part_c), wts, batches, rows, cols,
+      blocks, r, c);
+  OPP_CHECK_CUDA(cudaGetLastError());
+  return OPP_OK;
+}
+
+extern "C" int opp_coarse_focal_bwd_sparse(const float* a, const float* b, const float* st_rows,
+                                           const float* st_cols, const double* r, const double* c, const float* wts,
+                                           const float* grad, const int* row_ptr, const long long* j_ids,
+                                           const int* col_ptr, const int* col_rows, const unsigned char* col_mask,
+                                           int batches, int rows, int cols, int k, float scale, float alpha,
+                                           float gamma, float* da, float* db, opp_stream_t stream) {
+  OPP_FOCAL_SHAPE("opp_coarse_focal_bwd_sparse");
+  OPP_REQUIRE(st_rows && st_cols && row_ptr && col_ptr, "opp_coarse_focal_bwd_sparse: null pointer");
+  OPP_REQUIRE(r && c && wts && grad && da && db, "opp_coarse_focal_bwd_sparse: null pointer");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const FocalCfg f{alpha, gamma};
+  const float2* sr = reinterpret_cast<const float2*>(st_rows);
+  const float2* sc = reinterpret_cast<const float2*>(st_cols);
+  OPP_CHECK_CUDA((launch_focal<kBwd, true, true>(dim3(opp_coarse_focal_blocks(rows), batches), st, a, b, sr, sc, r, c,
+                                                 wts, grad, SparseGt{row_ptr, j_ids}, 0, col_mask, rows, cols, scale,
+                                                 f, nullptr, nullptr, nullptr, nullptr, da)));
+  OPP_CHECK_CUDA((launch_focal<kBwd, false, true>(dim3(opp_coarse_focal_blocks(cols), batches), st, b, a, sc, sr, c,
+                                                  r, wts, grad, SparseGt{col_ptr, col_rows}, 0, col_mask, cols, rows,
+                                                  scale, f, nullptr, nullptr, nullptr, nullptr, db)));
+  return OPP_OK;
+}
+
+extern "C" int opp_fine_supervision(const long long* b_ids, const long long* i_ids, const long long* j_ids,
+                                    const float* fine_xy, int g, int batches, int rows, int cols,
+                                    const long long* m_b, const long long* m_i, const long long* m_j, int m, int w_c,
+                                    int coarse_res, int fine_res, int radius, const float* img_scale, float* out,
+                                    opp_stream_t stream) {
+  OPP_GT_LIST("opp_fine_supervision");
+  OPP_REQUIRE(g == 0 || fine_xy, "opp_fine_supervision: null fine_xy");
+  OPP_REQUIRE(m >= 0 && (m == 0 || (m_b && m_i && m_j && out)), "opp_fine_supervision: bad matches (m=%d)", m);
+  OPP_REQUIRE(w_c > 0 && cols % w_c == 0 && coarse_res > 0 && fine_res > 0 && radius > 0,
+              "opp_fine_supervision: bad geometry w_c=%d S=%d resolution=(%d, %d) radius=%d", w_c, cols, coarse_res,
+              fine_res, radius);
+  if (m == 0) return OPP_OK;
+  fine_supervision_kernel<<<(unsigned)((m + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      b_ids, i_ids, j_ids, fine_xy, g, m_b, m_i, m_j, m, w_c, coarse_res, fine_res, 1.f / (float)fine_res,
+      1.f / (float)radius, img_scale, out);
+  OPP_CHECK_CUDA(cudaGetLastError());
   return OPP_OK;
 }

@@ -3,11 +3,13 @@ focal loss on the device when the model leaves a TrainConfHandle in ``data["conf
 (``conf_matrix_mode = "lazy"`` in train mode): forward and backward run on the opp_coarse_focal
 kernels and the [B, L, S] confidence matrix is never built.  With a tensor in
 ``data["conf_matrix"]`` the loss is the reference formula on that tensor.  The fine loss (M x 3) is
-PyTorch either way.
+PyTorch either way.  The ground truth is data["conf_matrix_gt"] or the list data["gt_sparse"]
+(train_gt.SparseGT), which the handle's kernels read without its dense form.
 """
 import torch
 import torch.nn as nn
 
+from .train_gt import SparseGT, gt_of
 from .train_path import TrainConfHandle
 
 try:
@@ -40,10 +42,43 @@ class _CoarseFocal(torch.autograd.Function):
         return da, db, None, None, None, None, None, None
 
 
+class _CoarseFocalSparse(torch.autograd.Function):
+    """_CoarseFocal with the ground truth as a SparseGT: its index is built once, here, and kept for
+    the backward."""
+
+    @staticmethod
+    def forward(ctx, feat3d, feat2d, handle, gt, alpha, gamma, pos_w, neg_w):
+        from . import ops
+        row_ptr, col_ptr, col_rows = ops.gt_index(gt.b_ids, gt.i_ids, gt.j_ids, gt.shape)
+        loss, counts, wts, r, c = ops.coarse_focal_fwd_sparse(handle.a32, handle.b32, handle.st_rows, handle.st_cols,
+                                                              row_ptr, gt.j_ids, handle.col_mask, handle.scale,
+                                                              alpha, gamma, pos_w, neg_w)
+        ctx.save_for_backward(r, c, wts, row_ptr, gt.j_ids, col_ptr, col_rows)
+        ctx.handle, ctx.focal = handle, (alpha, gamma)
+        ctx.mark_non_differentiable(counts)
+        return loss, counts
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_counts):
+        from . import ops
+        r, c, wts, row_ptr, j_ids, col_ptr, col_rows = ctx.saved_tensors
+        h = ctx.handle
+        grad = grad_loss.detach().float().contiguous()
+        da, db = ops.coarse_focal_bwd_sparse(h.a32, h.b32, h.st_rows, h.st_cols, r, c, wts, grad, row_ptr, j_ids,
+                                             col_ptr, col_rows, h.col_mask, h.scale, *ctx.focal)
+        return da, db, None, None, None, None, None, None
+
+
 def coarse_focal_loss(handle, conf_gt, alpha, gamma, pos_w, neg_w):
     """Focal loss of the dual-softmax confidence of `handle` against conf_gt (bool, uint8 or int16
-    [B, L, S] on the device), differentiable with respect to handle.feat3d / handle.feat2d.
+    [B, L, S] on the device, or a SparseGT on the device: every listed element is a positive, every
+    other one a negative), differentiable with respect to handle.feat3d / handle.feat2d.
     Returns (loss, counts): counts = int64 [2] (positives, negatives) on the device."""
+    if isinstance(conf_gt, SparseGT):
+        if tuple(conf_gt.shape) != tuple(handle.shape):
+            raise ValueError(f"gt_sparse has shape {tuple(conf_gt.shape)}, the confidence {tuple(handle.shape)}")
+        return _CoarseFocalSparse.apply(handle.feat3d, handle.feat2d, handle, conf_gt, float(alpha), float(gamma),
+                                        float(pos_w), float(neg_w))
     if conf_gt.dtype not in (torch.bool, torch.uint8, torch.int16):
         raise TypeError(f"conf_matrix_gt: expected bool, uint8 or int16, got {conf_gt.dtype}")
     if tuple(conf_gt.shape) != tuple(handle.shape):
@@ -65,7 +100,9 @@ class Loss(nn.Module):
 
     def compute_coarse_loss(self, conf, conf_gt, weight=None):
         """Focal loss over the positives (gt == 1) and negatives (gt == 0) of conf, each class
-        averaged; an empty class drops out with a warning.  conf: tensor or TrainConfHandle."""
+        averaged; an empty class drops out with a warning.  conf: tensor or TrainConfHandle; conf_gt:
+        tensor or SparseGT.  A tensor conf with a SparseGT is the formula below on the list's dense
+        form: correct, and as large as the dense ground truth while it runs."""
         if self.config["coarse_type"] != "focal":
             raise NotImplementedError
         alpha, gamma = self.config["focal_alpha"], self.config["focal_gamma"]
@@ -79,6 +116,8 @@ class Loss(nn.Module):
             elif nneg == 0:
                 logger.warning('len of loss neg is zero!')
             return loss
+        if isinstance(conf_gt, SparseGT):
+            conf_gt = conf_gt.to_dense()[0]
         c = torch.clamp(conf, 1e-6, 1 - 1e-6)
         pos, neg = conf_gt == 1, conf_gt == 0
         loss_pos = -alpha * torch.pow(1 - c[pos], gamma) * c[pos].log()
@@ -126,7 +165,8 @@ class Loss(nn.Module):
         scalars = {}
         if "mask0" in data and isinstance(data["conf_matrix"], TrainConfHandle):
             raise NotImplementedError("mask0 / mask1 loss weights are not built for the lazy confidence")
-        loss_c = self.compute_coarse_loss(data["conf_matrix"], data["conf_matrix_gt"],
+        gt = gt_of(data)
+        loss_c = self.compute_coarse_loss(data["conf_matrix"], gt if gt is not None else data["conf_matrix_gt"],
                                           weight=self.compute_c_weight(data))
         loss = loss_c * self.config["coarse_weight"]
         scalars["loss_c"] = loss_c.clone().detach().cpu()

@@ -315,6 +315,100 @@ def coarse_focal_bwd(a, b, st_rows, st_cols, r, c, wts, grad, gt, col_mask, scal
     return da, db
 
 
+def _chk_gt_list(b_ids, i_ids, j_ids):
+    for name, t in (("b_ids", b_ids), ("i_ids", i_ids), ("j_ids", j_ids)):
+        _chk(t, torch.int64, "gt_sparse." + name)
+    if not (b_ids.shape == i_ids.shape == j_ids.shape and b_ids.dim() == 1):
+        raise ValueError("gt_sparse: b_ids, i_ids and j_ids must be 1-d tensors of one length")
+    if b_ids.numel() >= 2 ** 31:
+        raise ValueError("gt_sparse: more than 2^31 - 1 correspondences")
+
+
+def gt_index(b_ids, i_ids, j_ids, shape):
+    """Row and column index of a ground-truth list sorted by (b, i, j): (row_ptr int32 [B*L+1],
+    col_ptr int32 [B*S+1], col_rows int32 [G] = the i of each column's entries, ascending)."""
+    _chk_gt_list(b_ids, i_ids, j_ids)
+    B, L, S = shape
+    G, dev, i32 = b_ids.numel(), b_ids.device, torch.int32
+    row_ptr = torch.empty(B * L + 1, dtype=i32, device=dev)
+    col_ptr = torch.empty(B * S + 1, dtype=i32, device=dev)
+    col_rows = torch.empty(G, dtype=i32, device=dev)
+    fill = torch.empty(B * S, dtype=i32, device=dev)
+    call("opp_gt_index", ptr(b_ids), ptr(i_ids), ptr(j_ids), G, B, L, S, ptr(row_ptr), ptr(col_ptr), ptr(col_rows),
+         ptr(fill), stream())
+    return row_ptr, col_ptr, col_rows
+
+
+def coarse_focal_fwd_sparse(a, b, st_rows, st_cols, row_ptr, j_ids, col_mask, scale, alpha, gamma, pos_w, neg_w):
+    """coarse_focal_fwd with the positives given as a list (row_ptr from gt_index, the list's j_ids):
+    the same outputs, bit for bit, as the dense call on the dense form of the list."""
+    _chk(a, torch.float32, "feat3d")
+    _chk(b, torch.float32, "feat2d")
+    _chk(col_mask, torch.uint8, "col_mask")
+    _chk(row_ptr, torch.int32, "row_ptr")
+    _chk(j_ids, torch.int64, "gt_sparse.j_ids")
+    B, L, K = a.shape
+    S = b.shape[1]
+    if row_ptr.numel() != B * L + 1:
+        raise ValueError(f"row_ptr has {row_ptr.numel()} entries, the features need {B * L + 1}")
+    nb = _lib.load().opp_coarse_focal_blocks(L)
+    dev, f32 = a.device, torch.float32
+    part_loss = torch.empty(B * nb, 2, dtype=torch.float64, device=dev)
+    part_cnt = torch.empty(B * nb, 2, dtype=torch.int64, device=dev)
+    part_r = torch.empty(B, L, 2, dtype=torch.float64, device=dev)
+    part_c = torch.empty(B, nb, S, 2, dtype=torch.float64, device=dev)
+    loss = torch.empty((), dtype=f32, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    wts = torch.empty(2, dtype=f32, device=dev)
+    r = torch.empty(B, L, dtype=torch.float64, device=dev)
+    c = torch.empty(B, S, dtype=torch.float64, device=dev)
+    call("opp_coarse_focal_fwd_sparse", ptr(a), ptr(b), ptr(st_rows), ptr(st_cols), ptr(row_ptr), ptr(j_ids),
+         ptr(col_mask), B, L, S, K, float(scale), float(alpha), float(gamma), float(pos_w), float(neg_w),
+         ptr(part_loss), ptr(part_cnt), ptr(part_r), ptr(part_c), ptr(loss), ptr(counts), ptr(wts), ptr(r), ptr(c),
+         stream())
+    return loss, counts, wts, r, c
+
+
+def coarse_focal_bwd_sparse(a, b, st_rows, st_cols, r, c, wts, grad, row_ptr, j_ids, col_ptr, col_rows, col_mask,
+                            scale, alpha, gamma):
+    """coarse_focal_bwd with the positives given as a list and its gt_index."""
+    _chk(a, torch.float32, "feat3d")
+    _chk(b, torch.float32, "feat2d")
+    _chk(grad, torch.float32, "grad")
+    _chk(col_mask, torch.uint8, "col_mask")
+    for name, t in (("row_ptr", row_ptr), ("col_ptr", col_ptr), ("col_rows", col_rows)):
+        _chk(t, torch.int32, name)
+    _chk(j_ids, torch.int64, "gt_sparse.j_ids")
+    B, L, K = a.shape
+    S = b.shape[1]
+    if row_ptr.numel() != B * L + 1 or col_ptr.numel() != B * S + 1:
+        raise ValueError("row_ptr / col_ptr do not belong to features of this shape")
+    da, db = torch.empty_like(a), torch.empty_like(b)
+    call("opp_coarse_focal_bwd_sparse", ptr(a), ptr(b), ptr(st_rows), ptr(st_cols), ptr(r), ptr(c), ptr(wts),
+         ptr(grad), ptr(row_ptr), ptr(j_ids), ptr(col_ptr), ptr(col_rows), ptr(col_mask), B, L, S, K, float(scale),
+         float(alpha), float(gamma), ptr(da), ptr(db), stream())
+    return da, db
+
+
+def fine_supervision(b_ids, i_ids, j_ids, fine_xy, shape, m_b, m_i, m_j, w_c, resolution, radius, img_scale):
+    """expec_f_gt fp32 [M, 2] of the matches (m_b, m_i, m_j) from a ground-truth list sorted by
+    (b, i, j) with fine locations fine_xy [G, 2]; img_scale fp32 [B, 2] (query_image_scale) or None."""
+    _chk_gt_list(b_ids, i_ids, j_ids)
+    _chk(fine_xy, torch.float32, "gt_sparse.fine_xy")
+    for name, t in (("b_ids", m_b), ("i_ids", m_i), ("j_ids", m_j)):
+        _chk(t, torch.int64, name)
+    _chk(img_scale, torch.float32, "query_image_scale")
+    B, L, S = shape
+    if img_scale is not None and tuple(img_scale.shape) != (B, 2):
+        raise ValueError(f"query_image_scale has shape {tuple(img_scale.shape)}, expected {(B, 2)}")
+    M = m_b.numel()
+    out = torch.empty(M, 2, dtype=torch.float32, device=m_b.device)
+    call("opp_fine_supervision", ptr(b_ids), ptr(i_ids), ptr(j_ids), ptr(fine_xy), b_ids.numel(), B, L, S,
+         ptr(m_b), ptr(m_i), ptr(m_j), M, int(w_c), int(resolution[0]), int(resolution[1]), int(radius),
+         ptr(img_scale), ptr(out), stream())
+    return out
+
+
 def fine_gather(fine, desc3d, b_ids, i_ids, j_ids, x32, x16, m, hf, wf, wc, stride, n, split,
                 bank_shared=False, count=None, windows=False, bank_of_batch=None):
     """windows: `fine` is the compact [m, 5, 8, planes*128] window tensor of conv_win.

@@ -14,12 +14,15 @@ This is the slow path by construction (SURVEY §8 f4 "keep the PyTorch path for 
 the coarse supervision: with ``model.conf_matrix_mode == "lazy"`` on CUDA tensors the L x S
 confidence matrix is not built — the statistics and the match selection run on the inference
 kernels and ``data["conf_matrix"]`` is a TrainConfHandle that ``losses.Loss`` differentiates with
-the opp_coarse_focal kernels (DESIGN §7 f4).
+the opp_coarse_focal kernels (DESIGN §7 f4).  The ground truth the padding draws from is
+data["conf_matrix_gt"] or, in its place, the correspondence list data["gt_sparse"] (train_gt.py).
 
 Every function cites the reference lines it follows.
 """
 import torch
 import torch.nn.functional as F
+
+from . import train_gt
 
 
 def _block(blk, x):
@@ -140,7 +143,15 @@ def _pad_matches(cm, b_ids, i_ids, j_ids, mconf, shape, data, training):
             pred_idx = torch.arange(n_pred, device=dev)
         else:
             pred_idx = torch.randint(n_pred, (n_max - pad_min,), device=dev)
-        sb, si, sj = torch.where(data["conf_matrix_gt"])
+        gt = train_gt.gt_of(data)
+        if gt is not None:      # the list is in the order of torch.where: the same draws pick the same paddings
+            if tuple(gt.shape) != (B, L, S):
+                raise ValueError(f"gt_sparse has shape {tuple(gt.shape)}, the confidence {(B, L, S)}")
+            if gt.device != dev:
+                raise ValueError(f"gt_sparse is on {gt.device}, the matches on {dev}")
+            sb, si, sj = gt.b_ids, gt.i_ids, gt.j_ids
+        else:
+            sb, si, sj = torch.where(data["conf_matrix_gt"])
         assert len(sb) != 0
         pad_idx = torch.randint(len(sb), (max(n_max - n_pred, pad_min),), device=dev)
         zeros = torch.zeros(len(sb), device=dev)   # confidence of the gt paddings is 0
