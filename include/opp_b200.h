@@ -541,6 +541,62 @@ int opp_fine_supervision(const long long* b_ids, const long long* i_ids, const l
                          const long long* m_i, const long long* m_j, int m, int w_c, int coarse_res, int fine_res,
                          int radius, const float* img_scale, float* out, opp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training, fine level (opp_train_fine.cu): window gather, the two fine LoFTR layers and the
+ * heatmap expectation, forward and backward, fp32.  Match m owns the 26 token rows m*26 + t
+ * (t = ky*5 + kx the window, 25 the 3D token).  No floating-point atomics: every result is
+ * bit-reproducible.
+ * ---------------------------------------------------------------------------------------- */
+
+/* Row groups (partials) of opp_fine_train_wgrad / _ln_bwd for `rows` rows. */
+int opp_fine_train_groups(int rows);
+
+/* x[m*26 + t][0..127] (row stride ldx): the 5 x 5 window of F.unfold(feat, 5, padding 2, stride)
+ * around cell j_ids[m] (cells (j / wc, j % wc)), zeros outside the map, then desc3d[b][:, i].
+ * feat fp32 [B][128][hf][wf], desc3d fp32 [B][128][n3d]. */
+int opp_fine_train_gather(const float* feat, const float* desc3d, const long long* b_ids, const long long* i_ids,
+                          const long long* j_ids, int m, int hf, int wf, int hc, int wc, int n3d, int stride,
+                          float* x, int ldx, opp_stream_t stream);
+
+/* d feat [B][128][hf][wf] (overwritten) from the window rows' gradient dx, one thread per element:
+ * the cells whose window covers it in raster order, each cell's matches in the order of
+ * col_rows[col_ptr[b*hc*wc + j] ..) (opp_gt_index's column view of the matches). */
+int opp_fine_train_gather_bwd(const float* dx, int ldx, const int* col_ptr, const int* col_rows, int batches,
+                              int hf, int wf, int hc, int wc, int stride, float* dfeat, opp_stream_t stream);
+
+/* c[r][0..n) = epi(a[r][0..k) . B): B(k, n) = w[n][k] when trans_w, else w[k][n].  epi 0 store,
+ * 1 ReLU (trans_w), 2 zero where aux <= 0, 3 add aux and aux2 (either may be NULL); 2 and 3 need
+ * !trans_w.  n % 64 == 0, k % 16 == 0, 16-byte aligned rows. */
+int opp_fine_train_linear(const float* a, int lda, const float* w, int trans_w, int rows, int n, int k, float* c,
+                          int ldc, int epi, const float* aux, int ldaux, const float* aux2, int ldaux2,
+                          opp_stream_t stream);
+
+/* dw[n][k] (+)= sum_r g[r][n] a[r][k]: part fp32 [groups][n][k] per group of rows, then summed in
+ * group order.  n, k multiples of 64. */
+int opp_fine_train_wgrad(const float* g, int ldg, const float* a, int lda, int rows, int n, int k, float* part,
+                         float* dw, int accumulate, opp_stream_t stream);
+
+/* LayerNorm over 128 channels (eps 1e-5): y = LN(x) * gamma + beta (+ resid); stats [rows][2] =
+ * (mean, rstd). */
+int opp_fine_train_ln(const float* x, int ldx, const float* gamma, const float* beta, const float* resid, int ldr,
+                      float* y, int ldy, float* stats, int rows, opp_stream_t stream);
+
+/* Its backward: dx (overwritten) and dgb [2][128] (+)= (dgamma, dbeta); part [groups][2][128]. */
+int opp_fine_train_ln_bwd(const float* x, int ldx, const float* gamma, const float* stats, const float* dy, int lddy,
+                          float* dx, int lddx, int rows, float* part, float* dgb, int accumulate,
+                          opp_stream_t stream);
+
+/* Linear attention of one fine layer: qkv [m*26][384] = (q | k | v), out [m*26][128].  cross 0:
+ * the window attends to the window and the 3D token to itself; cross 1: each to the other. */
+int opp_fine_train_attention(const float* qkv, float* out, int m, int cross, float eps, opp_stream_t stream);
+int opp_fine_train_attention_bwd(const float* qkv, const float* dout, float* dqkv, int m, int cross, float eps,
+                                 opp_stream_t stream);
+
+/* Heatmap expectation of x [m*26][128] (the last layer's output): expec_f [m][3] = (x, y, std), and
+ * its backward to dx [m*26][128] (overwritten). */
+int opp_fine_train_match(const float* x, int m, float* expec_f, opp_stream_t stream);
+int opp_fine_train_match_bwd(const float* x, const float* dexpec, int m, float* dx, opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -70,12 +70,23 @@ SIGNATURES = {
     "opp_coarse_focal_fwd_sparse": [P] * 7 + [I, I, I, I, F, F, F, F, F] + [P] * 10,
     "opp_coarse_focal_bwd_sparse": [P] * 13 + [I, I, I, I, F, F, F, P, P, P],
     "opp_fine_supervision": [P, P, P, P, I, I, I, I, P, P, P, I, I, I, I, I, P, P, P],
+    "opp_fine_train_gather": [P] * 5 + [I] * 7 + [P, I, P],
+    "opp_fine_train_gather_bwd": [P, I, P, P] + [I] * 6 + [P, P],
+    "opp_fine_train_linear": [P, I, P, I, I, I, I, P, I, I, P, I, P, I, P],
+    "opp_fine_train_wgrad": [P, I, P, I, I, I, I, P, P, I, P],
+    "opp_fine_train_ln": [P, I, P, P, P, I, P, I, P, I, P],
+    "opp_fine_train_ln_bwd": [P, I, P, P, P, I, P, I, I, P, P, I, P],
+    "opp_fine_train_attention": [P, P, I, I, F, P],
+    "opp_fine_train_attention_bwd": [P, P, P, I, I, F, P],
+    "opp_fine_train_match": [P, I, P, P],
+    "opp_fine_train_match_bwd": [P, P, I, P, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),
          "opp_kv_chunks_b": ([I, I], c_int),
          "opp_conv_win_pitch": ([I], c_int),
          "opp_coarse_focal_blocks": ([I], c_int),
+         "opp_fine_train_groups": ([I], c_int),
          "opp_pose_metrics_scratch_bytes": ([I, I], c_longlong),
          "opp_last_error": ([], ctypes.c_char_p)}
 
@@ -115,7 +126,8 @@ def stream():
 KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_match_select_colmax_set": 3,
                     "opp_pose_metrics": 3,
                     "opp_coarse_focal_stats": 2, "opp_coarse_focal_fwd": 3, "opp_coarse_focal_bwd": 2,
-                    "opp_gt_index": 5, "opp_coarse_focal_fwd_sparse": 3, "opp_coarse_focal_bwd_sparse": 2}
+                    "opp_gt_index": 5, "opp_coarse_focal_fwd_sparse": 3, "opp_coarse_focal_bwd_sparse": 2,
+                    "opp_fine_train_wgrad": 2, "opp_fine_train_ln_bwd": 2}
 LAUNCHES = 0
 _PROFILE = None
 

@@ -651,6 +651,9 @@ class OnePosePlus_model(_Engine):
         # that materialises on demand (no inference consumer reads the matrix:
         # inference_OnePosePlus_worker.py:20-31); "skip" = key not written.
         self.conf_matrix_mode = os.environ.get("OPP_B200_CONF", "eager")
+        # fine level of .train() on CUDA: "autograd" = train_path's PyTorch functions, "kernels" = the
+        # opp_fine_train_* kernels forward and backward (train_fine.py; no unfold tensor)
+        self.fine_train_mode = os.environ.get("OPP_B200_FINE_TRAIN", "autograd")
         # one-pass dual softmax: column statistics of sim / conf from the row passes (warp
         # butterflies in the epilogue) instead of two more sim GEMM passes
         self.coarse_colmax = os.environ.get("OPP_B200_COLMAX", "1") == "1"

@@ -482,3 +482,77 @@ def seq_attention(q, kv, out, groups, l, s, split, eps=1e-6):
 def fine_match_2d(x32, mkpts1_c, b_ids, scale1, expec_f, mkpts1_f, m, window, fine_scale):
     call("opp_fine_match_2d", ptr(x32), ptr(mkpts1_c), ptr(b_ids), ptr(scale1), ptr(expec_f), ptr(mkpts1_f), m,
          window, float(fine_scale), stream())
+
+
+# ---- training, fine level (opp_train_fine.cu; used by train_fine.py) ------------------------------
+# Row operands are fp32 CUDA tensors addressed by (tensor, row stride); a column slice of a wider
+# buffer (x[:, 128:]) passes its own data pointer with the buffer's stride.
+
+def _ld(t):
+    if t is None:
+        return 0
+    if t.dtype != torch.float32 or not t.is_cuda or t.stride(-1) != 1:
+        raise ValueError("fine training operands are fp32 CUDA rows with unit column stride")
+    return t.stride(0)
+
+
+def fine_train_gather(feat, desc3d, b_ids, i_ids, j_ids, hc, wc, stride, x):
+    _chk(feat, torch.float32, "feat_f")
+    _chk(desc3d, torch.float32, "descriptors3d_db")
+    _, _, hf, wf = feat.shape
+    call("opp_fine_train_gather", ptr(feat), ptr(desc3d), ptr(b_ids), ptr(i_ids), ptr(j_ids), b_ids.numel(), hf, wf,
+         hc, wc, desc3d.shape[2], stride, ptr(x), _ld(x), stream())
+
+
+def fine_train_gather_bwd(dx, col_ptr, col_rows, hc, wc, stride, dfeat):
+    B, _, hf, wf = dfeat.shape
+    call("opp_fine_train_gather_bwd", ptr(dx), _ld(dx), ptr(col_ptr), ptr(col_rows), B, hf, wf, hc, wc, stride,
+         ptr(dfeat), stream())
+
+
+EPI_STORE, EPI_RELU, EPI_MASK, EPI_ADD = 0, 1, 2, 3
+
+
+def fine_train_linear(a, w, trans_w, out, epi=EPI_STORE, aux=None, aux2=None):
+    """out = epi(a @ w.T) (trans_w) or epi(a @ w); w contiguous fp32."""
+    _chk(w, torch.float32, "weight")
+    n, k = (w.shape[0], w.shape[1]) if trans_w else (w.shape[1], w.shape[0])
+    call("opp_fine_train_linear", ptr(a), _ld(a), ptr(w), int(trans_w), a.shape[0], n, k, ptr(out), _ld(out), epi,
+         ptr(aux), _ld(aux), ptr(aux2), _ld(aux2), stream())
+
+
+def fine_train_wgrad(g, a, part, dw, accumulate):
+    """dw (+)= g.T @ a, summed over row groups in a fixed order."""
+    call("opp_fine_train_wgrad", ptr(g), _ld(g), ptr(a), _ld(a), g.shape[0], dw.shape[0], dw.shape[1], ptr(part),
+         ptr(dw), int(accumulate), stream())
+
+
+def fine_train_ln(x, gamma, beta, resid, y, stats):
+    call("opp_fine_train_ln", ptr(x), _ld(x), ptr(gamma), ptr(beta), ptr(resid), _ld(resid), ptr(y), _ld(y),
+         ptr(stats), x.shape[0], stream())
+
+
+def fine_train_ln_bwd(x, gamma, stats, dy, dx, part, dgb, accumulate):
+    call("opp_fine_train_ln_bwd", ptr(x), _ld(x), ptr(gamma), ptr(stats), ptr(dy), _ld(dy), ptr(dx), _ld(dx),
+         x.shape[0], ptr(part), ptr(dgb), int(accumulate), stream())
+
+
+def fine_train_attention(qkv, out, m, cross, eps=1e-6):
+    call("opp_fine_train_attention", ptr(qkv), ptr(out), m, int(cross), eps, stream())
+
+
+def fine_train_attention_bwd(qkv, dout, dqkv, m, cross, eps=1e-6):
+    call("opp_fine_train_attention_bwd", ptr(qkv), ptr(dout), ptr(dqkv), m, int(cross), eps, stream())
+
+
+def fine_train_match(x, m, expec_f):
+    call("opp_fine_train_match", ptr(x), m, ptr(expec_f), stream())
+
+
+def fine_train_match_bwd(x, dexpec, m, dx):
+    _chk(dexpec, torch.float32, "grad of expec_f")
+    call("opp_fine_train_match_bwd", ptr(x), ptr(dexpec), m, ptr(dx), stream())
+
+
+def fine_train_groups(rows):
+    return _lib.load().opp_fine_train_groups(rows)

@@ -14,7 +14,9 @@ This is the slow path by construction (SURVEY §8 f4 "keep the PyTorch path for 
 the coarse supervision: with ``model.conf_matrix_mode == "lazy"`` on CUDA tensors the L x S
 confidence matrix is not built — the statistics and the match selection run on the inference
 kernels and ``data["conf_matrix"]`` is a TrainConfHandle that ``losses.Loss`` differentiates with
-the opp_coarse_focal kernels (DESIGN §7 f4).  The ground truth the padding draws from is
+the opp_coarse_focal kernels (DESIGN §7 f4).  With ``model.fine_train_mode == "kernels"`` on CUDA
+tensors the fine level (fine_preprocess -> loftr_fine -> fine_matching) runs on the
+opp_fine_train_* kernels instead (train_fine.py).  The ground truth the padding draws from is
 data["conf_matrix_gt"] or, in its place, the correspondence list data["gt_sparse"] (train_gt.py).
 
 Every function cites the reference lines it follows.
@@ -22,7 +24,7 @@ Every function cites the reference lines it follows.
 import torch
 import torch.nn.functional as F
 
-from . import train_gt
+from . import train_fine, train_gt
 
 
 def _block(blk, x):
@@ -316,6 +318,7 @@ def forward_train(model, data):
         # single fp16 operands would select matches from a sim that differs from the eager fp32 one
         raise ValueError('conf_matrix_mode "lazy" in train mode needs precision "fp16x3" (the match '
                          'selection runs on the fp32-grade split operands)')
+    fine_kernels = train_fine.use_kernels(model, data)
     data.update({"bs": img.size(0), "q_hw_i": img.shape[2:]})
     feat_c, feat_f = backbone(model.backbone, img)
     data.update({"q_hw_c": feat_c.shape[2:], "q_hw_f": feat_f.shape[2:]})
@@ -329,6 +332,9 @@ def forward_train(model, data):
     coarse_matching(model.coarse_matching, d3, q_c, data, qmask, model.training, lazy_split)
     if not cfg["fine_matching"]["enable"]:
         data.update({"mkpts_query_f": data["mkpts_query_c"]})
+        return
+    if fine_kernels:
+        train_fine.fine_stage(model, data, feat_f)
         return
     f3d, f2d = fine_preprocess(model.fine_preprocess.W, cfg["loftr_fine"]["d_model"], data,
                                data["descriptors3d_db"], feat_f)
