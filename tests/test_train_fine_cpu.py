@@ -100,6 +100,49 @@ def test_gather_backward_index_against_fold(stride):
     assert worst == (4 if stride == 4 else 9)                       # 2 x 2 cells at the training stride
 
 
+@pytest.mark.parametrize("stride", [2, 4, 8])
+def test_fold_reference_against_fine_preprocess_autograd(stride):
+    """The gather-backward reference of test_train_fine_kernels_gpu (index_put_ + F.fold) is the
+    fp64 autograd backward of train_path.fine_preprocess's window rows."""
+    from tests.test_train_fine_kernels_gpu import fold_reference
+    from onepose_plus_plus_b200 import train_path
+    case = mtf.make_case(seed=7, B=3, hc=5, wc=7, stride=stride, n3d=4, M=60)
+    B, _, hf, wf = case["feat_f"].shape
+    feat = case["feat_f"].clone().requires_grad_(True)
+    _, f2d = train_path.fine_preprocess(5, 128, mtf.fine_data(case), case["desc3d"], feat)
+    dx = torch.randn(f2d.shape, generator=torch.Generator().manual_seed(stride), dtype=torch.float64)
+    (ref,) = torch.autograd.grad(f2d, feat, dx)
+    got = fold_reference(dx, case["b_ids"], case["j_ids"], B, 5, 7, stride, hf, wf)
+    assert torch.allclose(got, ref, rtol=0, atol=1e-12)
+
+
+def test_attention_reference_against_train_path_transformer(monkeypatch):
+    """The attention reference of test_train_fine_kernels_gpu (train_path._linear_attention on the
+    26-row [q | k | v] layout, self and cross) gives the messages train_path.transformer computes
+    in the two fine layers, from the q, k, v those calls receive."""
+    from tests.test_train_fine_kernels_gpu import attention_reference
+    from onepose_plus_plus_b200 import train_path
+    calls = []
+    orig = train_path._linear_attention
+
+    def record(q, k, v, q_mask=None, kv_mask=None, eps=1e-6):
+        out = orig(q, k, v, q_mask, kv_mask, eps)
+        calls.append([t.reshape(t.shape[0], t.shape[1], 128) for t in (q, k, v, out)])
+        return out
+
+    monkeypatch.setattr(train_path, "_linear_attention", record)
+    g = torch.Generator().manual_seed(6)
+    f3d = torch.randn(7, 128, 1, generator=g, dtype=torch.float64)
+    f2d = torch.randn(7, 25, 128, generator=g, dtype=torch.float64)
+    with torch.no_grad():
+        train_path.transformer(mtf.fine_module(workload.synthetic_state_dict(0)), f3d, f2d)
+    (qa, ka, va, oa), (qb, kb, vb, ob), (qc, kc, vc, oc), (qd, kd, vd, od) = calls   # self 2D, 3D; cross 2D, 3D
+    self_qkv = torch.cat([torch.cat([qa, ka, va], 2), torch.cat([qb, kb, vb], 2)], 1)
+    cross_qkv = torch.cat([torch.cat([qc, kd, vd], 2), torch.cat([qd, kc, vc], 2)], 1)
+    for qkv, cross, outs in ((self_qkv, 0, (oa, ob)), (cross_qkv, 1, (oc, od))):
+        assert torch.allclose(attention_reference(qkv, cross), torch.cat(outs, 1), rtol=1e-12, atol=1e-14)
+
+
 def test_fixture_against_train_path_fp64():
     z = np.load(GOLDEN)
     case = mtf.make_case()
