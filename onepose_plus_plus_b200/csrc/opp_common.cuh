@@ -297,6 +297,16 @@ __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
   d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
+// The same with 64-byte swizzle (TMA SWIZZLE_64B, inner box extent 32 fp16): rows of 64 B, 8-row
+// groups 512 B apart, layout type 2.  A K step of 16 fp16 is still +32 B inside the row.
+__device__ __forceinline__ uint64_t make_kmajor_sw64_desc(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>(512 >> 4) << 32;
+  d |= static_cast<uint64_t>(2) << 62;
+  return d;
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>

@@ -54,8 +54,8 @@ int num_sms() {
   return n;
 }
 
-// fp16 tensor map, 128B swizzle, zero OOB fill. dims/strides fastest-first; strides in elements
-// for dims 1..rank-1.
+// fp16 tensor map, zero OOB fill, swizzled by the inner box row: 64 fp16 (a K chunk of 64) = 128B
+// swizzle, 32 fp16 = 64B swizzle. dims/strides fastest-first; strides in elements for dims 1..rank-1.
 static int make_map(CUtensorMap* map, const void* ptr, int rank, const uint64_t* dims,
                     const uint64_t* strides_elems, const uint32_t* box) {
   EncodeTiledFn fn = get_encode_fn();
@@ -64,6 +64,7 @@ static int make_map(CUtensorMap* map, const void* ptr, int rank, const uint64_t*
     return OPP_ERR_CUDA;
   }
   OPP_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "TMA base pointer not 16B aligned");
+  OPP_REQUIRE(box[0] == 64 || box[0] == 32, "TMA inner box %u is not one swizzle row", box[0]);
   cuuint64_t gdim[5], gstr[4];
   cuuint32_t bdim[5], estr[5];
   for (int i = 0; i < rank; ++i) {
@@ -78,7 +79,8 @@ static int make_map(CUtensorMap* map, const void* ptr, int rank, const uint64_t*
                 (unsigned long long)gstr[i]);
   }
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(ptr), gdim, gstr,
-                  bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  box[0] == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled failed with CUresult %d (rank %d dims %llu %llu %llu)",
@@ -89,12 +91,12 @@ static int make_map(CUtensorMap* map, const void* ptr, int rank, const uint64_t*
   return OPP_OK;
 }
 
-// A / W operand as [batch][rows][K] with row stride ld (elements)
+// A / W operand as [batch][rows][K] with row stride ld (elements), boxes of bk K columns
 static int map_rows(CUtensorMap* map, const void* ptr, long long k, long long rows,
-                    long long batches, long long ld, long long batch_stride, int box_rows) {
+                    long long batches, long long ld, long long batch_stride, int box_rows, int bk = kBlockK) {
   uint64_t dims[3] = {(uint64_t)k, (uint64_t)rows, (uint64_t)batches};
   uint64_t str[2] = {(uint64_t)ld, (uint64_t)batch_stride};
-  uint32_t box[3] = {(uint32_t)kBlockK, (uint32_t)box_rows, 1};
+  uint32_t box[3] = {(uint32_t)bk, (uint32_t)box_rows, 1};
   return make_map(map, ptr, 3, dims, str, box);
 }
 
@@ -114,9 +116,9 @@ static void log_tile_once(int a_mode, const GemmShape& s, const char* epi) {
   static char seen[256][128];
   static int n_seen = 0;
   char key[128];
-  snprintf(key, sizeof(key), "mode %d n %d block_n %d mma_n %d k %d conv_c %d stages %d alias %d cluster %d pair %d",
+  snprintf(key, sizeof(key), "mode %d n %d block_n %d mma_n %d k %d conv_c %d stages %d alias %d cluster %d pair %d bk %d",
            a_mode, s.n_total, s.block_n, s.mma_n, s.k_chunks * kBlockK, s.conv_c, s.stages, s.acc_alias,
-           s.cluster, s.pair);
+           s.cluster, s.pair, s.bk);
   std::lock_guard<std::mutex> lock(mu);
   if (on == 2) {
     fprintf(stderr, "opp gemm tile: %s epi %s\n", key, epi);
@@ -151,17 +153,27 @@ static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Param
   }
   const int smem = gemm_smem_bytes<Epi>(s);
   log_tile_once(A_MODE, s, Epi::kName);
+  // 32-wide ring slots are compiled for the conv modes only
+  OPP_REQUIRE(s.bk == kBlockK || (s.bk == 32 && A_MODE != A_ROWS), "ring slot width %d not compiled for mode %d",
+              s.bk, A_MODE);
   const void* kern;
   if constexpr (DYN) kern = (const void*)gemm_kernel_dyn<A_MODE, Epi>;
   else kern = (const void*)gemm_kernel<A_MODE, Epi>;
-  // function attributes are per device: set once per (template instantiation, device)
-  static unsigned long long attr_done = 0;
+  if constexpr (A_MODE != A_ROWS) {
+    if (s.bk == 32) {
+      if constexpr (DYN) kern = (const void*)gemm_kernel_dyn<A_MODE, Epi, 32>;
+      else kern = (const void*)gemm_kernel<A_MODE, Epi, 32>;
+    }
+  }
+  // function attributes are per device: set once per (kernel, device)
+  static unsigned long long attr_done[2] = {0, 0};
+  unsigned long long& done = attr_done[s.bk == 32];
   int dev = 0;
   OPP_CHECK_CUDA(cudaGetDevice(&dev));
-  if (dev < 64 && !((attr_done >> dev) & 1ull)) {
+  if (dev < 64 && !((done >> dev) & 1ull)) {
     OPP_CHECK_CUDA(
         cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_done |= 1ull << dev;
+    done |= 1ull << dev;
   }
   const long long total = (long long)s.batches * s.msup * s.n_tiles;   // super tiles
   if (total == 0) return OPP_OK;
@@ -213,6 +225,27 @@ static int pick_cluster(int block_n, int m_tiles) {
   int c = forced > 1 ? forced : 2;
   while (c > 1 && (mma_width_for(block_n) % (8 * c) != 0 || m_tiles < c)) c >>= 1;
   return c;
+}
+
+// Ring slot width of a convolution layer (A_CONV, A_WIN): 32 channels for the 3x3 layers whose
+// padded output width is above 128, else 64.  At N = 208 / 256 a 64-wide stage is 84 / 96 KB and
+// only two fit, and the MMA warpgroups keep the previous slot until the next slot's MMAs are issued:
+// with one slot per stage they hold both stages and no load is in flight.  Two 32-wide slots per
+// stage (the same shared memory) leave a stage's first half free to load while its second half and
+// the other stage are read (3x3 layers at batch 64: 15-39 % less time).  The 1x1 layers (2-4 chunks
+// per tile) and the N <= 128 layers (three stages) measured 1-15 % slower with 32-wide slots, all but
+// one 1x1 lateral (7 % faster).  The slot width sets the order of the fp32 accumulation (the three
+// split products per slot), so it depends on the layer only - never on the batch, tile, ring, cluster
+// or N split - and the dense and window forms of a layer, and its launches at every batch, give the
+// same bits.  $OPP_CONV_BK=32|64 forces one width for every conv layer.
+static int conv_chunk_k(int ksize, int c_out_pad) {
+  static int forced = -1;
+  if (forced < 0) {
+    const char* e = getenv("OPP_CONV_BK");
+    forced = e ? atoi(e) : 0;
+  }
+  if (forced == 32 || forced == 64) return forced;
+  return ksize == 3 && c_out_pad > 128 ? 32 : 64;
 }
 
 static int pick_block_n(int n) {
@@ -297,6 +330,7 @@ static int setup_rows(TensorMaps& maps, GemmShape& s, const void* a0, int k0, co
   OPP_REQUIRE(s.block_n % 16 == 0 && s.block_n <= 256, "bad block_n %d", s.block_n);
   s.n_tiles = (n + s.block_n - 1) / s.block_n;
   s.n_total = n;
+  s.bk = kBlockK;
   s.k_chunks_a0 = k0 / 64;
   s.k_chunks = (k0 + k1) / 64;
   s.b_batched = w_batched;
@@ -469,6 +503,7 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   s.n_tiles = 1;
   s.n_total = c_out_pad;
   s.conv_c = c_in_pad;
+  s.bk = conv_chunk_k(ksize, c_out_pad);
   s.conv_cchunks = (c_in_pad + 63) / 64;
   s.k_chunks = ksize * ksize * s.conv_cchunks;
   s.conv_kw = ksize;
@@ -477,7 +512,7 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   s.out_w = out_w;
   s.out_h = out_h;
   s.split = split ? 1 : 0;
-  // A maps are 5-D (channel, plane, x, y, image) with channel extent c_in_pad: the last 64-channel
+  // A maps are 5-D (channel, plane, x, y, image) with channel extent c_in_pad: the last bk-channel
   // box of a row reads zeros past c_in_pad (the mainloop skips the MMA steps of a 16-channel tail)
   const long long C = (long long)planes * c_in_pad;  // pixel stride in elements
   const __half* base = (const __half*)in;
@@ -485,7 +520,7 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   if (stride == 1) {
     uint64_t dims[5] = {(uint64_t)c_in_pad, (uint64_t)planes, (uint64_t)in_w, (uint64_t)in_h, (uint64_t)batch};
     uint64_t str[4] = {(uint64_t)c_in_pad, (uint64_t)C, (uint64_t)(in_w * C), (uint64_t)((long long)in_h * in_w * C)};
-    uint32_t box[5] = {64, 1, (uint32_t)s.tile_w, (uint32_t)s.tile_h, 1};
+    uint32_t box[5] = {(uint32_t)s.bk, 1, (uint32_t)s.tile_w, (uint32_t)s.tile_h, 1};
     rc = make_map(&maps.a[0], base, 5, dims, str, box);
     if (rc) return rc;
     maps.a[1] = maps.a[2] = maps.a[3] = maps.a[0];
@@ -496,7 +531,7 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
                             (uint64_t)(in_h / 2), (uint64_t)batch};
         uint64_t str[4] = {(uint64_t)c_in_pad, (uint64_t)(2 * C), (uint64_t)(2LL * in_w * C),
                            (uint64_t)((long long)in_h * in_w * C)};
-        uint32_t box[5] = {64, 1, (uint32_t)s.tile_w, (uint32_t)s.tile_h, 1};
+        uint32_t box[5] = {(uint32_t)s.bk, 1, (uint32_t)s.tile_w, (uint32_t)s.tile_h, 1};
         rc = make_map(&maps.a[py * 2 + px], base + ((long long)py * in_w + px) * C, 5, dims, str,
                       box);
         if (rc) return rc;
@@ -509,7 +544,7 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   split_n_for_latency(s);   // the 1/8-resolution layers at batch 1: 16 clusters -> 64
   rc = up ? fit_tile<EpiConvUp>(s) : fit_tile<EpiConv>(s);
   if (rc) return rc;
-  rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.mma_n / s.cluster);
+  rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.mma_n / s.cluster, s.bk);
   if (rc) return rc;
   OPP_REQUIRE(!up || (out_h % 2 == 0 && out_w % 2 == 0 && out_h >= 4 && out_w >= 4),
               "fused upsample-add needs even output dims >= 4 (got %d x %d)", out_h, out_w);
@@ -563,6 +598,10 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
   s.n_tiles = 1;
   s.n_total = c_out_pad;
   s.conv_c = c_in_pad;
+  s.bk = conv_chunk_k(3, c_out_pad);
+  // a window's box lands at a multiple of its size in the A stage: a whole number of swizzle atoms
+  // (8 rows of 2 bk bytes) for pitch 8, not for the five-5x5-boxes packing at bk = 32
+  OPP_REQUIRE(pitch == 8 || s.bk == 64, "OPP_WIN5_PACK needs 64-wide ring slots (layer has %d)", s.bk);
   s.conv_cchunks = (c_in_pad + 63) / 64;
   s.k_chunks = 9 * s.conv_cchunks;
   s.conv_kw = 3;
@@ -577,7 +616,7 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
     const uint64_t iw = j_ids ? in_w : 8, ih = j_ids ? in_h : win + 2, ib = j_ids ? batch : matches;
     uint64_t dims[5] = {(uint64_t)c_in_pad, (uint64_t)planes, iw, ih, ib};   // 5-D: see opp_conv2d_nhwc
     uint64_t str[4] = {(uint64_t)c_in_pad, (uint64_t)C, (uint64_t)(iw * C), (uint64_t)(ih * iw * C)};
-    uint32_t box[5] = {64, 1, (uint32_t)pitch, (uint32_t)win, 1};
+    uint32_t box[5] = {(uint32_t)s.bk, 1, (uint32_t)pitch, (uint32_t)win, 1};
     rc = make_map(&maps.a[0], in, 5, dims, str, box);
     if (rc) return rc;
     maps.a[1] = maps.a[2] = maps.a[3] = maps.a[0];
@@ -588,7 +627,7 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
   pick_grouping(s);
   rc = fit_tile<EpiWin>(s);
   if (rc) return rc;
-  rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.mma_n / s.cluster);
+  rc = map_rows(&maps.b, w, kt, c_out_pad, 1, kt, (long long)c_out_pad * kt, s.mma_n / s.cluster, s.bk);
   if (rc) return rc;
   EpiWin::Params ep{(__half*)out, (long long)c_out_pad * planes, split ? c_out_pad : 0, bias, act, slope,
                     b_ids, j_ids, wc, stride, org, in_h, in_w};

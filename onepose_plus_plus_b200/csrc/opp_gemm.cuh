@@ -1,7 +1,7 @@
 // opp_gemm.cuh — the one tensor-core engine of the hot path.
 //
 // D[M,N] = A[M,K] * W[N,K]^T on wgmma (fp16 operands, fp32 accumulators), operands staged by TMA
-// into 128B-swizzled shared memory through an mbarrier ring, persistent over output tiles.  The
+// into 128B- (or, for 32-wide slots, 64B-) swizzled shared memory through an mbarrier ring, persistent over output tiles.  The
 // producer warp keeps loading the next tile's operands while the epilogue of the current one runs.
 //
 // Precision: the reference computes in fp32 and the parity bar is 1e-3 on outputs whose logits
@@ -48,8 +48,12 @@
 namespace opp {
 
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;               // 64 fp16 = 128 B = one swizzle row
-constexpr int kABytes = kBlockM * kBlockK * 2;
+// A ring stage holds one K chunk of kBlockK = 64 fp16.  Its slot width (GemmShape.bk, the kernels'
+// BK) is the whole chunk, 128 B = one 128B-swizzle row, or half of it, 32 fp16 = one 64B-swizzle row:
+// the stage is then filled and released half by half, so the wide conv tiles (N = 208 / 256, two
+// stages) keep loads in flight while the MMAs still hold the other stage.
+constexpr int kBlockK = 64;
+__host__ __device__ constexpr int gemm_a_bytes(int bk) { return kBlockM * bk * 2; }   // one plane of the A tile
 constexpr int kMaxStages = 8;
 constexpr int kEpiParamBytes = 4096;   // bias / gamma,beta / lse vectors: 2 KB per epilogue group
 constexpr int kMaxEpiWarps = 8;
@@ -83,7 +87,9 @@ struct GemmShape {
   int block_n;      // output columns per tile (multiple of 16, <= 256)
   int mma_n;        // mma_width_for(block_n): W rows staged per tile and accumulator width
   int k_chunks;     // number of 64-wide K chunks per tile (per plane)
-  int stages;
+  int bk;           // K columns per ring slot: 64, or 32 (two slots per stage; conv modes only; a
+                    // compile-time parameter of the kernel)
+  int stages;       // ring stages of one K chunk each
   int b_batched;    // W operand has a leading batch dim
   int cluster;      // CTAs per cluster (1, 2, 4): they work on adjacent M tiles of the same
                     // (batch, n_tile) in lockstep and share the W tile through TMA multicast
@@ -1506,21 +1512,27 @@ __device__ __forceinline__ void mma_k_steps(float (&d)[N / 2], bool split, uint6
   }
 }
 
-template <int A_MODE, class Epi>
+template <int A_MODE, class Epi, int BK>
 __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShape& s,
                                           const typename Epi::Params& ep) {
   static_assert(Epi::kGroups == 2, "each of the two MMA warpgroups is one epilogue group");
+  static_assert(BK == 64 || BK == 32, "K chunk of one 128B- or 64B-swizzle row");
+  constexpr int kABytes = gemm_a_bytes(BK);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int planes = s.split ? 2 : 1;
   const bool nsc = s.pair == 2;   // N-split cluster: two independent CTAs, same M tile, N half = cluster rank
-  const int b_bytes = s.mma_n * kBlockK * 2;   // one plane of the W tile
-  const int a_stage = kABytes * planes;
+  // the ring: s.stages stages of one 64-wide K chunk each, a stage being kParts slots of BK columns
+  // with barriers of their own, so that it is filled and released a slot at a time
+  constexpr int kParts = kBlockK / BK;
+  const int slots = s.stages * kParts;
+  const int b_bytes = s.mma_n * BK * 2;   // one plane of the W tile of a slot
+  const int a_stage = kABytes * planes;    // bytes of a slot
   const int b_stage = b_bytes * planes;
-  const int ring = s.stages * (a_stage + b_stage);
+  const int ring = slots * (a_stage + b_stage);
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + s.stages * a_stage;
+  uint8_t* smem_b = smem + slots * a_stage;
   // register-fragment epilogues have no accumulator tile (and acc_alias = 0); only EpiConvUp has one
   constexpr bool kAccTile = !EpiFromRegs<Epi>::value;
   uint8_t* smem_acc = s.acc_alias ? smem : smem + ring;
@@ -1553,7 +1565,7 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
     tma_prefetch_desc(&maps.b);
   }
   if (warp == 0 && lane == 0) {
-    for (int i = 0; i < s.stages; ++i) {
+    for (int i = 0; i < slots; ++i) {
       mbar_init(&full[i], 1);
       // one arrival per MMA warpgroup of every CTA that reads the (multicast) stage
       mbar_init(&empty[i], 2 * csize);
@@ -1583,7 +1595,7 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
       int stage = 0;
       uint32_t phase = 0;
       const bool skip_b = (s.debug_skip & 1) != 0, skip_a = (s.debug_skip & 2) != 0;
-      const int a_tx = A_MODE == A_WIN ? s.tiles_x * s.tile_w * s.tile_h * (kBlockK * 2) * planes : a_stage;
+      const int a_tx = A_MODE == A_WIN ? s.tiles_x * s.tile_w * s.tile_h * (BK * 2) * planes : a_stage;
       const uint32_t tx_bytes = (skip_a ? 0 : a_tx) + (skip_b ? 0 : b_stage);
       int it = 0;
       for (int t = cluster_id; t < total_tiles; t += n_clusters, ++it) {
@@ -1623,95 +1635,93 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
         // incremental (tap, channel-chunk) counters instead of per-chunk divisions
         int cc = 0, ky = 0, kx = 0, kb_tap = 0;
         for (int chunk = 0; chunk < s.k_chunks; ++chunk) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          uint8_t* sa = smem_a + stage * a_stage;
-          uint8_t* sb = smem_b + stage * b_stage;
-          int kb;
-          if (A_MODE == A_ROWS) {
-            const bool first = chunk < s.k_chunks_a0;
-            const int kc = (first ? chunk : chunk - s.k_chunks_a0) * kBlockK;
-            const CUtensorMap* am = first ? &maps.a[0] : &maps.a[1];
-            const int lo = first ? s.a0_lo : s.a1_lo;
-            const int ba = (first && s.a0_shared) ? 0 : b;
-            kb = chunk * kBlockK;
-            if (elect_one()) {
-              mbar_expect_tx(&full[stage], tx_bytes);
-              if (!skip_a) {
-                tma_load_3d(am, &full[stage], sa, kc, m_tile * kBlockM, ba);
-                if (s.split) tma_load_3d(am, &full[stage], sa + kABytes, kc + lo, m_tile * kBlockM, ba);
-              }
-            }
-          } else if constexpr (A_MODE == A_WIN) {
-            // one TMA box (64 channels x tile_w x tile_h) per window and plane; windows past the match
-            // count re-read the last one (their rows are never stored)
-            kb = kb_tap + cc * kBlockK;
-            const int wbytes = s.tile_w * s.tile_h * (kBlockK * 2);
+          // K offset of this 64-wide chunk in A (A_ROWS) or its channel offset (conv modes), and in W
+          const bool first = A_MODE == A_ROWS && chunk < s.k_chunks_a0;
+          const int ka = A_MODE == A_ROWS ? (first ? chunk : chunk - s.k_chunks_a0) * kBlockK : cc * kBlockK;
+          const int kb = A_MODE == A_ROWS ? chunk * kBlockK : kb_tap + ka;
 #pragma unroll
-            for (int wi = 0; wi < 5; ++wi) {
-              if (wi >= s.tiles_x) break;
-              const int bx = win_x[wi] + kx, by = win_y[wi] + ky, bz = win_z[wi];
-              if (elect_one()) {
-                if (wi == 0) mbar_expect_tx(&full[stage], tx_bytes);
-                if (!skip_a) {
-                  tma_load_5d(&maps.a[0], &full[stage], sa + wi * wbytes, cc * kBlockK, 0, bx, by, bz);
+          for (int part = 0; part < kParts; ++part) {
+            const int kp = part * BK;   // K offset of this slot inside the chunk
+            mbar_wait(&empty[stage], phase ^ 1);
+            uint8_t* sa = smem_a + stage * a_stage;
+            uint8_t* sb = smem_b + stage * b_stage;
+            {
+              // (the second slot of a 16-channel tail chunk, 208 = 3 x 64 + 16, reads zeros past conv_c
+              // and the next tap's W columns: the MMA warpgroups issue no MMAs on it)
+              if constexpr (A_MODE == A_ROWS) {
+                const CUtensorMap* am = first ? &maps.a[0] : &maps.a[1];
+                const int lo = first ? s.a0_lo : s.a1_lo;
+                const int ba = (first && s.a0_shared) ? 0 : b;
+                if (elect_one()) {
+                  mbar_expect_tx(&full[stage], tx_bytes);
+                  if (!skip_a) {
+                    tma_load_3d(am, &full[stage], sa, ka + kp, m_tile * kBlockM, ba);
+                    if (s.split) tma_load_3d(am, &full[stage], sa + kABytes, ka + kp + lo, m_tile * kBlockM, ba);
+                  }
+                }
+              } else if constexpr (A_MODE == A_WIN) {
+                // one TMA box (BK channels x tile_w x tile_h) per window and plane; windows past the
+                // match count re-read the last one (their rows are never stored)
+                const int wbytes = s.tile_w * s.tile_h * (BK * 2);
+#pragma unroll
+                for (int wi = 0; wi < 5; ++wi) {
+                  if (wi >= s.tiles_x) break;
+                  const int bx = win_x[wi] + kx, by = win_y[wi] + ky, bz = win_z[wi];
+                  if (elect_one()) {
+                    if (wi == 0) mbar_expect_tx(&full[stage], tx_bytes);
+                    if (!skip_a) {
+                      tma_load_5d(&maps.a[0], &full[stage], sa + wi * wbytes, ka + kp, 0, bx, by, bz);
+                      if (s.split)
+                        tma_load_5d(&maps.a[0], &full[stage], sa + kABytes + wi * wbytes, ka + kp, 1, bx, by, bz);
+                    }
+                  }
+                }
+              } else {
+                int dy = ky - s.conv_pad, dx = kx - s.conv_pad, mi = 0;
+                if (s.conv_stride == 2) {
+                  const int py = dy & 1, px = dx & 1;
+                  dy = (dy - py) >> 1;
+                  dx = (dx - px) >> 1;
+                  mi = py * 2 + px;
+                }
+                const CUtensorMap* am = &maps.a[mi];
+                if (elect_one()) {
+                  mbar_expect_tx(&full[stage], tx_bytes);
+                  if (!skip_a) {
+                    tma_load_5d(am, &full[stage], sa, ka + kp, 0, ox0 + dx, oy0 + dy, b);
+                    if (s.split) tma_load_5d(am, &full[stage], sa + kABytes, ka + kp, 1, ox0 + dx, oy0 + dy, b);
+                  }
+                }
+              }
+              if (!skip_b && elect_one()) {
+                if (csize == 1) {
+                  tma_load_3d(&maps.b, &full[stage], sb, kb + kp, nrow0, bb);
+                  if (s.split) tma_load_3d(&maps.b, &full[stage], sb + b_bytes, s.b_lo + kb + kp, nrow0, bb);
+                } else {
+                  // this CTA fetches rows [crank*slice, +slice) of the W tile and multicasts them into
+                  // every CTA of the cluster (each CTA's full barrier expects the whole tile)
+                  const int slice = s.mma_n / csize;
+                  const int soff = crank * slice * (BK * 2);
+                  const int nrow = nrow0 + crank * slice;
+                  tma_load_3d_mc(&maps.b, &full[stage], sb + soff, kb + kp, nrow, bb, cmask);
                   if (s.split)
-                    tma_load_5d(&maps.a[0], &full[stage], sa + kABytes + wi * wbytes, cc * kBlockK, 1, bx, by, bz);
+                    tma_load_3d_mc(&maps.b, &full[stage], sb + b_bytes + soff, s.b_lo + kb + kp, nrow, bb, cmask);
                 }
               }
             }
-            if (++cc == s.conv_cchunks) {
-              cc = 0;
-              kb_tap += s.conv_c;
-              if (++kx == s.conv_kw) {
-                kx = 0;
-                ++ky;
-              }
-            }
-          } else {
-            int dy = ky - s.conv_pad, dx = kx - s.conv_pad, mi = 0;
-            if (s.conv_stride == 2) {
-              const int py = dy & 1, px = dx & 1;
-              dy = (dy - py) >> 1;
-              dx = (dx - px) >> 1;
-              mi = py * 2 + px;
-            }
-            kb = kb_tap + cc * kBlockK;
-            if (elect_one()) {
-              mbar_expect_tx(&full[stage], tx_bytes);
-              if (!skip_a) {
-                tma_load_5d(&maps.a[mi], &full[stage], sa, cc * kBlockK, 0, ox0 + dx, oy0 + dy, b);
-                if (s.split)
-                  tma_load_5d(&maps.a[mi], &full[stage], sa + kABytes, cc * kBlockK, 1, ox0 + dx, oy0 + dy, b);
-              }
-            }
-            if (++cc == s.conv_cchunks) {
-              cc = 0;
-              kb_tap += s.conv_c;
-              if (++kx == s.conv_kw) {
-                kx = 0;
-                ++ky;
-              }
+            __syncwarp();
+            if (++stage == slots) {
+              stage = 0;
+              phase ^= 1;
             }
           }
-          if (!skip_b && elect_one()) {
-            if (csize == 1) {
-              tma_load_3d(&maps.b, &full[stage], sb, kb, nrow0, bb);
-              if (s.split) tma_load_3d(&maps.b, &full[stage], sb + b_bytes, s.b_lo + kb, nrow0, bb);
-            } else {
-              // this CTA fetches rows [crank*slice, +slice) of the W tile and multicasts them into
-              // every CTA of the cluster (each CTA's full barrier expects the whole tile)
-              const int slice = s.mma_n / csize;
-              const int soff = crank * slice * (kBlockK * 2);
-              const int nrow = nrow0 + crank * slice;
-              tma_load_3d_mc(&maps.b, &full[stage], sb + soff, kb, nrow, bb, cmask);
-              if (s.split)
-                tma_load_3d_mc(&maps.b, &full[stage], sb + b_bytes + soff, s.b_lo + kb, nrow, bb, cmask);
+          if (A_MODE != A_ROWS && ++cc == s.conv_cchunks) {
+            cc = 0;
+            kb_tap += s.conv_c;
+            if (++kx == s.conv_kw) {
+              kx = 0;
+              ++ky;
             }
-          }
-          __syncwarp();
-          if (++stage == s.stages) {
-            stage = 0;
-            phase ^= 1;
           }
         }
       }
@@ -1734,10 +1744,10 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
     c.extra = reinterpret_cast<uint8_t*>(epi_smem) + epi_smem_bytes<Epi>() - EpiExtraSmem<Epi>::value;
     c.smem_s = smem_u32(c.smem);
     c.wstage_s = smem_u32(c.wstage);
-    // descriptors in 16-byte units: this warpgroup's 64 A rows start 64 * 128 B into the A tile;
-    // K advances 16 fp16 = 32 B (+2) inside the 128 B swizzle row; one wgmma reads all mma_n W rows
-    const uint64_t desc_tmpl = make_kmajor_sw128_desc(0);
-    const uint32_t sa0 = ((smem_u32(smem_a) >> 4) & 0x3FFF) + g * ((64 * 128) >> 4);
+    // descriptors in 16-byte units: this warpgroup's 64 A rows start 64 * (2 BK) B into the A tile;
+    // K advances 16 fp16 = 32 B (+2) inside the 2 BK-byte swizzle row; one wgmma reads all mma_n W rows
+    const uint64_t desc_tmpl = BK == 64 ? make_kmajor_sw128_desc(0) : make_kmajor_sw64_desc(0);
+    const uint32_t sa0 = ((smem_u32(smem_a) >> 4) & 0x3FFF) + g * ((64 * BK * 2) >> 4);
     const uint32_t sb0 = (smem_u32(smem_b) >> 4) & 0x3FFF;
     const uint32_t a_step = (uint32_t)a_stage >> 4, b_step = (uint32_t)b_stage >> 4;
     const uint32_t a_lo_off = kABytes >> 4, b_lo_off = (uint32_t)b_bytes >> 4;
@@ -1812,7 +1822,9 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
         for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
         wgmma_fence_acc(d);
         int prev = -1;
-        // one chunk: wait for its stage, KS K steps, then release the previous chunk's stage
+        static_assert(TAIL * 16 <= BK, "a tail chunk's channels lie in its first slot");
+        // one slot: wait for it, KS K steps (0: the empty second slot of a tail chunk), then release
+        // the previous slot
         auto chunk_step = [&](auto ks_c, auto& acc) {
           const uint64_t a_hi = desc_tmpl | sa, b_hi = desc_tmpl | sb;
           const uint64_t a_lo = desc_tmpl | (sa + a_lo_off), b_lo = desc_tmpl | (sb + b_lo_off);
@@ -1828,20 +1840,29 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
           prev = stage;
           sa += a_step;
           sb += b_step;
-          if (++stage == s.stages) {
+          if (++stage == slots) {
             stage = 0;
             phase ^= 1;
             sa = sa0;
             sb = sb0;
           }
         };
+        // one 64-wide chunk: its kParts slots; a tail chunk's steps all lie in the first slot
+        auto full_chunk = [&]() {
+#pragma unroll
+          for (int part = 0; part < kParts; ++part) chunk_step(std::integral_constant<int, BK / 16>{}, d);
+        };
+        auto tail_chunk = [&]() {
+          chunk_step(std::integral_constant<int, TAIL>{}, d);
+          if constexpr (kParts == 2) chunk_step(std::integral_constant<int, 0>{}, d);
+        };
         if constexpr (TAIL == 0) {
-          for (int chunk = 0; chunk < s.k_chunks; ++chunk) chunk_step(std::integral_constant<int, 4>{}, d);
+          for (int chunk = 0; chunk < s.k_chunks; ++chunk) full_chunk();
         } else {
           const int taps = s.k_chunks / s.conv_cchunks;
           for (int tap = 0; tap < taps; ++tap) {
-            for (int cc = 1; cc < s.conv_cchunks; ++cc) chunk_step(std::integral_constant<int, 4>{}, d);
-            chunk_step(std::integral_constant<int, TAIL>{}, d);
+            for (int cc = 1; cc < s.conv_cchunks; ++cc) full_chunk();
+            tail_chunk();
           }
         }
         wgmma_wait<0>();
@@ -1906,16 +1927,18 @@ __device__ __forceinline__ void gemm_body(const TensorMaps& maps, const GemmShap
   if (s.cluster > 1) cluster_sync_all(); else __syncthreads();
 }
 
-template <int A_MODE, class Epi>
+// BK (= GemmShape.bk) is a template parameter, not a runtime branch: a second copy of every mainloop
+// in one kernel made ptxas spill
+template <int A_MODE, class Epi, int BK = kBlockK>
 __global__ void __launch_bounds__(gemm_threads(Epi::kGroups), 1)
 gemm_kernel(const __grid_constant__ TensorMaps maps, const GemmShape s, const typename Epi::Params ep) {
-  gemm_body<A_MODE, Epi>(maps, s, ep);
+  gemm_body<A_MODE, Epi, BK>(maps, s, ep);
 }
 
 // Same kernel with the number of valid rows in device memory (the match count of the coarse
 // stage): rows = *rows_dev * rows_mult, so a whole forward can be enqueued — or captured in a CUDA
 // graph — without a host round trip.  The host-side rows / m_tiles describe the CAPACITY.
-template <int A_MODE, class Epi>
+template <int A_MODE, class Epi, int BK = kBlockK>
 __global__ void __launch_bounds__(gemm_threads(Epi::kGroups), 1)
 gemm_kernel_dyn(const __grid_constant__ TensorMaps maps, const GemmShape s_in,
                 const typename Epi::Params ep, const int* rows_dev, int rows_mult) {
@@ -1926,13 +1949,13 @@ gemm_kernel_dyn(const __grid_constant__ TensorMaps maps, const GemmShape s_in,
   const int tile_rows = A_MODE == A_WIN ? s_in.tiles_x * s_in.tile_w * s_in.tile_h : kBlockM;
   s.m_tiles = (s.rows + tile_rows - 1) / tile_rows;
   s.msup = (s.m_tiles + s_in.cluster - 1) / s_in.cluster;
-  gemm_body<A_MODE, Epi>(maps, s, ep);
+  gemm_body<A_MODE, Epi, BK>(maps, s, ep);
 }
 
 // Shared memory of a launch with epilogue Epi: operand ring, the accumulator tile (EpiConvUp only:
 // beside the ring, or over it when acc_alias), epilogue scratch, barriers and alignment slack.
 inline int gemm_stage_bytes(int mma_n, int split) {
-  return (kABytes + mma_n * kBlockK * 2) * (split ? 2 : 1);
+  return (gemm_a_bytes(kBlockK) + mma_n * kBlockK * 2) * (split ? 2 : 1);
 }
 template <class Epi>
 inline int gemm_smem_bytes(const GemmShape& s) {
@@ -1941,24 +1964,25 @@ inline int gemm_smem_bytes(const GemmShape& s) {
          epi_smem_bytes<Epi>() + (2 * kMaxStages + 2) * 8 + 16 + 1024;
 }
 constexpr int kSmemLimit = 227 * 1024;
-// Ring depth and accumulator placement for s.mma_n: the accumulator tile (if Epi has one) gets its
+// Ring depth (stages of one 64-wide K chunk, at most kMaxStages slots) and accumulator placement for s.mma_n: the accumulator tile (if Epi has one) gets its
 // own space when that leaves at least two stages, else it overlays the ring (which then holds at
 // least the tile).  `cap` (> 1) bounds the ring depth.  Returns false when even that does not fit.
 template <class Epi>
 inline bool gemm_pick_stages(GemmShape& s, int cap = 0) {
   const int avail = kSmemLimit - epi_smem_bytes<Epi>() - 2048;
   const int sb = gemm_stage_bytes(s.mma_n, s.split);
+  const int max_st = kMaxStages * s.bk / kBlockK;   // a barrier pair per slot
   const int ab = EpiFromRegs<Epi>::value ? 0 : gemm_acc_bytes(s.mma_n);
   int st = (avail - ab) / sb;
   s.acc_alias = ab > 0 && st < 2;
   if (s.acc_alias) st = avail / sb;
-  if (st > kMaxStages) st = kMaxStages;
+  if (st > max_st) st = max_st;
   if (st > s.k_chunks * 2 && s.k_chunks * 2 >= 2) st = s.k_chunks * 2;
   if (cap > 1 && st > cap) st = cap;
   if (st < 2) st = 2;
   if (s.acc_alias && st * sb < ab) st = (ab + sb - 1) / sb;
   s.stages = st;
-  return st <= kMaxStages && gemm_smem_bytes<Epi>(s) <= kSmemLimit;
+  return st <= max_st && gemm_smem_bytes<Epi>(s) <= kSmemLimit;
 }
 
 }  // namespace opp
