@@ -597,6 +597,45 @@ int opp_fine_train_attention_bwd(const float* qkv, const float* dout, float* dqk
 int opp_fine_train_match(const float* x, int m, float* expec_f, opp_stream_t stream);
 int opp_fine_train_match_bwd(const float* x, const float* dexpec, int m, float* dx, opp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training, coarse transformer (opp_train_coarse_tf.cu): linear attention of the coarse LoFTR
+ * layers (d = 256, 8 heads of 32) forward and backward, and LayerNorm over 256 channels, fp32.
+ * A sequence is passed as its first row, the row stride and len = rows per batch element (rows
+ * b*len + s); qkv rows are (q | k | v), 768 floats; masks are uint8 [batches*len] (1 = keep) or
+ * NULL.  Per head: K = elu(k) + 1, KV = sum_s (K_s m_s) (v_s m_s / len), ksum = sum_s K_s m_s,
+ * Q = (elu(q) + 1) m, out = (Q KV) v_len / (Q . ksum + eps).  Rows run in chunks
+ * (opp_coarse_tf_chunks); partials are summed in chunk order: every result is bit-reproducible.
+ * ---------------------------------------------------------------------------------------- */
+
+/* Chunks of a sequence of `len` rows per batch element (partials per batch element). */
+int opp_coarse_tf_chunks(int len);
+
+/* Source state of a sequence: kv fp32 [batches][8][32][32], ksum [batches][8][32]; part fp32
+ * [batches][chunks][8*32*32 + 8*32]. */
+int opp_coarse_tf_kv(const float* qkv, int ld, const unsigned char* mask, int batches, int len, float* part,
+                     float* kv, float* ksum, opp_stream_t stream);
+
+/* The message of every query row: out [batches*len][256] (row stride ldo). */
+int opp_coarse_tf_attn(const float* qkv, int ld, const unsigned char* q_mask, int batches, int len, const float* kv,
+                       const float* ksum, float v_len, float eps, float* out, int ldo, opp_stream_t stream);
+
+/* Backward, query rows: dqkv's q columns (overwritten) from dout, and the gradient of the source
+ * state dkv [batches][8][32][32], dksum [batches][8][32]; part as for opp_coarse_tf_kv. */
+int opp_coarse_tf_attn_bwd_q(const float* qkv, int ld, const unsigned char* q_mask, int batches, int len,
+                             const float* kv, const float* ksum, float v_len, float eps, const float* dout, int lddo,
+                             float* dqkv, int lddq, float* part, float* dkv, float* dksum, opp_stream_t stream);
+
+/* Backward, source rows (v_len = len): dqkv's k and v columns (overwritten) from dkv / dksum. */
+int opp_coarse_tf_attn_bwd_kv(const float* qkv, int ld, const unsigned char* mask, int batches, int len,
+                              const float* dkv, const float* dksum, float* dqkv, int lddq, opp_stream_t stream);
+
+/* LayerNorm over 256 channels, as opp_fine_train_ln / _ln_bwd (part [groups][2][256], dgb [2][256];
+ * groups = opp_fine_train_groups(rows)). */
+int opp_coarse_tf_ln(const float* x, int ldx, const float* gamma, const float* beta, const float* resid, int ldr,
+                     float* y, int ldy, float* stats, int rows, opp_stream_t stream);
+int opp_coarse_tf_ln_bwd(const float* x, int ldx, const float* gamma, const float* stats, const float* dy, int lddy,
+                         float* dx, int lddx, int rows, float* part, float* dgb, int accumulate, opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -80,6 +80,12 @@ SIGNATURES = {
     "opp_fine_train_attention_bwd": [P, P, P, I, I, F, P],
     "opp_fine_train_match": [P, I, P, P],
     "opp_fine_train_match_bwd": [P, P, I, P, P],
+    "opp_coarse_tf_kv": [P, I, P, I, I, P, P, P, P],
+    "opp_coarse_tf_attn": [P, I, P, I, I, P, P, F, F, P, I, P],
+    "opp_coarse_tf_attn_bwd_q": [P, I, P, I, I, P, P, F, F, P, I, P, I, P, P, P, P],
+    "opp_coarse_tf_attn_bwd_kv": [P, I, P, I, I, P, P, P, I, P],
+    "opp_coarse_tf_ln": [P, I, P, P, P, I, P, I, P, I, P],
+    "opp_coarse_tf_ln_bwd": [P, I, P, P, P, I, P, I, I, P, P, I, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),
@@ -87,6 +93,7 @@ PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles"
          "opp_conv_win_pitch": ([I], c_int),
          "opp_coarse_focal_blocks": ([I], c_int),
          "opp_fine_train_groups": ([I], c_int),
+         "opp_coarse_tf_chunks": ([I], c_int),
          "opp_pose_metrics_scratch_bytes": ([I, I], c_longlong),
          "opp_last_error": ([], ctypes.c_char_p)}
 
@@ -127,7 +134,8 @@ KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_ma
                     "opp_pose_metrics": 3,
                     "opp_coarse_focal_stats": 2, "opp_coarse_focal_fwd": 3, "opp_coarse_focal_bwd": 2,
                     "opp_gt_index": 5, "opp_coarse_focal_fwd_sparse": 3, "opp_coarse_focal_bwd_sparse": 2,
-                    "opp_fine_train_wgrad": 2, "opp_fine_train_ln_bwd": 2}
+                    "opp_fine_train_wgrad": 2, "opp_fine_train_ln_bwd": 2,
+                    "opp_coarse_tf_kv": 2, "opp_coarse_tf_attn_bwd_q": 2, "opp_coarse_tf_ln_bwd": 2}
 LAUNCHES = 0
 _PROFILE = None
 

@@ -23,6 +23,7 @@
 
 #include "../../include/opp_b200.h"
 #include "opp_common.cuh"
+#include "opp_train_rows.cuh"
 
 namespace opp {
 namespace {
@@ -31,14 +32,6 @@ constexpr int kTok = 26;        // 25 window tokens + the 3D token
 constexpr int kWin = 25;
 constexpr int kD = 128;         // d_model
 constexpr int kHeadDim = 16;    // d_model / nhead
-constexpr int kGroupRows = 256; // rows per partial of the weight / LayerNorm parameter gradients
-constexpr float kLnEps = 1e-5f;
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 // ------------------------------------------------------------------------------------------------
 // Gather: x[m·26 + t][0..127] (row stride ldx) from feat [B][128][Hf][Wf] and desc3d [B][128][N].
@@ -198,91 +191,6 @@ __global__ void __launch_bounds__(256) fine_wgrad_kernel(const float* __restrict
   for (int i = 0; i < 4; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) out[(size_t)(n0 + ty + 16 * i) * k + k0 + tx + 16 * j] = acc[i][j];
-}
-
-// out[e] (+)= sum_{g < groups} part[g][e], g ascending.
-__global__ void __launch_bounds__(256) fine_reduce_kernel(const float* __restrict__ part, int groups, int size,
-                                                          int accumulate, float* __restrict__ out) {
-  const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= size) return;
-  float s = 0.f;
-  for (int gi = 0; gi < groups; ++gi) s += part[(size_t)gi * size + e];
-  out[e] = accumulate ? out[e] + s : s;
-}
-
-// ------------------------------------------------------------------------------------------------
-// LayerNorm over 128 channels, one warp per row (4 channels per lane).
-// y = (x - mean) · rstd · gamma + beta (+ resid); stats[r] = (mean, rstd).
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) fine_ln_fwd_kernel(const float* __restrict__ x, int ldx,
-                                                          const float* __restrict__ gamma,
-                                                          const float* __restrict__ beta, const float* resid,
-                                                          int ldr, float* y, int ldy, float2* __restrict__ stats,
-                                                          int rows) {
-  const int lane = threadIdx.x & 31;
-  const int r = blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (r >= rows) return;
-  const float4 v = *reinterpret_cast<const float4*>(x + (size_t)r * ldx + lane * 4);
-  const float mean = warp_sum(v.x + v.y + v.z + v.w) * (1.f / kD);
-  const float d0 = v.x - mean, d1 = v.y - mean, d2 = v.z - mean, d3 = v.w - mean;
-  const float var = warp_sum(d0 * d0 + d1 * d1 + d2 * d2 + d3 * d3) * (1.f / kD);
-  const float rstd = rsqrtf(var + kLnEps);
-  const float4 gm = *reinterpret_cast<const float4*>(gamma + lane * 4);
-  const float4 bt = *reinterpret_cast<const float4*>(beta + lane * 4);
-  float4 o = make_float4(d0 * rstd * gm.x + bt.x, d1 * rstd * gm.y + bt.y, d2 * rstd * gm.z + bt.z,
-                         d3 * rstd * gm.w + bt.w);
-  if (resid) {
-    const float4 q = *reinterpret_cast<const float4*>(resid + (size_t)r * ldr + lane * 4);
-    o.x += q.x, o.y += q.y, o.z += q.z, o.w += q.w;
-  }
-  *reinterpret_cast<float4*>(y + (size_t)r * ldy + lane * 4) = o;
-  if (lane == 0) stats[r] = make_float2(mean, rstd);
-}
-
-// dx = rstd (dxh - mean(dxh) - xh mean(dxh xh)), dxh = dy gamma, xh = (x - mean) rstd; the partial
-// part[group][0 / 1][c] = sum over the group's rows of dy xh / dy (dgamma / dbeta).  8 warps per CTA,
-// kGroupRows rows per CTA; the warps' sums are combined in warp order.
-__global__ void __launch_bounds__(256) fine_ln_bwd_kernel(const float* __restrict__ x, int ldx,
-                                                          const float* __restrict__ gamma,
-                                                          const float2* __restrict__ stats,
-                                                          const float* __restrict__ dy, int lddy,
-                                                          float* __restrict__ dx, int lddx,
-                                                          float* __restrict__ part, int rows) {
-  __shared__ float red[8][2][kD];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int rb = blockIdx.x * kGroupRows, re = min(rows, rb + kGroupRows);
-  const float4 gm = *reinterpret_cast<const float4*>(gamma + lane * 4);
-  float sg[4] = {}, sb[4] = {};
-  for (int r = rb + wid; r < re; r += 8) {
-    const float2 st = stats[r];
-    const float4 v = *reinterpret_cast<const float4*>(x + (size_t)r * ldx + lane * 4);
-    const float4 g = *reinterpret_cast<const float4*>(dy + (size_t)r * lddy + lane * 4);
-    const float xh[4] = {(v.x - st.x) * st.y, (v.y - st.x) * st.y, (v.z - st.x) * st.y, (v.w - st.x) * st.y};
-    const float gg[4] = {g.x, g.y, g.z, g.w};
-    const float dxh[4] = {g.x * gm.x, g.y * gm.y, g.z * gm.z, g.w * gm.w};
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      s1 += dxh[i], s2 += dxh[i] * xh[i];
-      sg[i] = fmaf(gg[i], xh[i], sg[i]);
-      sb[i] += gg[i];
-    }
-    const float m1 = warp_sum(s1) * (1.f / kD), m2 = warp_sum(s2) * (1.f / kD);
-    float4 o;
-    o.x = st.y * (dxh[0] - m1 - xh[0] * m2);
-    o.y = st.y * (dxh[1] - m1 - xh[1] * m2);
-    o.z = st.y * (dxh[2] - m1 - xh[2] * m2);
-    o.w = st.y * (dxh[3] - m1 - xh[3] * m2);
-    *reinterpret_cast<float4*>(dx + (size_t)r * lddx + lane * 4) = o;
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) red[wid][0][lane * 4 + i] = sg[i], red[wid][1][lane * 4 + i] = sb[i];
-  __syncthreads();
-  const int e = threadIdx.x;   // 0..255 = (which, c)
-  float s = 0.f;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) s += red[w][e >> 7][e & (kD - 1)];
-  part[(size_t)blockIdx.x * 2 * kD + e] = s;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -627,7 +535,7 @@ int opp_fine_train_ln(const float* x, int ldx, const float* gamma, const float* 
   OPP_REQUIRE(x && gamma && beta && y && stats && aligned4(x, ldx) && aligned4(y, ldy) &&
                   (!resid || aligned4(resid, ldr)),
               "opp_fine_train_ln: bad operand");
-  fine_ln_fwd_kernel<<<(rows + 7) / 8, 256, 0, (cudaStream_t)stream>>>(x, ldx, gamma, beta, resid, ldr, y, ldy,
+  train_ln_fwd_kernel<kD><<<(rows + 7) / 8, 256, 0, (cudaStream_t)stream>>>(x, ldx, gamma, beta, resid, ldr, y, ldy,
                                                                       reinterpret_cast<float2*>(stats), rows);
   OPP_CHECK_CUDA(cudaGetLastError());
   return OPP_OK;
@@ -642,7 +550,7 @@ int opp_fine_train_ln_bwd(const float* x, int ldx, const float* gamma, const flo
               "opp_fine_train_ln_bwd: bad operand");
   const cudaStream_t st = (cudaStream_t)stream;
   const int groups = opp_fine_train_groups(rows);
-  fine_ln_bwd_kernel<<<groups, 256, 0, st>>>(x, ldx, gamma, reinterpret_cast<const float2*>(stats), dy, lddy, dx,
+  train_ln_bwd_kernel<kD><<<groups, 256, 0, st>>>(x, ldx, gamma, reinterpret_cast<const float2*>(stats), dy, lddy, dx,
                                              lddx, part, rows);
   OPP_CHECK_CUDA(cudaGetLastError());
   fine_reduce_kernel<<<1, 256, 0, st>>>(part, groups, 2 * kD, accumulate, dgb);

@@ -654,6 +654,9 @@ class OnePosePlus_model(_Engine):
         # fine level of .train() on CUDA: "autograd" = train_path's PyTorch functions, "kernels" = the
         # opp_fine_train_* kernels forward and backward (train_fine.py; no unfold tensor)
         self.fine_train_mode = os.environ.get("OPP_B200_FINE_TRAIN", "autograd")
+        # coarse transformer of .train() on CUDA: "autograd" = train_path.transformer, "kernels" = the
+        # opp_coarse_tf_* kernels forward and backward, recomputing one layer at a time (train_coarse_tf.py)
+        self.coarse_transformer_train_mode = os.environ.get("OPP_B200_COARSE_TF_TRAIN", "autograd")
         # one-pass dual softmax: column statistics of sim / conf from the row passes (warp
         # butterflies in the epilogue) instead of two more sim GEMM passes
         self.coarse_colmax = os.environ.get("OPP_B200_COLMAX", "1") == "1"

@@ -556,3 +556,67 @@ def fine_train_match_bwd(x, dexpec, m, dx):
 
 def fine_train_groups(rows):
     return _lib.load().opp_fine_train_groups(rows)
+
+
+# ---- training, coarse transformer (opp_train_coarse_tf.cu; used by train_coarse_tf.py) -----------
+# A sequence is a row view [batches * len, ...] of the shared row buffer; masks are uint8 [batches * len].
+
+COARSE_TF_STATE = 8 * 32 * 32 + 8 * 32      # floats per partial: KV [8][32][32], ksum [8][32]
+
+
+def coarse_tf_chunks(length):
+    return _lib.load().opp_coarse_tf_chunks(length)
+
+
+def coarse_tf_part(batches, length, device):
+    """The partial buffer of coarse_tf_kv / coarse_tf_attn_bwd_q for a sequence of `length` rows."""
+    return torch.empty(batches, coarse_tf_chunks(length), COARSE_TF_STATE, dtype=torch.float32, device=device)
+
+
+def _coarse_seq(qkv, mask, batches):
+    rows = qkv.shape[0]
+    if rows % batches:
+        raise ValueError(f"{rows} rows do not split into {batches} batch elements")
+    _chk(mask, torch.uint8, "mask")
+    if mask is not None and mask.numel() != rows:
+        raise ValueError(f"mask has {mask.numel()} entries for {rows} rows")
+    return rows // batches
+
+
+def coarse_tf_kv(qkv, mask, batches, part, kv, ksum):
+    """kv [B, 8, 32, 32], ksum [B, 8, 32] (contiguous fp32, overwritten) of the source rows qkv."""
+    length = _coarse_seq(qkv, mask, batches)
+    _chk(kv, torch.float32, "kv")
+    _chk(ksum, torch.float32, "ksum")
+    call("opp_coarse_tf_kv", ptr(qkv), _ld(qkv), ptr(mask), batches, length, ptr(part), ptr(kv), ptr(ksum), stream())
+
+
+def coarse_tf_attn(qkv, q_mask, batches, kv, ksum, v_len, out, eps=1e-6):
+    length = _coarse_seq(qkv, q_mask, batches)
+    call("opp_coarse_tf_attn", ptr(qkv), _ld(qkv), ptr(q_mask), batches, length, ptr(kv), ptr(ksum), float(v_len),
+         float(eps), ptr(out), _ld(out), stream())
+
+
+def coarse_tf_attn_bwd_q(qkv, q_mask, batches, kv, ksum, v_len, dout, dqkv, part, dkv, dksum, eps=1e-6):
+    length = _coarse_seq(qkv, q_mask, batches)
+    _chk(dkv, torch.float32, "dkv")
+    _chk(dksum, torch.float32, "dksum")
+    call("opp_coarse_tf_attn_bwd_q", ptr(qkv), _ld(qkv), ptr(q_mask), batches, length, ptr(kv), ptr(ksum),
+         float(v_len), float(eps), ptr(dout), _ld(dout), ptr(dqkv), _ld(dqkv), ptr(part), ptr(dkv), ptr(dksum),
+         stream())
+
+
+def coarse_tf_attn_bwd_kv(qkv, mask, batches, dkv, dksum, dqkv):
+    length = _coarse_seq(qkv, mask, batches)
+    call("opp_coarse_tf_attn_bwd_kv", ptr(qkv), _ld(qkv), ptr(mask), batches, length, ptr(dkv), ptr(dksum),
+         ptr(dqkv), _ld(dqkv), stream())
+
+
+def coarse_tf_ln(x, gamma, beta, resid, y, stats):
+    call("opp_coarse_tf_ln", ptr(x), _ld(x), ptr(gamma), ptr(beta), ptr(resid), _ld(resid), ptr(y), _ld(y),
+         ptr(stats), x.shape[0], stream())
+
+
+def coarse_tf_ln_bwd(x, gamma, stats, dy, dx, part, dgb, accumulate):
+    call("opp_coarse_tf_ln_bwd", ptr(x), _ld(x), ptr(gamma), ptr(stats), ptr(dy), _ld(dy), ptr(dx), _ld(dx),
+         x.shape[0], ptr(part), ptr(dgb), int(accumulate), stream())

@@ -16,7 +16,8 @@ confidence matrix is not built — the statistics and the match selection run on
 kernels and ``data["conf_matrix"]`` is a TrainConfHandle that ``losses.Loss`` differentiates with
 the opp_coarse_focal kernels (DESIGN §7 f4).  With ``model.fine_train_mode == "kernels"`` on CUDA
 tensors the fine level (fine_preprocess -> loftr_fine -> fine_matching) runs on the
-opp_fine_train_* kernels instead (train_fine.py).  The ground truth the padding draws from is
+opp_fine_train_* kernels instead (train_fine.py), and with model.coarse_transformer_train_mode ==
+"kernels" the coarse transformer runs on the opp_coarse_tf_* kernels (train_coarse_tf.py).  The ground truth the padding draws from is
 data["conf_matrix_gt"] or, in its place, the correspondence list data["gt_sparse"] (train_gt.py).
 
 Every function cites the reference lines it follows.
@@ -24,7 +25,7 @@ Every function cites the reference lines it follows.
 import torch
 import torch.nn.functional as F
 
-from . import train_fine, train_gt
+from . import train_coarse_tf, train_fine, train_gt
 
 
 def _block(blk, x):
@@ -319,6 +320,7 @@ def forward_train(model, data):
         raise ValueError('conf_matrix_mode "lazy" in train mode needs precision "fp16x3" (the match '
                          'selection runs on the fp32-grade split operands)')
     fine_kernels = train_fine.use_kernels(model, data)
+    coarse_tf_kernels = train_coarse_tf.use_kernels(model, data)
     data.update({"bs": img.size(0), "q_hw_i": img.shape[2:]})
     feat_c, feat_f = backbone(model.backbone, img)
     data.update({"q_hw_c": feat_c.shape[2:], "q_hw_f": feat_f.shape[2:]})
@@ -328,7 +330,10 @@ def forward_train(model, data):
     dsel = data["descriptors3d_coarse_db"] if "descriptors3d_coarse_db" in data else data["descriptors3d_db"]
     d3 = keypoint_encoding(model.kpt_3d_pos_encoding, normalize_3d_keypoints(data["keypoints3d"]), dsel)
     qmask = data["query_image_mask"].flatten(-2) if "query_image_mask" in data else None
-    d3, q_c = transformer(model.loftr_coarse, d3, q_c, qmask)
+    if coarse_tf_kernels:
+        d3, q_c = train_coarse_tf.coarse_transformer(model.loftr_coarse, d3, q_c, qmask)
+    else:
+        d3, q_c = transformer(model.loftr_coarse, d3, q_c, qmask)
     coarse_matching(model.coarse_matching, d3, q_c, data, qmask, model.training, lazy_split)
     if not cfg["fine_matching"]["enable"]:
         data.update({"mkpts_query_f": data["mkpts_query_c"]})
