@@ -636,6 +636,54 @@ int opp_coarse_tf_ln(const float* x, int ldx, const float* gamma, const float* b
 int opp_coarse_tf_ln_bwd(const float* x, int ldx, const float* gamma, const float* stats, const float* dy, int lddy,
                          float* dx, int lddx, int rows, float* part, float* dgb, int accumulate, opp_stream_t stream);
 
+
+/* ------------------------------------------------------------------------------------------
+ * Training, backbone (opp_train_backbone.cu): the ResNet-FPN's convolutions, batch-statistics
+ * BatchNorm + activation (+ residual) and the FPN's bilinear x2 upsample-add, forward and backward,
+ * fp32 on the CUDA cores.  Maps are NCHW fp32; weights [c_out][c_in][k][k]; k in {1, 3, 7},
+ * stride in {1, 2}, pad = k / 2; (h, w) is the convolution's input size.  Every sum runs in a fixed
+ * order without floating-point atomics: results are bit-reproducible.
+ * ---------------------------------------------------------------------------------------- */
+
+/* Output pixels per weight-gradient partial; BatchNorm partials of a [batches][c][hw] map per channel. */
+int opp_backbone_train_wgrad_group(void);
+int opp_backbone_train_bn_parts(int batches, int hw);
+
+/* y [batches][c_out][ho][wo] = conv(x, w). */
+int opp_backbone_train_conv(const float* x, const float* w, int batches, int c_in, int h, int wd, int c_out, int ksize,
+                            int stride, float* y, opp_stream_t stream);
+/* dx [batches][c_in][h][w] (+)= the data gradient of dy [batches][c_out][ho][wo]. */
+int opp_backbone_train_conv_dgrad(const float* dy, const float* w, int batches, int c_in, int h, int wd, int c_out,
+                                  int ksize, int stride, float* dx, int accumulate, opp_stream_t stream);
+/* dw (+)= the weight gradient summed over the output pixels [pix0, pix0 + npix) of the flat (b, oy, ox)
+ * index; pix0 a multiple of the group; part fp32 [ceil(npix / group)][c_out * c_in * k * k]. */
+int opp_backbone_train_conv_wgrad(const float* x, const float* dy, int batches, int c_in, int h, int wd, int c_out,
+                                  int ksize, int stride, int pix0, int npix, float* part, float* dw, int accumulate,
+                                  opp_stream_t stream);
+/* mean / invstd [c] of x [batches][c][hw] over batches * hw values (biased variance); when
+ * running_mean / running_var are given they are updated as F.batch_norm does (unbiased variance).
+ * part fp64 [c][parts][2]. */
+int opp_backbone_train_bn_stats(const float* x, int batches, int c, int hw, float eps, double* part, float* mean,
+                                float* invstd, float* running_mean, float* running_var, float momentum,
+                                opp_stream_t stream);
+/* y = act(gamma (x - mean) invstd + beta [+ res]); act 0 none, 1 ReLU, 2 LeakyReLU(0.01). */
+int opp_backbone_train_bn_act(const float* x, int batches, int c, int hw, const float* mean, const float* invstd,
+                              const float* gamma, const float* beta, const float* res, int act, float* y,
+                              opp_stream_t stream);
+/* Backward of opp_backbone_train_bn_act given its output y (NULL for act 0): dz = dy act'(y);
+ * dx = gamma invstd (dz - sum dz / n - xhat sum(dz xhat) / n) when batch_stats, else gamma invstd dz;
+ * dres = dz (or NULL); dgb [2][c] = (dgamma, dbeta).  dx may alias dy.  part fp64 [c][parts * 2 + 1]. */
+int opp_backbone_train_bn_act_bwd(const float* x, const float* y, const float* dy, int batches, int c, int hw,
+                                  const float* mean, const float* invstd, const float* gamma, int act,
+                                  int batch_stats, double* part, float* dx, float* dres, float* dgb,
+                                  opp_stream_t stream);
+/* out [batches][c][2h][2w] = lat + bilinear x2 (align_corners) of in [batches][c][h][w]; out may alias lat. */
+int opp_backbone_train_up2x_add(const float* in, const float* lat, int batches, int c, int h, int w, float* out,
+                                opp_stream_t stream);
+/* din [batches][c][h][w] (+)= the upsample's backward of dout [batches][c][2h][2w]. */
+int opp_backbone_train_up2x_bwd(const float* dout, int batches, int c, int h, int w, float* din, int accumulate,
+                                opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

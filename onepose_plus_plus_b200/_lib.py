@@ -86,6 +86,14 @@ SIGNATURES = {
     "opp_coarse_tf_attn_bwd_kv": [P, I, P, I, I, P, P, P, I, P],
     "opp_coarse_tf_ln": [P, I, P, P, P, I, P, I, P, I, P],
     "opp_coarse_tf_ln_bwd": [P, I, P, P, P, I, P, I, I, P, P, I, P],
+    "opp_backbone_train_conv": [P, P, I, I, I, I, I, I, I, P, P],
+    "opp_backbone_train_conv_dgrad": [P, P, I, I, I, I, I, I, I, P, I, P],
+    "opp_backbone_train_conv_wgrad": [P, P, I, I, I, I, I, I, I, I, I, P, P, I, P],
+    "opp_backbone_train_bn_stats": [P, I, I, I, F, P, P, P, P, P, F, P],
+    "opp_backbone_train_bn_act": [P, I, I, I, P, P, P, P, P, I, P, P],
+    "opp_backbone_train_bn_act_bwd": [P, P, P, I, I, I, P, P, P, I, I, P, P, P, P, P],
+    "opp_backbone_train_up2x_add": [P, P, I, I, I, I, P, P],
+    "opp_backbone_train_up2x_bwd": [P, I, I, I, I, P, I, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),
@@ -94,6 +102,8 @@ PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles"
          "opp_coarse_focal_blocks": ([I], c_int),
          "opp_fine_train_groups": ([I], c_int),
          "opp_coarse_tf_chunks": ([I], c_int),
+         "opp_backbone_train_wgrad_group": ([], c_int),
+         "opp_backbone_train_bn_parts": ([I, I], c_int),
          "opp_pose_metrics_scratch_bytes": ([I, I], c_longlong),
          "opp_last_error": ([], ctypes.c_char_p)}
 
@@ -135,7 +145,9 @@ KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_ma
                     "opp_coarse_focal_stats": 2, "opp_coarse_focal_fwd": 3, "opp_coarse_focal_bwd": 2,
                     "opp_gt_index": 5, "opp_coarse_focal_fwd_sparse": 3, "opp_coarse_focal_bwd_sparse": 2,
                     "opp_fine_train_wgrad": 2, "opp_fine_train_ln_bwd": 2,
-                    "opp_coarse_tf_kv": 2, "opp_coarse_tf_attn_bwd_q": 2, "opp_coarse_tf_ln_bwd": 2}
+                    "opp_coarse_tf_kv": 2, "opp_coarse_tf_attn_bwd_q": 2, "opp_coarse_tf_ln_bwd": 2,
+                    "opp_backbone_train_conv_wgrad": 2, "opp_backbone_train_bn_stats": 2,
+                    "opp_backbone_train_bn_act_bwd": 3}
 LAUNCHES = 0
 _PROFILE = None
 

@@ -657,6 +657,9 @@ class OnePosePlus_model(_Engine):
         # coarse transformer of .train() on CUDA: "autograd" = train_path.transformer, "kernels" = the
         # opp_coarse_tf_* kernels forward and backward, recomputing one layer at a time (train_coarse_tf.py)
         self.coarse_transformer_train_mode = os.environ.get("OPP_B200_COARSE_TF_TRAIN", "autograd")
+        # backbone of .train() on CUDA: "autograd" = train_path.backbone (cuDNN), "kernels" = the
+        # opp_backbone_train_* kernels forward and backward, recomputing one segment at a time (train_backbone.py)
+        self.backbone_train_mode = os.environ.get("OPP_B200_BACKBONE_TRAIN", "autograd")
         # one-pass dual softmax: column statistics of sim / conf from the row passes (warp
         # butterflies in the epilogue) instead of two more sim GEMM passes
         self.coarse_colmax = os.environ.get("OPP_B200_COLMAX", "1") == "1"

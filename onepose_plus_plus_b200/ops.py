@@ -620,3 +620,123 @@ def coarse_tf_ln(x, gamma, beta, resid, y, stats):
 def coarse_tf_ln_bwd(x, gamma, stats, dy, dx, part, dgb, accumulate):
     call("opp_coarse_tf_ln_bwd", ptr(x), _ld(x), ptr(gamma), ptr(stats), ptr(dy), _ld(dy), ptr(dx), _ld(dx),
          x.shape[0], ptr(part), ptr(dgb), int(accumulate), stream())
+
+
+# ---- training, backbone (opp_train_backbone.cu; used by train_backbone.py) ------------------------
+# Maps are contiguous NCHW fp32 CUDA tensors; weights [c_out, c_in, k, k] with pad k // 2.
+
+BB_ACT = {"none": 0, "relu": 1, "leaky": 2}
+
+
+def backbone_wgrad_group():
+    """Output pixels per weight-gradient partial (a slice of backbone_conv_wgrad starts at a multiple)."""
+    return _lib.load().opp_backbone_train_wgrad_group()
+
+
+def backbone_bn_part(batches, c, hw, device):
+    """The fp64 partial buffer of backbone_bn_stats / backbone_bn_act_bwd for a [batches, c, hw] map."""
+    parts = _lib.load().opp_backbone_train_bn_parts(batches, hw)
+    return torch.empty(c * (2 * parts + 1), dtype=torch.float64, device=device)
+
+
+def _conv_args(x, w, stride):
+    _chk(x, torch.float32, "x")
+    _chk(w, torch.float32, "w")
+    B, C, H, W = x.shape
+    co, ci, k, k2 = w.shape
+    if ci != C or k != k2:
+        raise ValueError(f"weight {tuple(w.shape)} does not fit input {tuple(x.shape)}")
+    return B, C, H, W, co, k, int(stride)
+
+
+def conv_out_hw(h, w, k, stride):
+    pad = k // 2
+    return (h + 2 * pad - k) // stride + 1, (w + 2 * pad - k) // stride + 1
+
+
+def backbone_conv(x, w, stride, y):
+    """y [B, c_out, ho, wo] = conv2d(x, w, stride, padding=k // 2)."""
+    B, C, H, W, co, k, s = _conv_args(x, w, stride)
+    _chk(y, torch.float32, "y")
+    if tuple(y.shape) != (B, co, *conv_out_hw(H, W, k, s)):
+        raise ValueError(f"y has shape {tuple(y.shape)}")
+    call("opp_backbone_train_conv", ptr(x), ptr(w), B, C, H, W, co, k, s, ptr(y), stream())
+
+
+def backbone_conv_dgrad(dy, w, stride, dx, accumulate):
+    """dx [B, c_in, h, w] (+)= the input gradient of conv2d(., w, stride) for the output gradient dy."""
+    B, C, H, W, co, k, s = _conv_args(dx, w, stride)
+    _chk(dy, torch.float32, "dy")
+    if tuple(dy.shape) != (B, co, *conv_out_hw(H, W, k, s)):
+        raise ValueError(f"dy has shape {tuple(dy.shape)}")
+    call("opp_backbone_train_conv_dgrad", ptr(dy), ptr(w), B, C, H, W, co, k, s, ptr(dx), int(accumulate), stream())
+
+
+def backbone_conv_wgrad(x, dy, stride, dw, part, pix0, npix, accumulate):
+    """dw (+)= the weight gradient over output pixels [pix0, pix0 + npix) of the flat (b, oy, ox) index;
+    part fp32 with at least ceil(npix / group) * dw.numel() entries."""
+    B, C, H, W, co, k, s = _conv_args(x, dw, stride)
+    _chk(dy, torch.float32, "dy")
+    _chk(part, torch.float32, "part")
+    if tuple(dy.shape) != (B, co, *conv_out_hw(H, W, k, s)):
+        raise ValueError(f"dy has shape {tuple(dy.shape)}")
+    group = backbone_wgrad_group()
+    if part.numel() < -(-npix // group) * dw.numel():
+        raise ValueError("wgrad partial buffer too small")
+    call("opp_backbone_train_conv_wgrad", ptr(x), ptr(dy), B, C, H, W, co, k, s, int(pix0), int(npix), ptr(part),
+         ptr(dw), int(accumulate), stream())
+
+
+def _bn_map(x):
+    _chk(x, torch.float32, "x")
+    B, C, H, W = x.shape
+    return B, C, H * W
+
+
+def backbone_bn_stats(x, eps, part, mean, invstd, running_mean=None, running_var=None, momentum=0.0):
+    """mean / invstd [C] of x over (B, H, W); running_mean / running_var updated in place when given."""
+    B, C, hw = _bn_map(x)
+    for t, n in ((mean, "mean"), (invstd, "invstd"), (running_mean, "running_mean"), (running_var, "running_var")):
+        _chk(t, torch.float32, n)
+    call("opp_backbone_train_bn_stats", ptr(x), B, C, hw, float(eps), ptr(part), ptr(mean), ptr(invstd),
+         ptr(running_mean), ptr(running_var), float(momentum), stream())
+
+
+def backbone_bn_act(x, mean, invstd, gamma, beta, res, act, y):
+    """y = act(gamma (x - mean) invstd + beta [+ res]), act "none" / "relu" / "leaky"."""
+    B, C, hw = _bn_map(x)
+    _chk(res, torch.float32, "res")
+    _chk(y, torch.float32, "y")
+    call("opp_backbone_train_bn_act", ptr(x), B, C, hw, ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(res),
+         BB_ACT[act], ptr(y), stream())
+
+
+def backbone_bn_act_bwd(x, y, dy, mean, invstd, gamma, act, batch_stats, part, dx, dres, dgb):
+    """Backward of backbone_bn_act from its output y (None for act "none"): dx, dres (= d res, or None)
+    and dgb [2, C] = (dgamma, dbeta), all overwritten; dx may be dy."""
+    B, C, hw = _bn_map(x)
+    for t, n in ((y, "y"), (dy, "dy"), (dx, "dx"), (dres, "dres"), (dgb, "dgb")):
+        _chk(t, torch.float32, n)
+    call("opp_backbone_train_bn_act_bwd", ptr(x), ptr(y), ptr(dy), B, C, hw, ptr(mean), ptr(invstd), ptr(gamma),
+         BB_ACT[act], int(batch_stats), ptr(part), ptr(dx), ptr(dres), ptr(dgb), stream())
+
+
+def backbone_up2x_add(x, lat, out):
+    """out = lat + interpolate(x, scale_factor=2, bilinear, align_corners=True); out may be lat."""
+    _chk(x, torch.float32, "x")
+    _chk(lat, torch.float32, "lat")
+    _chk(out, torch.float32, "out")
+    B, C, h, w = x.shape
+    if tuple(lat.shape) != (B, C, 2 * h, 2 * w) or lat.shape != out.shape:
+        raise ValueError(f"lateral {tuple(lat.shape)} does not match 2x {tuple(x.shape)}")
+    call("opp_backbone_train_up2x_add", ptr(x), ptr(lat), B, C, h, w, ptr(out), stream())
+
+
+def backbone_up2x_bwd(dout, din, accumulate):
+    """din [B, C, h, w] (+)= the backward of the x2 upsample for dout [B, C, 2h, 2w]."""
+    _chk(dout, torch.float32, "dout")
+    _chk(din, torch.float32, "din")
+    B, C, h, w = din.shape
+    if tuple(dout.shape) != (B, C, 2 * h, 2 * w):
+        raise ValueError(f"dout {tuple(dout.shape)} does not match 2x {tuple(din.shape)}")
+    call("opp_backbone_train_up2x_bwd", ptr(dout), B, C, h, w, ptr(din), int(accumulate), stream())

@@ -17,7 +17,9 @@ kernels and ``data["conf_matrix"]`` is a TrainConfHandle that ``losses.Loss`` di
 the opp_coarse_focal kernels (DESIGN §7 f4).  With ``model.fine_train_mode == "kernels"`` on CUDA
 tensors the fine level (fine_preprocess -> loftr_fine -> fine_matching) runs on the
 opp_fine_train_* kernels instead (train_fine.py), and with model.coarse_transformer_train_mode ==
-"kernels" the coarse transformer runs on the opp_coarse_tf_* kernels (train_coarse_tf.py).  The ground truth the padding draws from is
+"kernels" the coarse transformer runs on the opp_coarse_tf_* kernels (train_coarse_tf.py).  With
+model.backbone_train_mode == "kernels" the ResNet-FPN backbone runs on the opp_backbone_train_*
+kernels, BatchNorm following each module's .training (train_backbone.py).  The ground truth the padding draws from is
 data["conf_matrix_gt"] or, in its place, the correspondence list data["gt_sparse"] (train_gt.py).
 
 Every function cites the reference lines it follows.
@@ -25,7 +27,7 @@ Every function cites the reference lines it follows.
 import torch
 import torch.nn.functional as F
 
-from . import train_coarse_tf, train_fine, train_gt
+from . import train_backbone, train_coarse_tf, train_fine, train_gt
 
 
 def _block(blk, x):
@@ -321,8 +323,12 @@ def forward_train(model, data):
                          'selection runs on the fp32-grade split operands)')
     fine_kernels = train_fine.use_kernels(model, data)
     coarse_tf_kernels = train_coarse_tf.use_kernels(model, data)
+    backbone_kernels = train_backbone.use_kernels(model, data)
     data.update({"bs": img.size(0), "q_hw_i": img.shape[2:]})
-    feat_c, feat_f = backbone(model.backbone, img)
+    if backbone_kernels:
+        feat_c, feat_f = train_backbone.backbone(model.backbone, img)
+    else:
+        feat_c, feat_f = backbone(model.backbone, img)
     data.update({"q_hw_c": feat_c.shape[2:], "q_hw_f": feat_f.shape[2:]})
     if model.dense_pos_encoding is not None:
         feat_c = feat_c + model.dense_pos_encoding.pe[:, :, :feat_c.size(2), :feat_c.size(3)]
