@@ -684,6 +684,29 @@ int opp_backbone_train_up2x_add(const float* in, const float* lat, int batches, 
 int opp_backbone_train_up2x_bwd(const float* dout, int batches, int c, int h, int w, float* din, int accumulate,
                                 opp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training, keypoint encoder (opp_train_kpt.cu): KeypointEncoding_linear 3-32-64-128-256 with
+ * per-point InstanceNorm (eps 1e-5) + ReLU after the hidden layers, forward and backward, fp32 on the
+ * CUDA cores.  kpts fp32 [batch][n][3] with stats [batch][4] from opp_kpt_stats; rows are the flat
+ * (b, n) index.  pack fp32 [opp_kpt_train_pack_size()]: W1t b1 W2t b2 W3t b3 W4t b4 (weights
+ * transposed, [in][out]) then W2 W3 W4 ([out][in]).  dparams fp32 [opp_kpt_train_params()]: dW1 db1
+ * dW2 db2 dW3 db3 dW4 db4 in nn.Linear's layouts.  No floating-point atomics: bit-reproducible.
+ * ---------------------------------------------------------------------------------------- */
+
+/* Rows per weight-gradient partial (a backward slice starts at a multiple); floats of dparams / pack. */
+int opp_kpt_train_group(void);
+int opp_kpt_train_params(void);
+int opp_kpt_train_pack_size(void);
+
+/* out fp32 [batch * n][256] = desc^T + MLP(normalised kpts); desc fp32 [batch][256][n]. */
+int opp_kpt_train_fwd(const float* kpts, const float* stats, const float* desc, const float* pack, float* out,
+                      int batch, int n, opp_stream_t stream);
+/* dparams (+)= the parameter gradient of out for dout fp32 [batch * n][256], summed over the rows
+ * [row0, row0 + nrows) (row0 a multiple of the group) by recomputing their forward; part fp32
+ * [ceil(nrows / group)][opp_kpt_train_params()] holds one partial per group, summed in group order. */
+int opp_kpt_train_bwd(const float* kpts, const float* stats, const float* dout, const float* pack, int batch, int n,
+                      int row0, int nrows, float* part, float* dparams, int accumulate, opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -94,6 +94,8 @@ SIGNATURES = {
     "opp_backbone_train_bn_act_bwd": [P, P, P, I, I, I, P, P, P, I, I, P, P, P, P, P],
     "opp_backbone_train_up2x_add": [P, P, I, I, I, I, P, P],
     "opp_backbone_train_up2x_bwd": [P, I, I, I, I, P, I, P],
+    "opp_kpt_train_fwd": [P, P, P, P, P, I, I, P],
+    "opp_kpt_train_bwd": [P, P, P, P, I, I, I, I, P, P, I, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),
@@ -104,6 +106,9 @@ PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles"
          "opp_coarse_tf_chunks": ([I], c_int),
          "opp_backbone_train_wgrad_group": ([], c_int),
          "opp_backbone_train_bn_parts": ([I, I], c_int),
+         "opp_kpt_train_group": ([], c_int),
+         "opp_kpt_train_params": ([], c_int),
+         "opp_kpt_train_pack_size": ([], c_int),
          "opp_pose_metrics_scratch_bytes": ([I, I], c_longlong),
          "opp_last_error": ([], ctypes.c_char_p)}
 
@@ -147,7 +152,7 @@ KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_ma
                     "opp_fine_train_wgrad": 2, "opp_fine_train_ln_bwd": 2,
                     "opp_coarse_tf_kv": 2, "opp_coarse_tf_attn_bwd_q": 2, "opp_coarse_tf_ln_bwd": 2,
                     "opp_backbone_train_conv_wgrad": 2, "opp_backbone_train_bn_stats": 2,
-                    "opp_backbone_train_bn_act_bwd": 3}
+                    "opp_backbone_train_bn_act_bwd": 3, "opp_kpt_train_bwd": 2}
 LAUNCHES = 0
 _PROFILE = None
 

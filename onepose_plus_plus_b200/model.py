@@ -660,6 +660,9 @@ class OnePosePlus_model(_Engine):
         # backbone of .train() on CUDA: "autograd" = train_path.backbone (cuDNN), "kernels" = the
         # opp_backbone_train_* kernels forward and backward, recomputing one segment at a time (train_backbone.py)
         self.backbone_train_mode = os.environ.get("OPP_B200_BACKBONE_TRAIN", "autograd")
+        # keypoint encoder of .train() on CUDA: "autograd" = train_path.keypoint_encoding, "kernels" = the
+        # opp_kpt_train_* kernels forward and backward, recomputing each point's MLP (train_kpt.py)
+        self.kpt_encoder_train_mode = os.environ.get("OPP_B200_KPT_TRAIN", "autograd")
         # one-pass dual softmax: column statistics of sim / conf from the row passes (warp
         # butterflies in the epilogue) instead of two more sim GEMM passes
         self.coarse_colmax = os.environ.get("OPP_B200_COLMAX", "1") == "1"

@@ -740,3 +740,69 @@ def backbone_up2x_bwd(dout, din, accumulate):
     if tuple(dout.shape) != (B, C, 2 * h, 2 * w):
         raise ValueError(f"dout {tuple(dout.shape)} does not match 2x {tuple(din.shape)}")
     call("opp_backbone_train_up2x_bwd", ptr(dout), B, C, h, w, ptr(din), int(accumulate), stream())
+
+
+# ---- training, keypoint encoder (opp_train_kpt.cu; used by train_kpt.py) --------------------------
+# Rows are the flat (b, n) index of keypoints3d [B, N, 3]; stats [B, 4] from kpt_stats.
+
+
+def kpt_train_group():
+    """Rows per weight-gradient partial of kpt_train_bwd (a slice starts at a multiple)."""
+    return _lib.load().opp_kpt_train_group()
+
+
+def kpt_train_params():
+    """Floats of the flat parameter gradient: dW1 db1 dW2 db2 dW3 db3 dW4 db4."""
+    return _lib.load().opp_kpt_train_params()
+
+
+def kpt_train_pack_size():
+    """Floats of the weight pack kpt_train_fwd / kpt_train_bwd read."""
+    return _lib.load().opp_kpt_train_pack_size()
+
+
+def kpt_stats(kpts, stats):
+    """stats [B, 4] = (mean xyz of each batch element, 0.6 x the largest extent of element 0)."""
+    _chk(kpts, torch.float32, "keypoints3d")
+    _chk(stats, torch.float32, "stats")
+    B, N, _ = kpts.shape
+    if tuple(stats.shape) != (B, 4):
+        raise ValueError(f"stats has shape {tuple(stats.shape)}, expected {(B, 4)}")
+    call("opp_kpt_stats", ptr(kpts), ptr(stats), B, N, stream())
+
+
+def _kpt_args(kpts, stats, pack):
+    _chk(kpts, torch.float32, "keypoints3d")
+    _chk(stats, torch.float32, "stats")
+    _chk(pack, torch.float32, "pack")
+    B, N, three = kpts.shape
+    if three != 3 or tuple(stats.shape) != (B, 4):
+        raise ValueError(f"keypoints3d {tuple(kpts.shape)} / stats {tuple(stats.shape)}")
+    if pack.numel() != kpt_train_pack_size():
+        raise ValueError(f"pack has {pack.numel()} floats, expected {kpt_train_pack_size()}")
+    return B, N
+
+
+def kpt_train_fwd(kpts, stats, desc, pack, out):
+    """out [B * N, 256] = desc^T + the encoder MLP of the normalised keypoints; desc [B, 256, N]."""
+    B, N = _kpt_args(kpts, stats, pack)
+    _chk(desc, torch.float32, "descriptors")
+    _chk(out, torch.float32, "out")
+    if tuple(desc.shape) != (B, 256, N) or out.numel() != B * N * 256:
+        raise ValueError(f"descriptors {tuple(desc.shape)} / out {tuple(out.shape)} for {B} x {N} keypoints")
+    call("opp_kpt_train_fwd", ptr(kpts), ptr(stats), ptr(desc), ptr(pack), ptr(out), B, N, stream())
+
+
+def kpt_train_bwd(kpts, stats, dout, pack, row0, nrows, part, dparams, accumulate):
+    """dparams [kpt_train_params()] (+)= the parameter gradient for dout [B * N, 256] over the rows
+    [row0, row0 + nrows); part fp32 with at least ceil(nrows / group) * kpt_train_params() entries."""
+    B, N = _kpt_args(kpts, stats, pack)
+    _chk(dout, torch.float32, "dout")
+    _chk(part, torch.float32, "part")
+    _chk(dparams, torch.float32, "dparams")
+    if dout.numel() != B * N * 256 or dparams.numel() != kpt_train_params():
+        raise ValueError(f"dout {tuple(dout.shape)} / dparams {tuple(dparams.shape)}")
+    if part.numel() < -(-nrows // kpt_train_group()) * kpt_train_params():
+        raise ValueError("wgrad partial buffer too small")
+    call("opp_kpt_train_bwd", ptr(kpts), ptr(stats), ptr(dout), ptr(pack), B, N, int(row0), int(nrows), ptr(part),
+         ptr(dparams), int(accumulate), stream())

@@ -19,15 +19,17 @@ tensors the fine level (fine_preprocess -> loftr_fine -> fine_matching) runs on 
 opp_fine_train_* kernels instead (train_fine.py), and with model.coarse_transformer_train_mode ==
 "kernels" the coarse transformer runs on the opp_coarse_tf_* kernels (train_coarse_tf.py).  With
 model.backbone_train_mode == "kernels" the ResNet-FPN backbone runs on the opp_backbone_train_*
-kernels, BatchNorm following each module's .training (train_backbone.py).  The ground truth the padding draws from is
-data["conf_matrix_gt"] or, in its place, the correspondence list data["gt_sparse"] (train_gt.py).
+kernels, BatchNorm following each module's .training (train_backbone.py), and with
+model.kpt_encoder_train_mode == "kernels" the keypoint-encoder MLP runs on the opp_kpt_train_* kernels
+(train_kpt.py).  The ground truth the padding draws from is data["conf_matrix_gt"] or, in its place, the
+correspondence list data["gt_sparse"] (train_gt.py).
 
 Every function cites the reference lines it follows.
 """
 import torch
 import torch.nn.functional as F
 
-from . import train_backbone, train_coarse_tf, train_fine, train_gt
+from . import train_backbone, train_coarse_tf, train_fine, train_gt, train_kpt
 
 
 def _block(blk, x):
@@ -324,6 +326,7 @@ def forward_train(model, data):
     fine_kernels = train_fine.use_kernels(model, data)
     coarse_tf_kernels = train_coarse_tf.use_kernels(model, data)
     backbone_kernels = train_backbone.use_kernels(model, data)
+    kpt_kernels = train_kpt.use_kernels(model, data)
     data.update({"bs": img.size(0), "q_hw_i": img.shape[2:]})
     if backbone_kernels:
         feat_c, feat_f = train_backbone.backbone(model.backbone, img)
@@ -334,7 +337,10 @@ def forward_train(model, data):
         feat_c = feat_c + model.dense_pos_encoding.pe[:, :, :feat_c.size(2), :feat_c.size(3)]
     q_c = feat_c.flatten(2).transpose(1, 2)                        # 'n c h w -> n (h w) c'
     dsel = data["descriptors3d_coarse_db"] if "descriptors3d_coarse_db" in data else data["descriptors3d_db"]
-    d3 = keypoint_encoding(model.kpt_3d_pos_encoding, normalize_3d_keypoints(data["keypoints3d"]), dsel)
+    if kpt_kernels:
+        d3 = train_kpt.keypoint_encoding(model.kpt_3d_pos_encoding, data["keypoints3d"], dsel)
+    else:
+        d3 = keypoint_encoding(model.kpt_3d_pos_encoding, normalize_3d_keypoints(data["keypoints3d"]), dsel)
     qmask = data["query_image_mask"].flatten(-2) if "query_image_mask" in data else None
     if coarse_tf_kernels:
         d3, q_c = train_coarse_tf.coarse_transformer(model.loftr_coarse, d3, q_c, qmask)
