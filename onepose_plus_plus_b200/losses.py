@@ -69,20 +69,31 @@ class _CoarseFocalSparse(torch.autograd.Function):
         return da, db, None, None, None, None, None, None
 
 
+def _check_query_mask(handle):
+    if handle.col_mask is not None and not bool(handle.col_mask.any(1).all()):
+        raise ValueError("query_image_mask keeps no column of at least one sample: the coarse loss is not "
+                         "defined for a fully padded query image")
+
+
 def coarse_focal_loss(handle, conf_gt, alpha, gamma, pos_w, neg_w):
     """Focal loss of the dual-softmax confidence of `handle` against conf_gt (bool, uint8 or int16
     [B, L, S] on the device, or a SparseGT on the device: every listed element is a positive, every
     other one a negative), differentiable with respect to handle.feat3d / handle.feat2d.
-    Returns (loss, counts): counts = int64 [2] (positives, negatives) on the device."""
+    Returns (loss, counts): counts = int64 [2] (positives, negatives) on the device.
+    A query mask that keeps no column of some sample raises ValueError (one synchronisation): the
+    softmax over S of that sample has no terms, and the reference's -1e9 masking gives it a value
+    (the unmasked softmax in fp64, a uniform one in fp32) that the kernels do not reproduce."""
     if isinstance(conf_gt, SparseGT):
         if tuple(conf_gt.shape) != tuple(handle.shape):
             raise ValueError(f"gt_sparse has shape {tuple(conf_gt.shape)}, the confidence {tuple(handle.shape)}")
+        _check_query_mask(handle)
         return _CoarseFocalSparse.apply(handle.feat3d, handle.feat2d, handle, conf_gt, float(alpha), float(gamma),
                                         float(pos_w), float(neg_w))
     if conf_gt.dtype not in (torch.bool, torch.uint8, torch.int16):
         raise TypeError(f"conf_matrix_gt: expected bool, uint8 or int16, got {conf_gt.dtype}")
     if tuple(conf_gt.shape) != tuple(handle.shape):
         raise ValueError(f"conf_matrix_gt has shape {tuple(conf_gt.shape)}, the confidence {tuple(handle.shape)}")
+    _check_query_mask(handle)
     return _CoarseFocal.apply(handle.feat3d, handle.feat2d, handle, conf_gt, float(alpha), float(gamma),
                               float(pos_w), float(neg_w))
 

@@ -39,8 +39,18 @@ def dual_softmax(a, b, scale, mask=None):
     return p, q, p * q
 
 
-def focal_loss_and_grads(a, b, gt, scale, mask=None, alpha=0.5, gamma=2.0, pos_w=1.0, neg_w=1.0):
-    """fp64 loss, dA, dB (torch tensors on the device of a)."""
+def softmax_stats(a, b, scale, mask=None):
+    """fp64 softmax statistics of sim = scale A B^T: (row max, row log-sum-exp) over the kept columns
+    of each row and (column max, column log-sum-exp) over every row of each column."""
+    sim = scale * torch.einsum("blk,bsk->bls", a.double(), b.double())
+    col_max, col_lse = sim.amax(1), torch.logsumexp(sim, 1)
+    if mask is not None:
+        sim = sim.masked_fill(~mask.bool()[:, None, :], float("-inf"))
+    return sim.amax(2), torch.logsumexp(sim, 2), col_max, col_lse
+
+
+def focal_loss_and_grads(a, b, gt, scale, mask=None, alpha=0.5, gamma=2.0, pos_w=1.0, neg_w=1.0, with_rc=False):
+    """fp64 loss, dA, dB (torch tensors on the device of a); with_rc also R [B, L] and C [B, S]."""
     a, b = a.double(), b.double()
     p, q, c = dual_softmax(a, b, scale, mask)
     ct = c.clamp(LO, HI)
@@ -64,7 +74,10 @@ def focal_loss_and_grads(a, b, gt, scale, mask=None, alpha=0.5, gamma=2.0, pos_w
     dsim = 2 * gc - p * gc.sum(1, keepdim=True) - q * gc.sum(2, keepdim=True)
     da = scale * torch.einsum("bls,bsk->blk", dsim, b)
     db = scale * torch.einsum("bls,blk->bsk", dsim, a)
-    return torch.as_tensor(loss, dtype=torch.float64), da, db
+    loss = torch.as_tensor(loss, dtype=torch.float64)
+    if with_rc:
+        return loss, da, db, gc.sum(2), gc.sum(1)
+    return loss, da, db
 
 
 def make_case(name, batch=2, rows=40, cols=48, k=256, seed=0):
@@ -110,9 +123,10 @@ GOLDEN_CASES = {"planted_300x192": ("planted", 2, 300, 192), "masked_300x192": (
                 "planted_130x150": ("planted", 2, 130, 150), "clamp_300x192": ("clamp", 2, 300, 192)}
 
 
-def reference_loss_and_grads(a, b, gt, scale, mask=None):
+def reference_loss_and_grads(a, b, gt, scale, mask=None, config=None):
     """Autograd through the UNMODIFIED reference Loss.compute_coarse_loss (imported from the
-    reference tree through oracle/ref_shims.py) on the fp64 dual softmax of a, b."""
+    reference tree through oracle/ref_shims.py) on the fp64 dual softmax of a, b; config: the loss
+    section (LOSS_CONFIG by default)."""
     from . import ref_shims
     ref_shims.install()
     from src.lightning_model.losses import Loss as RefLoss   # type: ignore
@@ -124,7 +138,7 @@ def reference_loss_and_grads(a, b, gt, scale, mask=None):
         neg[~mask.bool()[:, None].expand_as(sim)] = -1e9
         sim = sim + neg
     conf = torch.softmax(sim, 1) * torch.softmax(sim, 2)
-    loss = RefLoss(LOSS_CONFIG).compute_coarse_loss(conf, gt)
+    loss = RefLoss(LOSS_CONFIG if config is None else config).compute_coarse_loss(conf, gt)
     loss.backward()
     return loss.detach(), a.grad, b.grad
 

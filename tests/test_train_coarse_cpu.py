@@ -8,7 +8,7 @@ import torch
 
 from oracle import coarse_loss as cl
 from oracle import ref_shims
-from onepose_plus_plus_b200 import losses
+from onepose_plus_plus_b200 import SparseGT, losses
 
 needs_ref = pytest.mark.skipif(not ref_shims.available(), reason="needs the reference tree")
 
@@ -22,13 +22,18 @@ def test_oracle_gradient_matches_reference_autograd(name, gt_dtype):
         pytest.skip("bool cannot hold a value that is neither class")
     gt = gt.to(gt_dtype)
     s = cl.scale_of()
-    ref_loss, ref_da, ref_db = cl.reference_loss_and_grads(a, b, gt, s, mask)
-    loss, da, db = cl.focal_loss_and_grads(a, b, gt, s, mask)
-    assert torch.isfinite(loss)
-    assert abs(loss.item() - ref_loss.item()) <= 1e-12 * abs(ref_loss.item())
-    for got, ref in ((da, ref_da), (db, ref_db)):
-        assert ref.abs().max() > 0
-        assert torch.allclose(got, ref, rtol=1e-9, atol=1e-12 * float(ref.abs().max()))
+    # the reference's settings, then LoFTR's alpha with a non-integer gamma and unequal class weights:
+    # at alpha = 0.5 and pos_w = neg_w the two classes' factors cannot be told apart
+    for focal in ((0.5, 2.0, 1.0, 1.0), (0.25, 2.5, 2.0, 0.5)):
+        config = dict(cl.LOSS_CONFIG, focal_alpha=focal[0], focal_gamma=focal[1], pos_weight=focal[2],
+                      neg_weight=focal[3])
+        ref_loss, ref_da, ref_db = cl.reference_loss_and_grads(a, b, gt, s, mask, config)
+        loss, da, db = cl.focal_loss_and_grads(a, b, gt, s, mask, *focal)
+        assert torch.isfinite(loss)
+        assert abs(loss.item() - ref_loss.item()) <= 1e-12 * abs(ref_loss.item()), focal
+        for got, ref in ((da, ref_da), (db, ref_db)):
+            assert ref.abs().max() > 0
+            assert torch.allclose(got, ref, rtol=1e-9, atol=1e-12 * float(ref.abs().max())), focal
 
 
 def test_cases_cover_their_corners():
@@ -93,6 +98,21 @@ def test_gt_dtype_is_checked_on_the_host():
             self.shape = torch.Size((1, 2, 3))
     with pytest.raises(TypeError, match="bool, uint8 or int16"):
         losses.coarse_focal_loss(_H(), torch.zeros(1, 2, 3, dtype=torch.float32), 0.5, 2.0, 1.0, 1.0)
+
+
+def test_fully_masked_sample_is_rejected():
+    """A query mask that keeps no column of a sample leaves its softmax over S without terms: the
+    eager path (sim - 1e9 on every column) gives the unmasked or a uniform softmax there, the kernels
+    would give c = 0.  coarse_focal_loss refuses such a mask before any launch."""
+    class _H(losses.TrainConfHandle):
+        def __init__(self, col_mask):
+            self.shape = torch.Size((2, 2, 3))
+            self.col_mask = col_mask
+    gt = torch.zeros(2, 2, 3, dtype=torch.int16)
+    mask = torch.tensor([[1, 0, 1], [0, 0, 0]], dtype=torch.uint8)
+    for g in (gt, SparseGT(*(torch.zeros(0, dtype=torch.int64),) * 3, torch.zeros(0, 2), (2, 2, 3))):
+        with pytest.raises(ValueError, match="keeps no column"):
+            losses.coarse_focal_loss(_H(mask), g, 0.5, 2.0, 1.0, 1.0)
 
 
 def test_skip_mode_cannot_train():

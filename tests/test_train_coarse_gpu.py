@@ -58,15 +58,29 @@ def test_kernels_match_oracle_and_reference(key):
     assert torch.equal(loss, loss2) and torch.equal(da, da2) and torch.equal(db, db2)
 
 
-@pytest.mark.parametrize("name", ["random", "no_pos", "no_neg"])
+def _odd_values(gt):
+    """The "neither" entries (2) of gt as other values that are neither class: int16 -1, 2, 255, 256
+    and 257 (256 and 257 have the low bytes 0 and 1 of a negative and a positive), uint8 2 and 255."""
+    other = gt == 2
+    k = torch.arange(int(other.sum()))
+    i16 = gt.masked_scatter(other, torch.tensor([-1, 2, 255, 256, 257], dtype=torch.int16)[k % 5])
+    u8 = gt.to(torch.uint8).masked_scatter(other, torch.tensor([2, 255], dtype=torch.uint8)[k % 2])
+    assert int((i16 == 256).sum()) > 0 and int((i16 == 257).sum()) > 0
+    return [u8, i16]
+
+
+@pytest.mark.parametrize("name", ["random", "no_pos", "no_neg", "odd_values"])
 def test_kernels_gt_dtypes_and_empty_classes(name):
-    a, b, gt, mask = cl.make_case(name, 2, 70, 90)
+    a, b, gt, mask = cl.make_case("random" if name == "odd_values" else name, 2, 70, 90)
     outs = []
     dtypes = [torch.uint8, torch.int16] + ([torch.bool] if name == "no_pos" else [])
-    for dt in dtypes:
-        outs.append(_fused(a, b, gt.to(dt), mask))
+    gts = _odd_values(gt) if name == "odd_values" else [gt.to(dt) for dt in dtypes]
+    for g in gts:
+        outs.append(_fused(a, b, g, mask))
     for o in outs[1:]:
         assert all(torch.equal(x, y) for x, y in zip(o[:3], outs[0][:3]))
+    for g, o in zip(gts, outs):
+        assert o[3].tolist() == [int((g == 1).sum()), int((g == 0).sum())]
     loss, da, db, _ = outs[0]
     r_loss, r_da, r_db = cl.focal_loss_and_grads(a.cuda(), b.cuda(), gt.cuda(), cl.scale_of())
     assert abs(loss.item() - r_loss.item()) <= RTOL * abs(r_loss.item())

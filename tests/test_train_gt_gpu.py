@@ -56,10 +56,18 @@ def index_by_torch(gt):
     return row_ptr, col_ptr, gt.i_ids[order].to(i32)
 
 
-@pytest.mark.parametrize("case", ["planted", "one_sample_empty", "many_to_many", "empty"])
+# B S + 1 column pointers: 1025, 2049 and 16385 (B = 4, S = 4096, the training shape) take the
+# one-CTA scan through 2, 3 and 17 rounds of 1024; "crowded_column" puts 899 entries in one column
+SCANS = {"scan_1025": (4, 50, 256, 0.05), "scan_2049": (8, 40, 256, 0.05), "scan_16385": (4, 30, 4096, 0.01),
+         "crowded_column": (2, 900, 70, 0.02)}
+
+
+@pytest.mark.parametrize("case", ["planted", "one_sample_empty", "many_to_many", "empty"] + list(SCANS))
 def test_gt_index(case):
     if case == "many_to_many":
         gt = list_of(many_to_many(3, 130, 150, 0.05, 0))
+    elif case in SCANS:
+        gt = list_of(many_to_many(*SCANS[case], 5))
     else:
         conf = mrg.train_batch(workload.synthetic_state_dict(0), False)["conf_matrix_gt"].clone()
         if case == "one_sample_empty":
@@ -73,6 +81,10 @@ def test_gt_index(case):
     for name, g, a, w in zip(("row_ptr", "col_ptr", "col_rows"), got, again, index_by_torch(gt)):
         assert g.dtype == torch.int32 and torch.equal(g, w), name
         assert torch.equal(g, a), name
+    if case == "crowded_column":
+        assert int(got[1].diff().max()) > 800
+    elif case in SCANS:
+        assert got[1].numel() == int(case[5:])
 
 
 def _dense_and_sparse(a, b, conf_gt, mask, grad=0.7):
