@@ -660,6 +660,17 @@ int opp_backbone_train_conv_dgrad(const float* dy, const float* w, int batches, 
 int opp_backbone_train_conv_wgrad(const float* x, const float* dy, int batches, int c_in, int h, int wd, int c_out,
                                   int ksize, int stride, int pix0, int npix, float* part, float* dw, int accumulate,
                                   opp_stream_t stream);
+/* The same three passes on the tensor cores in 3xTF32 (opp_train_backbone_tc.cu): each operand is split
+ * into tf32 hi + lo and every k8 step sums lo·hi, hi·lo and hi·hi in fp32.  Arguments as above; the
+ * weight gradient uses the same group (opp_backbone_train_wgrad_group) and partial buffer. */
+int opp_backbone_train_conv_tf32x3(const float* x, const float* w, int batches, int c_in, int h, int wd, int c_out,
+                                   int ksize, int stride, float* y, opp_stream_t stream);
+int opp_backbone_train_conv_dgrad_tf32x3(const float* dy, const float* w, int batches, int c_in, int h, int wd,
+                                         int c_out, int ksize, int stride, float* dx, int accumulate,
+                                         opp_stream_t stream);
+int opp_backbone_train_conv_wgrad_tf32x3(const float* x, const float* dy, int batches, int c_in, int h, int wd,
+                                         int c_out, int ksize, int stride, int pix0, int npix, float* part,
+                                         float* dw, int accumulate, opp_stream_t stream);
 /* mean / invstd [c] of x [batches][c][hw] over batches * hw values (biased variance); when
  * running_mean / running_var are given they are updated as F.batch_norm does (unbiased variance).
  * part fp64 [c][parts][2]. */
