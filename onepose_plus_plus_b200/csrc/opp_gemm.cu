@@ -153,18 +153,12 @@ static int launch(const TensorMaps& maps, GemmShape s, const typename Epi::Param
   }
   const int smem = gemm_smem_bytes<Epi>(s);
   log_tile_once(A_MODE, s, Epi::kName);
-  // 32-wide ring slots are compiled for the conv modes only
-  OPP_REQUIRE(s.bk == kBlockK || (s.bk == 32 && A_MODE != A_ROWS), "ring slot width %d not compiled for mode %d",
-              s.bk, A_MODE);
+  OPP_REQUIRE(s.bk == kBlockK || s.bk == 32, "ring slot width %d not compiled", s.bk);
   const void* kern;
-  if constexpr (DYN) kern = (const void*)gemm_kernel_dyn<A_MODE, Epi>;
-  else kern = (const void*)gemm_kernel<A_MODE, Epi>;
-  if constexpr (A_MODE != A_ROWS) {
-    if (s.bk == 32) {
-      if constexpr (DYN) kern = (const void*)gemm_kernel_dyn<A_MODE, Epi, 32>;
-      else kern = (const void*)gemm_kernel<A_MODE, Epi, 32>;
-    }
-  }
+  if constexpr (DYN)
+    kern = s.bk == 32 ? (const void*)gemm_kernel_dyn<A_MODE, Epi, 32> : (const void*)gemm_kernel_dyn<A_MODE, Epi>;
+  else
+    kern = s.bk == 32 ? (const void*)gemm_kernel<A_MODE, Epi, 32> : (const void*)gemm_kernel<A_MODE, Epi>;
   // function attributes are per device: set once per (kernel, device)
   static unsigned long long attr_done[2] = {0, 0};
   unsigned long long& done = attr_done[s.bk == 32];
@@ -255,6 +249,25 @@ static int pick_block_n(int n) {
   return 256;
 }
 
+// Ring slot width of a token-row GEMM (A_ROWS): 32 columns when the layer's full-width tile is above
+// 128 columns (the coarse transformer's N = 256 / 512 projections and the dual-softmax passes over
+// S >= 256 columns), else 64.  A 64-wide fp16x3 stage at N = 256 is 96 KB and only two fit beside the
+// epilogue scratch, so, as in conv_chunk_k, one slot per stage leaves no load in flight while the MMAs
+// hold both stages.  The rule reads the layer (N, K) only - never the batch, rows, tile width,
+// cluster or N split - so that the batch-1 launches (N split, LayerNorm pair cluster, the dynamic-row
+// kernels) sum the split products in the same order as the batch-64 ones and give the same bits.
+// $OPP_ROWS_BK=32|64 forces one width for every token-row GEMM.
+static int rows_chunk_k(int n, int k) {
+  static int forced = -1;
+  if (forced < 0) {
+    const char* e = getenv("OPP_ROWS_BK");
+    forced = e ? atoi(e) : 0;
+  }
+  if (forced == 32 || forced == 64) return forced;
+  (void)k;
+  return pick_block_n(n) > 128 ? 32 : 64;
+}
+
 // Latency shapes (batch 1-2: a GEMM has fewer super tiles than half the SMs, e.g. 16 clusters
 // for 4096 tokens): halve the N tile, down to 64 columns, so that 2-4x as many SMs share the MMAs
 // and the epilogue of the same output.  A is re-read once per N tile — a few hundred KB from L2.
@@ -330,7 +343,7 @@ static int setup_rows(TensorMaps& maps, GemmShape& s, const void* a0, int k0, co
   OPP_REQUIRE(s.block_n % 16 == 0 && s.block_n <= 256, "bad block_n %d", s.block_n);
   s.n_tiles = (n + s.block_n - 1) / s.block_n;
   s.n_total = n;
-  s.bk = kBlockK;
+  s.bk = rows_chunk_k(n, k0 + k1);
   s.k_chunks_a0 = k0 / 64;
   s.k_chunks = (k0 + k1) / 64;
   s.b_batched = w_batched;
@@ -340,11 +353,11 @@ static int setup_rows(TensorMaps& maps, GemmShape& s, const void* a0, int k0, co
   s.b_lo = k0 + k1;
   s.a0_shared = a0_shared ? 1 : 0;
   const long long ld0 = (long long)planes * k0, ld1 = (long long)planes * k1;
-  int rc = map_rows(&maps.a[0], a0, ld0, rows, a0_shared ? 1 : batches, ld0, rows * ld0, kBlockM);
+  int rc = map_rows(&maps.a[0], a0, ld0, rows, a0_shared ? 1 : batches, ld0, rows * ld0, kBlockM, s.bk);
   if (rc) return rc;
   if (k1 > 0) {
     OPP_REQUIRE(a1, "null second A operand");
-    rc = map_rows(&maps.a[1], a1, ld1, rows, batches, ld1, rows * ld1, kBlockM);
+    rc = map_rows(&maps.a[1], a1, ld1, rows, batches, ld1, rows * ld1, kBlockM, s.bk);
     if (rc) return rc;
   } else {
     maps.a[1] = maps.a[0];
@@ -358,7 +371,7 @@ static int setup_rows(TensorMaps& maps, GemmShape& s, const void* a0, int k0, co
   if (rc) return rc;
   const long long kt = (long long)planes * (k0 + k1);
   return map_rows(&maps.b, w, kt, n, w_batched ? batches : 1, kt, (long long)n * kt,
-                  s.pair == 2 ? s.mma_n : s.mma_n / s.cluster);
+                  s.pair == 2 ? s.mma_n : s.mma_n / s.cluster, s.bk);
 }
 
 }  // namespace opp

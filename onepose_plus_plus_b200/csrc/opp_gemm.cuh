@@ -87,8 +87,8 @@ struct GemmShape {
   int block_n;      // output columns per tile (multiple of 16, <= 256)
   int mma_n;        // mma_width_for(block_n): W rows staged per tile and accumulator width
   int k_chunks;     // number of 64-wide K chunks per tile (per plane)
-  int bk;           // K columns per ring slot: 64, or 32 (two slots per stage; conv modes only; a
-                    // compile-time parameter of the kernel)
+  int bk;           // K columns per ring slot: 64, or 32 (two slots per stage; conv_chunk_k and
+                    // rows_chunk_k pick it per layer; a compile-time parameter of the kernel)
   int stages;       // ring stages of one K chunk each
   int b_batched;    // W operand has a leading batch dim
   int cluster;      // CTAs per cluster (1, 2, 4): they work on adjacent M tiles of the same

@@ -1,15 +1,21 @@
 """Per-launch attribution of the token-row GEMMs (A_ROWS) of one forward at the bench shapes.
 
-    python scripts/rows_probe.py [--batch 64] [--reps 20] [--out FILE.json]
+    python scripts/rows_probe.py [--batch 64] [--reps 20] [--skip 4,5,6] [--rows-bk 64,32] [--rounds 1]
+                                 [--out FILE.json]
 
 Records every distinct token-row GEMM launch of one forward over a batch of 512x512 planted images
 (conv1, the five GEMM kinds of every coarse encoder layer on the 2D and the 3D side, the two
 dual-softmax passes), adds the fine-stage GEMMs at the forward's match count (26 rows per match,
 plain and with the row count read on the device), then times each one alone with CUDA events,
-twice, each in a child process of its own (the engine reads its environment once per process):
+in child processes of their own (the engine reads its environment once per process):
   * as built;
   * with OPP_DEBUG_SKIP=4, the epilogue switched off (MMAs and loads unchanged): the difference is
-    the most that hiding the epilogue behind the MMAs can give.
+    the most that hiding the epilogue behind the MMAs can give;
+  * with each further OPP_DEBUG_SKIP value of --skip: 5 = no epilogue and no W loads, 6 = no
+    epilogue and no A loads (the MMAs read whatever the ring holds).  A launch that gets no faster
+    without its loads is not bound by them.
+--rows-bk 64,32 repeats all of it once per token-row ring slot width ($OPP_ROWS_BK), the widths
+alternated --rounds times (each launch keeps the median of its rounds), for an A/B in one build.
 Per launch: time, issued TFLOP/s (what the tensor pipe executes: three fp16 passes over the padded
 tile widths), the epilogue share, and the engine's OPP_LOG_TILES line (ring depth, accumulator
 alias, cluster, N-split pair).  The card name, power limit and median SM clock are read in the same
@@ -18,6 +24,7 @@ import argparse
 import json
 import math
 import os
+import statistics
 import subprocess
 import sys
 import tempfile
@@ -234,27 +241,14 @@ def launch_key(L):
     return (L["what"], L["name"], L["batches"], L["rows"], L["n"], L["k"])
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--batch", type=int, default=64)
-    ap.add_argument("--reps", type=int, default=20)
-    ap.add_argument("--out")
-    ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
-    ap.add_argument("--tmp", help=argparse.SUPPRESS)
-    args = ap.parse_args()
-    if args.child:
-        return child(args)
-    import torch
-    if not torch.cuda.is_available():
-        raise SystemExit("rows_probe needs a CUDA device")
-    with tempfile.TemporaryDirectory() as tmp:
-        full = run_child(args, tmp, {})
-        noepi = run_child(args, tmp, {"OPP_DEBUG_SKIP": "4"})
-    skip_ms = {launch_key(S): S["ms"] for S in noepi["launches"]}
+def table(full, arms):
+    """per-launch rows of the as-built child `full`, with the time of each OPP_DEBUG_SKIP arm"""
+    skip_ms = {v: {launch_key(S): S["ms"] for S in a["launches"]} for v, a in arms.items()}
     rows = []
     for L in full["launches"]:
         r = {k: L[k] for k in ("what", "name", "epilogue", "batches", "rows", "n", "k", "ms", "tile")}
-        off = skip_ms.get(launch_key(L))
+        r["ms_skip"] = {v: m.get(launch_key(L)) for v, m in skip_ms.items()}
+        off = r["ms_skip"].get("4")
         r["ms_epilogue_off"] = off
         r["epilogue_share"] = None if off is None else 1.0 - off / L["ms"]
         if L["tile"]:
@@ -265,18 +259,61 @@ def main():
             r["issued_tflop"] = issued / 1e12
             r["issued_tflops"] = issued / (L["ms"] * 1e-3) / 1e12
         rows.append(r)
+    return rows
+
+
+def median_of(runs):
+    """one child result whose launch times are the medians over `runs` (same launches, same order)"""
+    out = dict(runs[0])
+    out["launches"] = [dict(L, ms=statistics.median(R["launches"][i]["ms"] for R in runs))
+                       for i, L in enumerate(runs[0]["launches"])]
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=64)
+    ap.add_argument("--reps", type=int, default=20)
+    ap.add_argument("--skip", default="4", help="comma-separated OPP_DEBUG_SKIP arms (4 = no epilogue, "
+                                                 "5 = + no W loads, 6 = + no A loads)")
+    ap.add_argument("--rows-bk", default="", help="comma-separated OPP_ROWS_BK arms (default: as built)")
+    ap.add_argument("--rounds", type=int, default=1, help="alternations of the --rows-bk arms")
+    ap.add_argument("--out")
+    ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
+    ap.add_argument("--tmp", help=argparse.SUPPRESS)
+    args = ap.parse_args()
+    if args.child:
+        return child(args)
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("rows_probe needs a CUDA device")
+    skips = [v for v in args.skip.split(",") if v]
+    bks = [v for v in args.rows_bk.split(",") if v] or [None]
+    fulls = {bk: [] for bk in bks}
+    arms = {bk: {v: [] for v in skips} for bk in bks}
+    with tempfile.TemporaryDirectory() as tmp:
+        for _ in range(args.rounds):
+            for bk in bks:
+                env = {"OPP_ROWS_BK": bk} if bk else {}
+                fulls[bk].append(run_child(args, tmp, env))
+                for v in skips:
+                    arms[bk][v].append(run_child(args, tmp, env | {"OPP_DEBUG_SKIP": v}))
     doc = {"device": device_info() | {"sms": torch.cuda.get_device_properties(0).multi_processor_count},
-           "batch": args.batch, "reps": args.reps, "clocks": full["clocks"],
-           "clocks_epilogue_off": noepi["clocks"], "matches": full["matches"], "launches": rows,
+           "batch": args.batch, "reps": args.reps, "rounds": args.rounds, "skip_arms": skips,
            "note": "issued = (3 if split) fp16 MMA passes x 128 rows x mma_n columns x K per tile; rows of the "
-                   "dyn launches = the capacity = the count; ms_epilogue_off = the same launch with "
-                   "OPP_DEBUG_SKIP=4 (no epilogue) in another process"}
-    for r in rows:
-        off = r["ms_epilogue_off"]
-        sys.stderr.write(f"{r['what'][:40]:<40} {r['name'][4:]:<20} {r['ms']:8.3f} ms  no-epi "
-                         f"{off if off is not None else float('nan'):8.3f} ms "
-                         f"({100 * (r['epilogue_share'] or 0):5.1f} %)  {r.get('issued_tflops', 0):6.1f} TF issued  "
-                         f"{(r['tile'] or ['?'])[0]}\n")
+                   "dyn launches = the capacity = the count; ms_skip[v] = the same launch with OPP_DEBUG_SKIP=v "
+                   "in another process (4: no epilogue, 5: + no W loads, 6: + no A loads); ms = median over "
+                   "the rounds", "arms": {}}
+    for bk in bks:
+        full = median_of(fulls[bk])
+        rows = table(full, {v: median_of(a) for v, a in arms[bk].items()})
+        doc["arms"][bk or "as built"] = {"clocks": full["clocks"], "matches": full["matches"], "launches": rows}
+        sys.stderr.write(f"== OPP_ROWS_BK={bk or '(as built)'}\n")
+        for r in rows:
+            sk = "  ".join(f"skip{v} {r['ms_skip'][v] if r['ms_skip'][v] is not None else float('nan'):7.3f}"
+                           for v in skips)
+            sys.stderr.write(f"{r['what'][:34]:<34} {r['name'][4:]:<20} {r['ms']:7.3f} ms  {sk}  "
+                             f"{r.get('issued_tflops', 0):6.1f} TF  {(r['tile'] or ['?'])[0]}\n")
     s = json.dumps(doc)
     print(s)
     if args.out:
