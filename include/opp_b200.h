@@ -127,8 +127,7 @@ int opp_linear_act_f16_b(const void* a0, int k0, int a0_shared, const void* a1, 
                          int split, const unsigned char* row_mask, opp_stream_t stream);
 
 /* Same GEMM with split (hi|lo) operands but a single-plane fp16 output [rows][n]: for the K'/V rows
- * of the linear-attention state, whose consumer sums over thousands of rows (built for the next
- * GPU session; selected by $OPP_B200_KV1). */
+ * of the linear-attention state, whose consumer sums over thousands of rows. */
 int opp_linear_act_f16_out1(const void* a0, int k0, const void* a1, int k1, const void* w, void* out,
                             long long rows, int n, int act, int act_cols, const unsigned char* row_mask,
                             opp_stream_t stream);
@@ -169,7 +168,8 @@ int opp_full_attention(const void* q, const void* kv, void* out, int batch, int 
                        int head_dim, int split, opp_stream_t stream);
 
 /* Source side state of linear attention (linear_attention.py:55-57):
- * kv16 fp16 [B][S][planes*2d] holds K' = elu(k)+1 in columns [0,d) and V in [d,2d) of each plane.
+ * kv16 fp16 [B][S][2d] (one plane in both operand modes) holds K' = elu(k)+1 in columns [0,d) and
+ * V in [d,2d).
  * part fp32 [B][chunks][H][33][32], chunks = opp_kv_chunks_b(S, B): per-chunk sum_s K'^T V (rows
  * 0..31) and sum_s K' (row 32) for each of the H = d/32 heads.  opp_kv_partial picks the chunk length
  * from (S, B) — 256 tokens, 128 when that would leave fewer than 64 CTAs — and opp_kv_finalize must
@@ -177,8 +177,7 @@ int opp_full_attention(const void* q, const void* kv, void* out, int batch, int 
  * (what large batches use), kept for callers that size buffers once. */
 int opp_kv_chunks(int s);
 int opp_kv_chunks_b(int s, int batch);
-int opp_kv_partial(const void* kv16, float* part, int batch, int s, int d, int split,
-                   opp_stream_t stream);
+int opp_kv_partial(const void* kv16, float* part, int batch, int s, int d, opp_stream_t stream);
 
 /* Reduces the chunk partials, scales KV by 1/v_len and folds the merge projection
  * (transformer.py:85): mt[b][c][h*32+dd] = sum_v merge_w[c][h*32+v] * KV[b][h][dd][v] / v_len.
@@ -193,25 +192,16 @@ int opp_kv_finalize(const float* part, const float* merge_w, void* mt, float* ks
 
 int opp_sim_tiles(int cols); /* column tiles used by the two calls below */
 
-/* per-row partial (max, sum exp) of sim = scale * a @ b^T over each column tile.
- * a fp16 [B][rows][planes*k], b fp16 [B][cols][planes*k];
- * part_m/part_s fp32 [B*rows][opp_sim_tiles(cols)] */
-int opp_sim_lse(const void* a, const void* b, float* part_m, float* part_s, int batches, int rows,
-                int cols, int k, float scale, int split, opp_stream_t stream);
-
 /* lse[r] = logsumexp over tiles */
 int opp_lse_finalize(const float* part_m, const float* part_s, float* lse, long long rows,
                      int tiles, opp_stream_t stream);
 
-/* conf = exp((2 sim - lse_pt) - lse_px) (coarse_matching.py:115); per-row per-tile (max, first
- * argmax); conf (or NULL) fp32 [B*rows][cols] is data["conf_matrix"] when rows are 3D points. */
-int opp_sim_conf(const void* a, const void* b, const float* lse_own, const float* lse_other,
-                 int own_is_pt, float* conf, float* part_val, int* part_idx, int batches,
-                 int rows, int cols, int k, float scale, int split, opp_stream_t stream);
-
-/* opp_sim_lse for rows = 3D points that also produces the COLUMN statistics (saves the second lse
- * pass): col_m/col_s fp32 [B][ceil(rows/32)][cols] = per 32-row group (max, sum exp(x - max)) of
- * every column; opp_lse_col_finalize merges the groups into lse[b][s] = logsumexp_l sim[b, l, s].
+/* Dual-softmax statistics of sim = scale * a @ b^T in one GEMM pass, rows = 3D points.
+ * a fp16 [B][rows][planes*k], b fp16 [B][cols][planes*k].  Row side: part_m/part_s fp32
+ * [B*rows][opp_sim_tiles(cols)] = per-row partial (max, sum exp) over each column tile, merged by
+ * opp_lse_finalize.  Column side: col_m/col_s fp32 [B][ceil(rows/32)][cols] = per 32-row group
+ * (max, sum exp(x - max)) of every column; opp_lse_col_finalize merges the groups into
+ * lse[b][s] = logsumexp_l sim[b, l, s].
  * col_mask (uint8 [B][cols] or NULL) = query_image_mask at coarse resolution: masked columns get
  * sim - 1e9 (coarse_matching.py:108-114), i.e. they drop out of every row's softmax, and
  * opp_lse_col_finalize writes lse = +inf for them so that conf is exactly 0 there. */
@@ -221,9 +211,12 @@ int opp_sim_lse_cols(const void* a, const void* b, float* part_m, float* part_s,
 int opp_lse_col_finalize(const float* col_m, const float* col_s, float* lse, int batches, int groups,
                          int cols, const unsigned char* col_mask, opp_stream_t stream);
 
-/* opp_sim_conf for rows = 3D points with the column maxima folded in (saves the second conf pass):
- * colmax uint32 [B][cols] receives the float bits of max_l conf[b, l, s] (zeroed inside, then
- * atomicMax per 32-row group; conf >= 0 so the bits order like the values). */
+/* conf = exp((2 sim - lse_pt) - lse_px) (coarse_matching.py:115), rows = 3D points: per-row per-tile
+ * (max, first argmax) into part_val/part_idx [B*rows][opp_sim_tiles(cols)], merged by
+ * opp_best_finalize; conf (or NULL) fp32 [B*rows][cols] is data["conf_matrix"].  The column maxima
+ * are folded into the same pass: colmax uint32 [B][cols] receives the float bits of
+ * max_l conf[b, l, s] (zeroed inside, then atomicMax per 32-row group; conf >= 0 so the bits order
+ * like the values). */
 int opp_sim_conf_colmax(const void* a, const void* b, const float* lse_own, const float* lse_other,
                         float* conf, float* part_val, int* part_idx, unsigned* colmax, int batches,
                         int rows, int cols, int k, float scale, int split, opp_stream_t stream);
@@ -247,22 +240,16 @@ int opp_best_finalize(const float* part_val, const int* part_idx, float* best_va
                       long long rows, int tiles, opp_stream_t stream);
 
 /* Threshold + top/left border + mutual nearest neighbour + ordered compaction
- * (coarse_matching.py:142-172, 223-239).  Capacity of every output is batch*min(l, s).
- *   pt_val/pt_idx [B][l]: row maxima of conf;  px_idx [B][s]: column argmax of conf
+ * (coarse_matching.py:142-172, 223-239).  The mutual test is on values (coarse_matching.py:157-165
+ * compares conf == conf.max(dim) the same way): row l keeps its argmax cell j iff pt_val[b][l] has
+ * the same float bits as colmax[b][j] (from opp_sim_conf_colmax), so every row of an exact tie is
+ * kept and the capacity of every output is batch*l.
+ *   pt_val/pt_idx [B][l]: row maxima of conf;  colmax uint32 [B][s]: column maxima of conf
  *   kpts fp32 [B][l][3]; img_scale fp32 [B][2] = (h_scale, w_scale) or NULL
  *   scratch int32 [ceil(B*l/1024) + 2]
  *   bank_shared != 0: one object for the whole batch, kpts is [1][l][3] (no per-image copies)
  * Outputs (ascending (b, i) order): b_ids/i_ids/j_ids int64, mconf fp32, mkpts3d fp32 [.][3],
  * mkpts_c fp32 [.][2]; count_out int32 [1] = number of matches. */
-int opp_match_select(const float* pt_val, const int* pt_idx, const int* px_idx, const float* kpts,
-                     const float* img_scale, int batch, int l, int hc, int wc, float thr,
-                     int border, float cell, int* scratch, long long* b_ids, long long* i_ids,
-                     long long* j_ids, float* mconf, float* mkpts3d, float* mkpts_c,
-                     int* count_out, int bank_shared, opp_stream_t stream);
-
-/* opp_match_select with the mutual-nearest test on values (coarse_matching.py:157-165 compares
- * conf == conf.max(dim) the same way): row l keeps its argmax cell j iff pt_val[b][l] has the same
- * float bits as colmax[b][j] (from opp_sim_conf_colmax). */
 int opp_match_select_colmax(const float* pt_val, const int* pt_idx, const unsigned* colmax,
                             const float* kpts, const float* img_scale, int batch, int l, int hc,
                             int wc, float thr, int border, float cell, int* scratch,
@@ -287,7 +274,7 @@ int opp_match_select_colmax_set(const float* pt_val, const int* pt_idx, const un
 
 /* Every fine-level entry point takes `count_dev`: NULL = `m` is the exact number of matches (known
  * on the host); otherwise `m` is the CAPACITY the buffers were sized for and the kernels read the
- * real match count from *count_dev (int32, device; written by opp_match_select*), so the whole
+ * real match count from *count_dev (int32, device; written by the opp_match_select_* calls), so the whole
  * forward can be enqueued / captured in a CUDA graph without the host learning M first (the
  * reference synchronises in torch.where: coarse_matching.py:170). */
 

@@ -34,16 +34,13 @@ SIGNATURES = {
     "opp_linear_q_f16": [P, P, P, P, I, I, I, F, F, I, I, P, P],
     "opp_linear_ln": [P, I, P, I, P, I, P, P, F, P, I, P, P, I, L, I, I, P],
     "opp_full_attention": [P, P, P, I, I, I, I, I, I, P],
-    "opp_kv_partial": [P, P, I, I, I, I, P],
+    "opp_kv_partial": [P, P, I, I, I, P],
     "opp_kv_finalize": [P, P, P, P, I, I, I, F, I, P],
-    "opp_sim_lse": [P, P, P, P, I, I, I, I, F, I, P],
     "opp_lse_finalize": [P, P, P, L, I, P],
-    "opp_sim_conf": [P, P, P, P, I, P, P, P, I, I, I, I, F, I, P],
     "opp_sim_lse_cols": [P, P, P, P, P, P, I, I, I, I, F, I, P, P],
     "opp_lse_col_finalize": [P, P, P, I, I, I, P, P],
     "opp_sim_conf_colmax": [P, P, P, P, P, P, P, P, I, I, I, I, F, I, P],
     "opp_best_finalize": [P, P, P, P, L, I, P],
-    "opp_match_select": [P, P, P, P, P, I, I, I, I, F, I, F, P, P, P, P, P, P, P, P, I, P],
     "opp_match_select_colmax": [P, P, P, P, P, I, I, I, I, F, I, F, P, P, P, P, P, P, P, P, I, P],
     "opp_fine_gather": [P, P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, P, P],
     "opp_sim_lse_cols_rows": [P, P, P, P, P, P, I, I, I, I, F, I, P, P, P],
@@ -148,7 +145,7 @@ def stream():
 
 
 # kernels launched per entry point (bench.py reports the per-step total as gpu_launches)
-KERNELS_PER_CALL = {"opp_match_select": 3, "opp_match_select_colmax": 3, "opp_match_select_colmax_set": 3,
+KERNELS_PER_CALL = {"opp_match_select_colmax": 3, "opp_match_select_colmax_set": 3,
                     "opp_pose_metrics": 3,
                     "opp_coarse_focal_stats": 2, "opp_coarse_focal_fwd": 3, "opp_coarse_focal_bwd": 2,
                     "opp_gt_index": 5, "opp_coarse_focal_fwd_sparse": 3, "opp_coarse_focal_bwd_sparse": 2,

@@ -570,18 +570,10 @@ int opp_conv2d_nhwc(const void* in, const void* w, const float* bias, const void
   return launch<A_CONV, EpiConv>(maps, s, ep, (cudaStream_t)stream);
 }
 
-// Row pitch of the compact output windows of opp_conv_win(win).  7x7 windows: pitch 8 (two windows =
-// 112 accumulator rows, each a whole number of 1024-byte swizzle atoms in the A stage).  5x5 windows:
-// $OPP_WIN5_PACK=1 packs FIVE 5x5 boxes (125 rows, 25 x 128 B apart: 128-byte aligned only) instead
-// of three 5x8 ones (120 rows, 75 of them valid).
-int opp_conv_win_pitch(int win) {
-  static int pack5 = -1;
-  if (pack5 < 0) {
-    const char* e = getenv("OPP_WIN5_PACK");
-    pack5 = e ? atoi(e) : 0;
-  }
-  return (win == 5 && pack5) ? 5 : 8;
-}
+// Row pitch of the compact output windows of opp_conv_win: 8 for both window sides, so that a
+// window's box is a whole number of swizzle atoms in the A stage (7x8: two windows = 112 accumulator
+// rows; 5x8: three windows = 120 rows, 75 of them valid).
+int opp_conv_win_pitch(int) { return 8; }
 
 int opp_conv_win(const void* in, const void* w, const float* bias, void* out, const long long* b_ids,
                  const long long* j_ids, int matches, const int* count, int batch, int in_h, int in_w,
@@ -603,7 +595,7 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
   const int pitch = opp_conv_win_pitch(win);
   s.tile_w = pitch;
   s.tile_h = win;
-  s.tiles_x = 128 / (pitch * win);   // windows per M tile: 2 (7x8), 3 (5x8) or 5 (5x5)
+  s.tiles_x = 128 / (pitch * win);   // windows per M tile: 2 (7x8) or 3 (5x8)
   s.tiles_y = 1;
   s.rows = matches * pitch * win;
   s.m_tiles = (matches + s.tiles_x - 1) / s.tiles_x;
@@ -612,9 +604,6 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
   s.n_total = c_out_pad;
   s.conv_c = c_in_pad;
   s.bk = conv_chunk_k(3, c_out_pad);
-  // a window's box lands at a multiple of its size in the A stage: a whole number of swizzle atoms
-  // (8 rows of 2 bk bytes) for pitch 8, not for the five-5x5-boxes packing at bk = 32
-  OPP_REQUIRE(pitch == 8 || s.bk == 64, "OPP_WIN5_PACK needs 64-wide ring slots (layer has %d)", s.bk);
   s.conv_cchunks = (c_in_pad + 63) / 64;
   s.k_chunks = 9 * s.conv_cchunks;
   s.conv_kw = 3;
@@ -646,27 +635,6 @@ int opp_conv_win(const void* in, const void* w, const float* bias, void* out, co
                     b_ids, j_ids, wc, stride, org, in_h, in_w};
   if (count) return launch<A_WIN, EpiWin, true>(maps, s, ep, (cudaStream_t)stream, count, pitch * win);
   return launch<A_WIN, EpiWin>(maps, s, ep, (cudaStream_t)stream);
-}
-
-int opp_sim_lse(const void* a, const void* b, float* part_m, float* part_s, int batches, int rows,
-                int cols, int k, float scale, int split, opp_stream_t stream) {
-  TensorMaps maps;
-  GemmShape s;
-  int rc = setup_rows(maps, s, a, k, nullptr, 0, b, 1, batches, rows, cols, split, 1);
-  if (rc) return rc;
-  EpiLse::Params ep{part_m, part_s, scale};
-  return launch<A_ROWS, EpiLse>(maps, s, ep, (cudaStream_t)stream);
-}
-
-int opp_sim_conf(const void* a, const void* b, const float* lse_own, const float* lse_other,
-                 int own_is_pt, float* conf, float* part_val, int* part_idx, int batches,
-                 int rows, int cols, int k, float scale, int split, opp_stream_t stream) {
-  TensorMaps maps;
-  GemmShape s;
-  int rc = setup_rows(maps, s, a, k, nullptr, 0, b, 1, batches, rows, cols, split, 1);
-  if (rc) return rc;
-  EpiConf::Params ep{lse_own, lse_other, scale, own_is_pt, conf, part_val, part_idx};
-  return launch<A_ROWS, EpiConf>(maps, s, ep, (cudaStream_t)stream);
 }
 
 int opp_sim_lse_cols_rows(const void* a, const void* b, float* part_m, float* part_s, float* col_m,

@@ -1109,45 +1109,6 @@ struct EpiLN {
   }
 };
 
-// Dual-softmax statistics (coarse_matching.py:102-115): per row, over this tile's columns,
-// (max, sum exp) of sim = acc*scale.  Partials [grow][n_tile] are merged by a finalize kernel.
-struct EpiLse {
-  static constexpr int kGroups = 2;
-  static constexpr const char* kName = "lse";   // $OPP_LOG_TILES
-  static constexpr bool kFromRegs = true;
-  struct Params {
-    float* part_m;
-    float* part_s;
-    float scale;
-  };
-  __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  template <int N>
-  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
-    const int c0 = 2 * (threadIdx.x & 3);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float m = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < N / 8; ++i)
-#pragma unroll
-        for (int e = 0; e < 2; ++e)
-          if (8 * i + c0 + e < c.ncols) m = fmaxf(m, d[4 * i + 2 * h + e] * p.scale);
-      m = quad_max(m);
-      float sum = 0.f;
-#pragma unroll
-      for (int i = 0; i < N / 8; ++i)
-#pragma unroll
-        for (int e = 0; e < 2; ++e)
-          if (8 * i + c0 + e < c.ncols) sum += fast_exp(d[4 * i + 2 * h + e] * p.scale - m);
-      sum = quad_sum(sum);
-      if ((threadIdx.x & 3) == 0 && ((c.svalid >> h) & 1u)) {
-        p.part_m[c.sgrow[h] * s.n_tiles + c.n_tile] = m;
-        p.part_s[c.sgrow[h] * s.n_tiles + c.n_tile] = sum;
-      }
-    }
-  }
-};
-
 // fp32 conf_matrix store of one slice (row stride n_total): staged when rows are 16-byte aligned,
 // else element by element
 __device__ __forceinline__ void conf_store(const GemmShape& s, const EpiCtx& c, float* conf, int col,
@@ -1171,11 +1132,10 @@ __device__ __forceinline__ void conf_store(const GemmShape& s, const EpiCtx& c, 
 
 // conf = softmax_dim1(sim) * softmax_dim2(sim) = exp((2*sim - lse_pt) - lse_px) of one slice
 // (coarse_matching.py:115), and the running per-row (max, first argmax) over the tile's columns
-// (coarse_matching.py:157-165): a lane visits its columns in increasing order.  `own_is_pt` says
-// whether rows are 3D points (pass A) or query cells (pass B); the expression is evaluated in the
-// same order in both passes.
+// (coarse_matching.py:157-165): a lane visits its columns in increasing order.  Rows are 3D points
+// (lown = their lse_pt), columns query cells (lse_px staged in smem_s).
 __device__ __forceinline__ void conf_slice(const EpiCtx& c, int col, float scale, const float (&lown)[2],
-                                           bool own_is_pt, float (&v)[16], float (&best)[2], int (&bidx)[2]) {
+                                           float (&v)[16], float (&best)[2], int (&bidx)[2]) {
   const int c0 = 2 * (threadIdx.x & 3);
 #pragma unroll
   for (int ii = 0; ii < 4; ++ii)
@@ -1186,7 +1146,7 @@ __device__ __forceinline__ void conf_slice(const EpiCtx& c, int col, float scale
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const float x2 = 2.f * (v[4 * ii + 2 * h + e] * scale);
-        const float x = fast_exp(own_is_pt ? (x2 - lown[h]) - lo : (x2 - lo) - lown[h]);
+        const float x = fast_exp((x2 - lown[h]) - lo);
         v[4 * ii + 2 * h + e] = x;
         if (cl < c.ncols && x > best[h]) {
           best[h] = x;
@@ -1208,45 +1168,9 @@ __device__ __forceinline__ void conf_best_store(const GemmShape& s, const EpiCtx
   }
 }
 
-// conf per element, optional fp32 store of conf_matrix, and the per-row (max, first argmax) over
-// this tile's columns for the mutual-nearest test (the four-pass flow).
-struct EpiConf {
-  static constexpr int kGroups = 2;
-  static constexpr const char* kName = "conf";   // $OPP_LOG_TILES
-  static constexpr bool kFromRegs = true;
-  struct Params {
-    const float* lse_own;    // [batches*rows]
-    const float* lse_other;  // [batches][n_total]
-    float scale;
-    int own_is_pt;
-    float* conf;             // [batches*rows][n_total] or null
-    float* part_val;         // [batches*rows][n_tiles]
-    int* part_idx;
-  };
-  __device__ static void prefetch(const Params&, const GemmShape&, const EpiCtx&) {}
-  template <int N>
-  __device__ __forceinline__ static void run_frag(const Params& p, const GemmShape& s, const EpiCtx& c, float (&d)[N / 2]) {
-    epi_stage_cols_b(s, c, p.lse_other);
-    float lown[2], best[2] = {-1.f, -1.f};
-    int bidx[2] = {c.n0, c.n0};
-#pragma unroll
-    for (int h = 0; h < 2; ++h) lown[h] = ((c.svalid >> h) & 1u) ? p.lse_own[c.sgrow[h]] : 0.f;
-#pragma unroll
-    for (int j = 0; j < (N + 31) / 32; ++j) {
-      const int col = 32 * j;
-      if (col < c.ncols) {
-        float v[16];
-        frag_slice<N>(d, j, v);
-        conf_slice(c, col, p.scale, lown, p.own_is_pt != 0, v, best, bidx);
-        if (p.conf) conf_store(s, c, p.conf, col, v);
-      }
-    }
-    conf_best_store(s, c, p.part_val, p.part_idx, best, bidx);
-  }
-};
-
-// lse pass with the COLUMN statistics folded in (replaces the second lse pass): rows are 3D points.
-// Row partials as in EpiLse; in addition every warp reduces each column of a 32-column slice over
+// Dual-softmax statistics (coarse_matching.py:102-115) of sim = acc*scale in one pass: rows are 3D
+// points.  Per row, over this tile's columns, (max, sum exp) into part_m / part_s [grow][n_tile]
+// (merged by opp_lse_finalize); in addition every warp reduces each column of a 32-column slice over
 // its 16 rows (the column max with an xor butterfly, then the sum of exp(x - that max) with a halving
 // one, after which lane holds column frag_lane_col()), the two warps of a 32-row group merge their
 // (max, sum) through the odd warp's stage (even warp first), and the even warp writes the pair to
@@ -1390,8 +1314,9 @@ using EpiLseCol = EpiLseColT<false>;
 using EpiLseColMasked = EpiLseColT<true>;   // + query_image_mask (-1e9 on the padded query cells)
 using EpiLseColRows = EpiLseColT<false, true>;   // + per-batch row counts (bank sets)
 
-// conf pass with the column maxima folded in (replaces the second conf pass): rows are 3D points,
-// conf and the row (max, first argmax) as in EpiConf with own_is_pt.  Every warp reduces each
+// conf pass with the column maxima folded in: rows are 3D points; conf per element (conf_slice),
+// optional fp32 store of conf_matrix, and the per-row (max, first argmax) over this tile's columns
+// into part_val / part_idx (merged by opp_best_finalize).  Every warp reduces each
 // column of a slice over its 16 rows with a halving butterfly (lane ends with column
 // frag_lane_col()), the two warps of a 32-row group merge through the odd warp's stage, and the even
 // warp does one atomicMax per column on colmax[b][column] (conf >= 0, so its float bits order like
@@ -1442,7 +1367,7 @@ struct EpiConfColT {
       if (col < c.ncols) {
         float v[16];
         frag_slice<N>(d, j, v);
-        conf_slice(c, col, p.scale, lown, true, v, best, bidx);
+        conf_slice(c, col, p.scale, lown, v, best, bidx);
         if constexpr (kRows) {
 #pragma unroll
           for (int k = 0; k < 16; ++k)

@@ -244,9 +244,9 @@ constexpr int kKvChunk = 256;   // tokens per CTA (128 -> 256: half the partial-
 // M = d, N = v, K = token.  The tile is far too small for the wgmma engine (M = 128 would compute 8x the
 // needed head blocks and wants token-major operands transposed), so each warp (= head) runs
 // mma.sync m16n8k16 on fragments fetched with ldmatrix.trans straight from the token-major rows:
-// the kernel is a pure stream over kv16 (2 KB per token in split mode) and should sit on the HBM
-// roofline instead of the shared-memory/FMA issue limit of the SIMT version.
-//   split: K' = Kh + Kl, V = Vh + Vl  ->  Kh*Vh + Kh*Vl + Kl*Vh (fp32 accumulate, lo*lo dropped)
+// the kernel is a pure stream over kv16 (1 KB per token: one fp16 plane, whatever the operand mode
+// of the projections) and should sit on the HBM roofline instead of the shared-memory/FMA issue
+// limit of the SIMT version.
 //   ksum:  one extra n-tile whose B fragment is the constant 1.0 (no loads): C[d][*] = sum_t K'[t][d]
 // Rows are staged by cp.async (16 B, zero-filled past the end of the sequence) into a 3-stage
 // ring of 16-token slabs; the 16 B row padding makes the 8 row addresses of every ldmatrix 8x8
@@ -254,6 +254,9 @@ constexpr int kKvChunk = 256;   // tokens per CTA (128 -> 256: half the partial-
 // ---------------------------------------------------------------------------------------------
 constexpr int kKvmTok = 16;     // tokens per pipeline stage = one k16 MMA step
 constexpr int kKvmStages = 3;
+constexpr int kKvmRowB = 1024;  // [K'(256) V(256)] fp16
+constexpr int kKvmStride = kKvmRowB + 16;
+constexpr int kKvmSmem = kKvmStages * kKvmTok * kKvmStride;
 
 __device__ __forceinline__ void ldsm_x4_trans(uint32_t (&r)[4], uint32_t addr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
@@ -270,24 +273,20 @@ __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4],
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-template <bool SPLIT>
 __global__ void __launch_bounds__(256) kv_partial_mma_kernel(const __half* __restrict__ kv16,
                                                              float* __restrict__ part, int S,
                                                              int kv_chunk) {
   pdl_sync();
   extern __shared__ __align__(16) uint8_t kvm_smem[];
-  constexpr int kRowB = SPLIT ? 2048 : 1024;      // [K'(256) V(256)] fp16, x2 planes when split
-  constexpr int kStride = kRowB + 16;
-  constexpr int kStageB = kKvmTok * kStride;
-  constexpr int kUnitsPerRow = kRowB / 16;
+  constexpr int kStageB = kKvmTok * kKvmStride;
+  constexpr int kUnitsPerRow = kKvmRowB / 16;
   constexpr int kUnits = kKvmTok * kUnitsPerRow;   // 16-byte units per stage
-  constexpr int kLoB = 1024;                       // byte offset of the lo plane inside a row
   const int chunk = blockIdx.x, b = blockIdx.y, chunks = gridDim.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int s0 = chunk * kv_chunk;
   const int cnt = min(kv_chunk, S - s0);
   const int nsteps = (cnt + kKvmTok - 1) / kKvmTok;
-  const uint8_t* src = reinterpret_cast<const uint8_t*>(kv16) + ((long long)b * S + s0) * kRowB;
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(kv16) + ((long long)b * S + s0) * kKvmRowB;
   const uint32_t sbase = smem_u32(kvm_smem);
 
   auto load_stage = [&](int step) {
@@ -299,7 +298,7 @@ __global__ void __launch_bounds__(256) kv_partial_mma_kernel(const __half* __res
         const int u = threadIdx.x + j * 256;
         const int t = u / kUnitsPerRow, o = (u % kUnitsPerRow) * 16;
         const bool ok = t0 + t < cnt;
-        cp_async16_zfill(st + t * kStride + o, src + (long long)(ok ? t0 + t : 0) * kRowB + o,
+        cp_async16_zfill(st + t * kKvmStride + o, src + (long long)(ok ? t0 + t : 0) * kKvmRowB + o,
                          ok ? 16 : 0);
       }
     }
@@ -319,9 +318,9 @@ __global__ void __launch_bounds__(256) kv_partial_mma_kernel(const __half* __res
   // ldmatrix row addresses of this lane: matrix q = lane / 8, row r = lane % 8
   const int q = lane >> 3, r = lane & 7;
   //   A (K', M = d): q -> (token half q >> 1, d half q & 1)
-  const uint32_t a_off = (uint32_t)(((q >> 1) * 8 + r) * kStride + (warp * 32 + (q & 1) * 8) * 2);
+  const uint32_t a_off = (uint32_t)(((q >> 1) * 8 + r) * kKvmStride + (warp * 32 + (q & 1) * 8) * 2);
   //   B (V, N = v):  q -> (token half q & 1, n-tile q >> 1 of the pair)
-  const uint32_t b_off = (uint32_t)(((q & 1) * 8 + r) * kStride + (256 + warp * 32 + (q >> 1) * 8) * 2);
+  const uint32_t b_off = (uint32_t)(((q & 1) * 8 + r) * kKvmStride + (256 + warp * 32 + (q >> 1) * 8) * 2);
   const uint32_t ones = 0x3C003C00u;   // half2(1, 1)
 
   load_stage(0);
@@ -331,30 +330,19 @@ __global__ void __launch_bounds__(256) kv_partial_mma_kernel(const __half* __res
     cp_async_wait<2>();
     __syncthreads();
     const uint32_t st = sbase + (step % kKvmStages) * kStageB;
-    uint32_t ah[2][4], al[2][4], bh[2][4], bl[2][4];
+    uint32_t ah[2][4], bh[2][4];
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt) {
-      ldsm_x4_trans(ah[mt], st + a_off + mt * 32);
-      if (SPLIT) ldsm_x4_trans(al[mt], st + a_off + kLoB + mt * 32);
-    }
+    for (int mt = 0; mt < 2; ++mt) ldsm_x4_trans(ah[mt], st + a_off + mt * 32);
 #pragma unroll
-    for (int np = 0; np < 2; ++np) {
-      ldsm_x4_trans(bh[np], st + b_off + np * 32);
-      if (SPLIT) ldsm_x4_trans(bl[np], st + b_off + kLoB + np * 32);
-    }
+    for (int np = 0; np < 2; ++np) ldsm_x4_trans(bh[np], st + b_off + np * 32);
 #pragma unroll
     for (int mt = 0; mt < 2; ++mt) {
 #pragma unroll
       for (int nt = 0; nt < 4; ++nt) {
         const int np = nt >> 1, o = (nt & 1) * 2;
         mma_16816(acc[mt][nt], ah[mt], bh[np][o], bh[np][o + 1]);
-        if (SPLIT) {
-          mma_16816(acc[mt][nt], ah[mt], bl[np][o], bl[np][o + 1]);
-          mma_16816(acc[mt][nt], al[mt], bh[np][o], bh[np][o + 1]);
-        }
       }
       mma_16816(ks[mt], ah[mt], ones, ones);
-      if (SPLIT) mma_16816(ks[mt], al[mt], ones, ones);
     }
     __syncthreads();   // the slab is refilled by the load issued at the top of the next iteration
   }
@@ -522,25 +510,12 @@ __global__ void best_finalize_kernel(const float* __restrict__ pv, const int* __
 // =============================================================================================
 // match selection + ordered compaction   (utils/coarse_matching.py:142-172, 223-239)
 //   keep (b, l) iff conf_max > thr, argmax cell j not in the top/left border (mask_border only
-//   clears rows < b and cols < b: coarse_matching.py:10-20), and l is the column argmax of j.
+//   clears rows < b and cols < b: coarse_matching.py:10-20), and l is a column maximum of j.
 // =============================================================================================
-__device__ __forceinline__ bool match_flag(const float* pt_val, const int* pt_idx,
-                                           const int* px_idx, long long r, int l, int s, int wc,
-                                           float thr, int border) {
-  const float v = pt_val[r];
-  if (!(v > thr)) return false;
-  const int j = pt_idx[r];
-  const int jy = j / wc, jx = j - jy * wc;
-  if (jy < border || jx < border) return false;
-  const long long b = r / l;
-  const int i = (int)(r - b * l);
-  return px_idx[b * s + j] == i;
-}
-
-// Same selection with the mutual test expressed on values: row i keeps its argmax cell j iff its
+// The mutual test is expressed on values: row i keeps its argmax cell j iff its
 // row maximum IS the column maximum of j (colmax holds the float bits written by EpiConfCol from
 // the very same conf values, so the comparison is exact; coarse_matching.py:157-165 compares
-// conf == conf.max(dim) the same way).
+// conf == conf.max(dim) the same way, so every row of an exact tie is kept).
 // kRows (bank sets): rows i >= row_count[b] are the padding of the frame's object and never match.
 template <bool kRows = false>
 __device__ __forceinline__ bool match_flag_colmax(const float* pt_val, const int* pt_idx,
@@ -572,17 +547,6 @@ __global__ void __launch_bounds__(1024) match_count_colmax_kernel(const float* p
   const long long r = (long long)blockIdx.x * 1024 + threadIdx.x;
   const bool f = r < rows && match_flag_colmax<kRows>(pt_val, pt_idx, colmax, r, l, s, wc, thr, border,
                                                       row_count);
-  const int c = __syncthreads_count(f);
-  if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
-}
-
-__global__ void __launch_bounds__(1024) match_count_kernel(const float* pt_val, const int* pt_idx,
-                                                           const int* px_idx, long long rows,
-                                                           int l, int s, int wc, float thr,
-                                                           int border, int* block_counts) {
-  pdl_sync();
-  const long long r = (long long)blockIdx.x * 1024 + threadIdx.x;
-  const bool f = r < rows && match_flag(pt_val, pt_idx, px_idx, r, l, s, wc, thr, border);
   const int c = __syncthreads_count(f);
   if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
 }
@@ -627,54 +591,6 @@ __global__ void __launch_bounds__(1024) match_scan_kernel(int* counts, int nbloc
     counts[nblocks] = carry_s;
     *count_out = carry_s;
   }
-}
-
-__global__ void __launch_bounds__(1024)
-match_scatter_kernel(const float* pt_val, const int* pt_idx, const int* px_idx, const float* kpts,
-                     const float* img_scale, long long rows, int l, int s, int wc, float thr,
-                     int border, float cell, const int* block_offsets, long long* b_ids,
-                     long long* i_ids, long long* j_ids, float* mconf, float* mkpts3d,
-                     float* mkpts_c, int kpts_shared) {
-  pdl_sync();
-  __shared__ int warp_sums[32];
-  const long long r = (long long)blockIdx.x * 1024 + threadIdx.x;
-  const bool f = r < rows && match_flag(pt_val, pt_idx, px_idx, r, l, s, wc, thr, border);
-  const unsigned ballot = __ballot_sync(0xffffffffu, f);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) warp_sums[warp] = __popc(ballot);
-  __syncthreads();
-  if (warp == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int y = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += y;
-    }
-    warp_sums[lane] = w;
-  }
-  __syncthreads();
-  if (!f) return;
-  const int pos = block_offsets[blockIdx.x] + (warp > 0 ? warp_sums[warp - 1] : 0) +
-                  __popc(ballot & ((1u << lane) - 1u));
-  const long long b = r / l;
-  const int i = (int)(r - b * l);
-  const int j = pt_idx[r];
-  b_ids[pos] = b;
-  i_ids[pos] = i;
-  j_ids[pos] = j;
-  mconf[pos] = pt_val[r];
-  const float* kp = kpts + ((kpts_shared ? 0 : b) * l + i) * 3;
-  mkpts3d[pos * 3 + 0] = kp[0];
-  mkpts3d[pos * 3 + 1] = kp[1];
-  mkpts3d[pos * 3 + 2] = kp[2];
-  // coarse_matching.py:223-229: [j % w, j // w] * (scale * query_image_scale[b][[1, 0]])
-  float sx = cell, sy = cell;
-  if (img_scale) {
-    sx = cell * img_scale[b * 2 + 1];
-    sy = cell * img_scale[b * 2 + 0];
-  }
-  mkpts_c[pos * 2 + 0] = (float)(j % wc) * sx;
-  mkpts_c[pos * 2 + 1] = (float)(j / wc) * sy;
 }
 
 // kSet (bank sets): kpts is [K][l][3], read at bank_of_batch[b]; rows past row_count[b] are skipped
@@ -753,7 +669,7 @@ __global__ void __launch_bounds__(128) fine_gather_kernel(
   const float d = desc3d[(db * 128 + c) * n + i];
   if (x32) x32[row0 * 128 + c] = d;
   store_split1(x16 + row0 * ld, c, d, lo_off);
-  // windows (= row pitch P, 8 or 5): `fine` holds the compact per-match windows of opp_conv_win, [m][5][P][ld]
+  // windows (= row pitch P, opp_conv_win_pitch): `fine` holds the compact per-match windows of opp_conv_win, [m][5][P][ld]
   const __half* fb = windows ? fine + (long long)m * 5 * windows * ld : fine + b * hf * wf * ld;
   // all 25 window loads in flight before the first store (one block per match: the dependent
   // load -> store pairs of the rolled loop were 25 serial round trips)
@@ -1345,27 +1261,21 @@ int opp_kv_chunks_b(int s, int batch) {
   return (s + c - 1) / c;
 }
 
-int opp_kv_partial(const void* kv16, float* part, int batch, int s, int d, int split,
-                   opp_stream_t stream) {
+int opp_kv_partial(const void* kv16, float* part, int batch, int s, int d, opp_stream_t stream) {
   OPP_REQUIRE(kv16 && part, "null pointer");
   OPP_REQUIRE(d == 256, "kv_partial is built for d = 256 (8 heads x 32), got %d", d);
   const int kv_chunk = kv_chunk_tokens(s, batch);
   dim3 grid((s + kv_chunk - 1) / kv_chunk, batch);
-  const int smem = kKvmStages * kKvmTok * ((split ? 2048 : 1024) + 16);
   static unsigned long long attr_done = 0;   // per device
   int dev = 0;
   OPP_CHECK_CUDA(cudaGetDevice(&dev));
   if (dev < 64 && !((attr_done >> dev) & 1ull)) {
-    OPP_CHECK_CUDA(cudaFuncSetAttribute(kv_partial_mma_kernel<true>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    OPP_CHECK_CUDA(cudaFuncSetAttribute(kv_partial_mma_kernel<false>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    OPP_CHECK_CUDA(cudaFuncSetAttribute(kv_partial_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        kKvmSmem));
     attr_done |= 1ull << dev;
   }
-  if (split)
-    OPP_CHECK_CUDA(opp::launch_pdl(kv_partial_mma_kernel<true>, dim3(grid), dim3(256), smem, (cudaStream_t)stream, (const __half*)kv16, part, s, kv_chunk));
-  else
-    OPP_CHECK_CUDA(opp::launch_pdl(kv_partial_mma_kernel<false>, dim3(grid), dim3(256), smem, (cudaStream_t)stream, (const __half*)kv16, part, s, kv_chunk));
+  OPP_CHECK_CUDA(opp::launch_pdl(kv_partial_mma_kernel, dim3(grid), dim3(256), kKvmSmem, (cudaStream_t)stream,
+                                 (const __half*)kv16, part, s, kv_chunk));
   OPP_CHECK_CUDA(cudaGetLastError());
   return OPP_OK;
 }
@@ -1405,26 +1315,6 @@ int opp_best_finalize(const float* part_val, const int* part_idx, float* best_va
   OPP_REQUIRE(part_val && part_idx && best_val && best_idx, "null pointer");
   OPP_CHECK_CUDA(opp::launch_pdl(best_finalize_kernel, dim3((unsigned)((rows + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, 
       part_val, part_idx, best_val, best_idx, rows, tiles));
-  OPP_CHECK_CUDA(cudaGetLastError());
-  return OPP_OK;
-}
-
-int opp_match_select(const float* pt_val, const int* pt_idx, const int* px_idx, const float* kpts,
-                     const float* img_scale, int batch, int l, int hc, int wc, float thr,
-                     int border, float cell, int* scratch, long long* b_ids, long long* i_ids,
-                     long long* j_ids, float* mconf, float* mkpts3d, float* mkpts_c,
-                     int* count_out, int bank_shared, opp_stream_t stream) {
-  OPP_REQUIRE(pt_val && pt_idx && px_idx && kpts && scratch && count_out, "null pointer");
-  const long long rows = (long long)batch * l;
-  const int nblocks = (int)((rows + 1023) / 1024);
-  const int s = hc * wc;
-  cudaStream_t st = (cudaStream_t)stream;
-  OPP_CHECK_CUDA(opp::launch_pdl(match_count_kernel, dim3(nblocks), dim3(1024), 0, st, pt_val, pt_idx, px_idx, rows, l, s, wc, thr, border,
-                                               scratch));
-  OPP_CHECK_CUDA(opp::launch_pdl(match_scan_kernel, dim3(1), dim3(1024), 0, st, scratch, nblocks, count_out));
-  OPP_CHECK_CUDA(opp::launch_pdl(match_scatter_kernel, dim3(nblocks), dim3(1024), 0, st, pt_val, pt_idx, px_idx, kpts, img_scale, rows, l,
-                                                 s, wc, thr, border, cell, scratch, b_ids, i_ids,
-                                                 j_ids, mconf, mkpts3d, mkpts_c, bank_shared));
   OPP_CHECK_CUDA(cudaGetLastError());
   return OPP_OK;
 }

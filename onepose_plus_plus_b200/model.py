@@ -276,10 +276,10 @@ class _Engine(nn.Module):
         self._ws = {}
         self._ws_epoch = 0
         self._graphs = {}
-        # K'/V rows of the coarse attention state stored as ONE fp16 plane: their only consumer sums
-        # them over thousands of tokens, so the 2^-12 rounding averages out (oracle experiment: conf
-        # changes by 1e-4; the whole GPU parity suite passes with it)
-        self.kv_single_plane = os.environ.get("OPP_B200_KV1", "1") == "1"
+
+    @property
+    def kv_single_plane(self):
+        return True   # read-only, reported by bench.py: the K'/V rows have no other layout
 
     def _pe_module(self):
         return getattr(self, "dense_pos_encoding", None)
@@ -520,20 +520,20 @@ class _Engine(nn.Module):
         """Source side of linear attention for one layer (linear_attention.py:46,55-57 +
         transformer.py:78-79,85): K' = elu(Wk src)+1, V = Wv src, per-head KV / Ksum, with `merge`
         folded in -> (Mt [B, 256, pl*256] fp16, Ksum [B, 256] fp32).  v_len (default ls): the
-        length the query side multiplies back by (linear_attention.py:55,61)."""
+        length the query side multiplies back by (linear_attention.py:55,61).  The K'/V rows are ONE
+        fp16 plane in both operand modes: their only consumer sums them over thousands of tokens, so
+        the 2^-12 rounding averages out (oracle experiment: conf changes by 1e-4)."""
         dev = src.device
         f16 = torch.float16
         split = self.split
         pl = 2 if split else 1
-        kv_split = split and not self.kv_single_plane
-        kv16 = self._buf(tag + "kv16", (B * ls, (2 if kv_split else 1) * 512), f16, dev)
-        ops.linear_act(src, None, L["wkv"], kv16, B * ls, 2, 256, split, out_split=kv_split,
+        kv16 = self._buf(tag + "kv16", (B * ls, 512), f16, dev)
+        ops.linear_act(src, None, L["wkv"], kv16, B * ls, 2, 256, split, out_split=False,
                        row_mask=src_mask)
         part = self._buf(tag + "part", (B, ops.kv_chunks(ls, B), 8, 33, 32), torch.float32, dev)
         mt = self._buf(tag + "mt", (B, 256, pl * 256), f16, dev)
         ksum = self._buf(tag + "ksum", (B, 256), torch.float32, dev)
-        ops.kv_state(kv16, part, L["merge32"], mt, ksum, B, ls, 256, ls if v_len is None else v_len, split,
-                     kv_split=kv_split)
+        ops.kv_state(kv16, part, L["merge32"], mt, ksum, B, ls, 256, ls if v_len is None else v_len, split)
         return mt, ksum
 
     def _encoder_layer(self, L, tag, x, src, B, lx, ls, out, x_shared=False, state=None, x_mask=None,
@@ -664,14 +664,19 @@ class OnePosePlus_model(_Engine):
         # keypoint encoder of .train() on CUDA: "autograd" = train_path.keypoint_encoding, "kernels" = the
         # opp_kpt_train_* kernels forward and backward, recomputing each point's MLP (train_kpt.py)
         self.kpt_encoder_train_mode = os.environ.get("OPP_B200_KPT_TRAIN", "autograd")
-        # one-pass dual softmax: column statistics of sim / conf from the row passes (warp
-        # butterflies in the epilogue) instead of two more sim GEMM passes
-        self.coarse_colmax = os.environ.get("OPP_B200_COLMAX", "1") == "1"
-        self.coarse_lse_cols = os.environ.get("OPP_B200_LSECOLS", "1") == "1"
         # layer1_outconv2 (the last two 3x3 convolutions of the FPN, 1/2 resolution) evaluated only on
         # the 5x5 windows the fine stage reads: "auto" = when cheaper than the dense map (by the
         # match count), "sparse" / "dense" = always / never
         self.fine_windows = os.environ.get("OPP_B200_FINE_WINDOWS", "auto")
+
+    # read-only, reported by bench.py: coarse matching is always the one-pass dual softmax
+    @property
+    def coarse_colmax(self):
+        return True
+
+    @property
+    def coarse_lse_cols(self):
+        return True
 
     # pickling (Ray ships the module object): drop device-side caches
     def __getstate__(self):
@@ -939,7 +944,7 @@ class OnePosePlus_model(_Engine):
 
     def _coarse_matching(self, q2, d3, bank, img_scale, B, N, hc, wc, cell, out, qmask=None, pack=None, side=None):
         """CoarseMatching.forward + get_coarse_match (coarse_matching.py:76-242), inference branch.
-        Enqueues everything up to the ordered match lists (capacity B*min(N,S)) and the device-side
+        Enqueues everything up to the ordered match lists (capacity B*N) and the device-side
         match count; nothing here synchronises.  Fills `out` with the full-capacity tensors."""
         dev = q2.device
         S = hc * wc
@@ -947,39 +952,26 @@ class OnePosePlus_model(_Engine):
         split = self.split
         cm = self.coarse_matching
         scale = 1.0 / (256.0 * (cm.temperature + 1e-4))  # (a/16).(b/16)/(T+1e-4)
-        ts, tl = ops.sim_tiles(S), ops.sim_tiles(N)
+        ts = ops.sim_tiles(S)
         pm_pt = self._buf("pm_pt", (B * N, ts), f32, dev)
         ps_pt = self._buf("ps_pt", (B * N, ts), f32, dev)
         lse_pt = self._buf("lse_pt", (B, N), f32, dev)
         lse_px = self._buf("lse_px", (B, S), f32, dev)
-        if qmask is not None and not (self.coarse_lse_cols and self.coarse_colmax):
-            raise NotImplementedError("query_image_mask is built for the one-pass dual softmax "
-                                      "(coarse_lse_cols and coarse_colmax on)")
         # bank set: rows >= row_count[b] are the padding of frame b's object
         rows_b, bank_of_batch = bank.get("row_count"), bank.get("bank_of_batch")
-        if rows_b is not None and not (self.coarse_lse_cols and self.coarse_colmax):
-            raise NotImplementedError("bank sets are built for the one-pass dual softmax "
-                                      "(coarse_lse_cols and coarse_colmax on)")
-        if self.coarse_lse_cols:
-            groups = (N + 31) // 32
-            col_m = self._buf("lse_col_m", (B, groups, S), f32, dev)
-            col_s = self._buf("lse_col_s", (B, groups, S), f32, dev)
-            ops.sim_lse_cols(d3, q2, B, N, S, 256, scale, pm_pt, ps_pt, lse_pt, col_m, col_s, lse_px, split,
-                             col_mask=qmask, side_stream=side, row_count=rows_b)
-        else:
-            pm_px = self._buf("pm_px", (B * S, tl), f32, dev)
-            ps_px = self._buf("ps_px", (B * S, tl), f32, dev)
-            ops.sim_lse(d3, q2, B, N, S, 256, scale, pm_pt, ps_pt, lse_pt, split)
-            ops.sim_lse(q2, d3, B, S, N, 256, scale, pm_px, ps_px, lse_px, split)
+        groups = (N + 31) // 32
+        col_m = self._buf("lse_col_m", (B, groups, S), f32, dev)
+        col_s = self._buf("lse_col_s", (B, groups, S), f32, dev)
+        ops.sim_lse_cols(d3, q2, B, N, S, 256, scale, pm_pt, ps_pt, lse_pt, col_m, col_s, lse_px, split,
+                         col_mask=qmask, side_stream=side, row_count=rows_b)
         mode = self.conf_matrix_mode
         conf = torch.empty((B, N, S), dtype=f32, device=dev) if mode == "eager" else None  # caller's
         pi_pt = self._buf("pi_pt", (B * N, ts), i32, dev)
         pt_val = self._buf("pt_val", (B, N), f32, dev)
         pt_idx = self._buf("pt_idx", (B, N), i32, dev)
-        # capacity: one match per 3D point and per query cell (mutual nearest neighbours); the
-        # value-based mutual test keeps every row of an exact tie (as the reference's mask does), so
-        # its capacity is one per 3D point
-        cap = B * N if self.coarse_colmax else B * min(N, S)
+        # capacity: one match per 3D point; the value-based mutual test keeps every row of an exact
+        # tie (as the reference's mask does), so a query cell can match more than one point
+        cap = B * N
         scratch = self._buf("match_scratch", ((B * N + 1023) // 1024 + 2,), i32, dev)
         count = self._buf("match_count", (1,), i32, dev)
         new = pack.new if pack is not None else (
@@ -990,27 +982,13 @@ class OnePosePlus_model(_Engine):
         mconf = new("mconf", (cap,), f32)
         mk3 = new("mkpts_3d_db", (cap, 3), f32)
         mkc = new("mkpts_query_c", (cap, 2), f32)
-        kshared = bank["Bb"] == 1
-        if self.coarse_colmax:
-            colmax = self._buf("colmax", (B, S), i32, dev)
-            ops.sim_conf_colmax(d3, q2, lse_pt, lse_px, conf, B, N, S, 256, scale, pm_pt, pi_pt,
-                                pt_val, pt_idx, colmax, split, row_count=rows_b)
-            ops.match_select_colmax(pt_val, pt_idx, colmax, bank["kpts"], img_scale, B, N, hc, wc,
-                                    cm.thr, cm.border_rm, cell, scratch, b_ids, i_ids, j_ids, mconf,
-                                    mk3, mkc, count, bank_shared=kshared, bank_of_batch=bank_of_batch,
-                                    row_count=rows_b)
-        else:
-            pi_px = self._buf("pi_px", (B * S, tl), i32, dev)
-            pm_px = self._buf("pm_px", (B * S, tl), f32, dev)
-            px_val = self._buf("px_val", (B, S), f32, dev)
-            px_idx = self._buf("px_idx", (B, S), i32, dev)
-            ops.sim_conf(d3, q2, lse_pt, lse_px, True, conf, B, N, S, 256, scale, pm_pt, pi_pt,
-                         pt_val, pt_idx, split)
-            ops.sim_conf(q2, d3, lse_px, lse_pt, False, None, B, S, N, 256, scale, pm_px, pi_px,
-                         px_val, px_idx, split)
-            ops.match_select(pt_val, pt_idx, px_idx, bank["kpts"], img_scale, B, N, hc, wc,
-                             cm.thr, cm.border_rm, cell, scratch, b_ids, i_ids, j_ids, mconf, mk3, mkc,
-                             count, bank_shared=kshared)
+        colmax = self._buf("colmax", (B, S), i32, dev)
+        ops.sim_conf_colmax(d3, q2, lse_pt, lse_px, conf, B, N, S, 256, scale, pm_pt, pi_pt,
+                            pt_val, pt_idx, colmax, split, row_count=rows_b)
+        ops.match_select_colmax(pt_val, pt_idx, colmax, bank["kpts"], img_scale, B, N, hc, wc,
+                                cm.thr, cm.border_rm, cell, scratch, b_ids, i_ids, j_ids, mconf,
+                                mk3, mkc, count, bank_shared=bank["Bb"] == 1, bank_of_batch=bank_of_batch,
+                                row_count=rows_b)
         if mode == "lazy":
             conf = LazyConfMatrix(self, d3, q2, lse_pt, lse_px, B, N, S, scale, rows_b)
         out.update({"conf_matrix": conf, "b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids, "mconf": mconf,
@@ -1018,18 +996,15 @@ class OnePosePlus_model(_Engine):
         return count, cap
 
     def _materialize_conf(self, d3, q2, lse_pt, lse_px, B, N, S, scale, rows_b=None):
-        """conf_matrix on demand (LazyConfMatrix): re-runs the conf pass with the fp32 store (for a
-        bank set the colmax pass, which stores 0 on the padded rows)."""
+        """conf_matrix on demand (LazyConfMatrix): re-runs the conf pass of the forward with the fp32
+        store (for a bank set it stores 0 on the padded rows); its row and column maxima go to scratch."""
         dev = q2.device
         ts = ops.sim_tiles(S)
         conf = torch.empty((B, N, S), dtype=torch.float32, device=dev)
         part = (self._buf("lz_pv", (B * N, ts), torch.float32, dev), self._buf("lz_pi", (B * N, ts), torch.int32, dev),
                 self._buf("lz_bv", (B, N), torch.float32, dev), self._buf("lz_bi", (B, N), torch.int32, dev))
-        if rows_b is not None:
-            ops.sim_conf_colmax(d3, q2, lse_pt, lse_px, conf, B, N, S, 256, scale, *part,
-                                self._buf("lz_colmax", (B, S), torch.int32, dev), self.split, row_count=rows_b)
-        else:
-            ops.sim_conf(d3, q2, lse_pt, lse_px, True, conf, B, N, S, 256, scale, *part, self.split)
+        ops.sim_conf_colmax(d3, q2, lse_pt, lse_px, conf, B, N, S, 256, scale, *part,
+                            self._buf("lz_colmax", (B, S), torch.int32, dev), self.split, row_count=rows_b)
         return conf
 
     def _fine(self, fine_map, bank, ids, M, img_scale, hc, wc, q_hw_i, out, count=None, pack=None, windows_hw=None):
@@ -1271,7 +1246,7 @@ class OnePosePlus_model(_Engine):
         pack = None
         if dynamic:
             S = hc * wc
-            cap = B * N if self.coarse_colmax else B * min(N, S)
+            cap = B * N
             fcap = min(cap, B * min(N, S))
             pack = _OutPack(_OutPack.nbytes(cap, fcap), img.device)
             out["gt_mask"] = pack.new("gt_mask", (cap,), torch.bool)   # zeroed once by _replay, never written
@@ -1340,7 +1315,7 @@ class OnePosePlus_model(_Engine):
                 bank_raw = tuple(t[:1] for t in bank_raw)
             bkey = tuple((tuple(t.shape), t.dtype) for t in bank_raw)
         key = (tuple(img.shape), img.dtype, img_scale is not None, bkey, fine_on, self.conf_matrix_mode,
-               self.coarse_colmax, self.coarse_lse_cols, self.kv_single_plane, self.fine_windows)
+               self.fine_windows)
         if prologue is not None:
             key = key + (prologue.key,)
         ent = self._graphs.get(key)

@@ -145,10 +145,9 @@ def kv_chunks(s, batches=None):
     return _lib.load().opp_kv_chunks_b(s, batches)
 
 
-def kv_state(kv16, part, merge_w, mt, ksum, batches, s, d, v_len, split, kv_split=None):
-    """kv_split: plane mode of the kv16 rows when it differs from the mode of the mt output."""
-    kv_split = split if kv_split is None else kv_split
-    call("opp_kv_partial", ptr(kv16), ptr(part), batches, s, d, int(kv_split), stream())
+def kv_state(kv16, part, merge_w, mt, ksum, batches, s, d, v_len, split):
+    """kv16: single-plane fp16 K'/V rows [batches * s, 2d]; split: plane mode of the mt output."""
+    call("opp_kv_partial", ptr(kv16), ptr(part), batches, s, d, stream())
     call("opp_kv_finalize", ptr(part), ptr(merge_w), ptr(mt), ptr(ksum), batches, kv_chunks(s, batches), d,
          float(v_len), int(split), stream())
 
@@ -157,25 +156,9 @@ def sim_tiles(cols):
     return _lib.load().opp_sim_tiles(cols)
 
 
-def sim_lse(a, b, batches, rows, cols, k, scale, part_m, part_s, lse, split):
-    tiles = sim_tiles(cols)
-    call("opp_sim_lse", ptr(a), ptr(b), ptr(part_m), ptr(part_s), batches, rows, cols, k,
-         float(scale), int(split), stream())
-    call("opp_lse_finalize", ptr(part_m), ptr(part_s), ptr(lse), batches * rows, tiles, stream())
-
-
-def sim_conf(a, b, lse_own, lse_other, own_is_pt, conf, batches, rows, cols, k, scale, part_val,
-             part_idx, best_val, best_idx, split):
-    tiles = sim_tiles(cols)
-    call("opp_sim_conf", ptr(a), ptr(b), ptr(lse_own), ptr(lse_other), int(own_is_pt), ptr(conf),
-         ptr(part_val), ptr(part_idx), batches, rows, cols, k, float(scale), int(split), stream())
-    call("opp_best_finalize", ptr(part_val), ptr(part_idx), ptr(best_val), ptr(best_idx),
-         batches * rows, tiles, stream())
-
-
 def sim_lse_cols(a, b, batches, rows, cols, k, scale, part_m, part_s, lse_rows, col_m, col_s, lse_cols,
                  split, col_mask=None, side_stream=None, row_count=None):
-    """lse over columns for every row (as sim_lse) AND lse over rows for every column, one GEMM pass.
+    """lse over columns for every row AND lse over rows for every column, one GEMM pass.
     col_mask uint8 [batches, cols]: masked columns (0) get sim - 1e9 and lse_cols = +inf (conf = 0).
     row_count int32 [batches] (bank sets): rows past the count drop out of lse_cols; their lse_rows
     are not meaningful.
@@ -233,13 +216,6 @@ def match_select_colmax(pt_val, pt_idx, colmax, kpts, img_scale, batch, l, hc, w
              ptr(bank_of_batch), ptr(row_count), stream())
         return
     call("opp_match_select_colmax", ptr(pt_val), ptr(pt_idx), ptr(colmax), ptr(kpts), ptr(img_scale),
-         batch, l, hc, wc, float(thr), int(border), float(cell), ptr(scratch), ptr(b_ids),
-         ptr(i_ids), ptr(j_ids), ptr(mconf), ptr(mkpts3d), ptr(mkpts_c), ptr(count), int(bank_shared), stream())
-
-
-def match_select(pt_val, pt_idx, px_idx, kpts, img_scale, batch, l, hc, wc, thr, border, cell,
-                 scratch, b_ids, i_ids, j_ids, mconf, mkpts3d, mkpts_c, count, bank_shared=False):
-    call("opp_match_select", ptr(pt_val), ptr(pt_idx), ptr(px_idx), ptr(kpts), ptr(img_scale),
          batch, l, hc, wc, float(thr), int(border), float(cell), ptr(scratch), ptr(b_ids),
          ptr(i_ids), ptr(j_ids), ptr(mconf), ptr(mkpts3d), ptr(mkpts_c), ptr(count), int(bank_shared), stream())
 

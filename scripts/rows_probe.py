@@ -46,16 +46,13 @@ SHAPES = {
     "opp_linear_q_f16": lambda a: (a[4], a[5], a[6], a[6], a[9]),
     "opp_linear_ln": lambda a: (a[13], a[14], a[15], a[1] + a[3], a[16]),
     "opp_linear_ln_dyn": lambda a: (1, a[11], a[14], a[1] + a[3], a[15]),
-    "opp_sim_lse": lambda a: (a[4], a[5], a[6], a[7], a[9]),
-    "opp_sim_conf": lambda a: (a[8], a[9], a[10], a[11], a[13]),
     "opp_sim_lse_cols": lambda a: (a[6], a[7], a[8], a[9], a[11]),
     "opp_sim_conf_colmax": lambda a: (a[8], a[9], a[10], a[11], a[13]),
 }
 EPILOGUE = {"opp_linear_act_f16": "EpiStoreF16", "opp_linear_act_f16_out1": "EpiStoreF16",
             "opp_linear_act_f16_b": "EpiStoreF16", "opp_linear_act_f16_dyn": "EpiStoreF16",
             "opp_linear_q_f16": "EpiQ", "opp_linear_ln": "EpiLN", "opp_linear_ln_dyn": "EpiLN",
-            "opp_sim_lse": "EpiLse", "opp_sim_conf": "EpiConf", "opp_sim_lse_cols": "EpiLseCol",
-            "opp_sim_conf_colmax": "EpiConfCol"}
+            "opp_sim_lse_cols": "EpiLseCol", "opp_sim_conf_colmax": "EpiConfCol"}
 
 
 def _scalar(x):
@@ -102,8 +99,7 @@ def child(args):
 
     # keep every tensor handed to an op alive, so the recorded device pointers stay valid
     wrapped = {}
-    for fname in ("linear_act", "linear_q", "linear_ln", "sim_lse", "sim_conf", "sim_lse_cols", "sim_conf_colmax",
-                  "conv1_gemm"):
+    for fname in ("linear_act", "linear_q", "linear_ln", "sim_lse_cols", "sim_conf_colmax", "conv1_gemm"):
         fn = getattr(ops, fname)
 
         def w(*a, _fn=fn, _name=fname, **kw):

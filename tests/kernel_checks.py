@@ -734,65 +734,6 @@ def check_conv_win_production():
     _run_child("conv_win_production_tiles", OPP_LOG_TILES="1")
 
 
-def check_sim():
-    for split in (0, 1):
-        for (B, L, S, K) in [(2, 700, 520, 256), (1, 300, 100, 256), (1, 5000, 4096, 256)]:
-            af = _rand(B, L, K, scale=0.9, seed=1)
-            bf = _rand(B, S, K, scale=0.9, seed=2)
-            a, b = _planes(af, split), _planes(bf, split)
-            scale = 1.0 / (256 * 0.0801)
-            sim = (torch.einsum("blk,bsk->bls", _q(af, split).double(), _q(bf, split).double()) * scale)
-            lse_pt_ref = torch.logsumexp(sim, 2).float()   # over query cells, per 3D point
-            lse_px_ref = torch.logsumexp(sim, 1).float()   # over 3D points, per query cell
-            lib = _lib.load()
-            ts, tl = lib.opp_sim_tiles(S), lib.opp_sim_tiles(L)
-
-            def lse(x, y, rows, cols, tiles):
-                pm = torch.empty(B * rows, tiles, device=DEV)
-                ps = torch.empty(B * rows, tiles, device=DEV)
-                out = torch.empty(B, rows, device=DEV)
-                _lib.call("opp_sim_lse", _lib.ptr(x), _lib.ptr(y), _lib.ptr(pm), _lib.ptr(ps), B, rows,
-                          cols, K, scale, split, _lib.stream())
-                _lib.call("opp_lse_finalize", _lib.ptr(pm), _lib.ptr(ps), _lib.ptr(out), B * rows, tiles,
-                          _lib.stream())
-                return out
-
-            lse_pt = lse(a, b, L, S, ts)
-            lse_px = lse(b, a, S, L, tl)
-            torch.cuda.synchronize()
-            _close(f"sim split={split} lse_pt B={B} L={L} S={S}", lse_pt, lse_pt_ref, 1e-5, 1e-4)
-            _close("sim lse_px", lse_px, lse_px_ref, 1e-5, 1e-4)
-
-            conf = torch.full((B, L, S), float("nan"), device=DEV)
-
-            def best(x, y, own, other, own_is_pt, rows, cols, tiles, conf_out):
-                pv = torch.empty(B * rows, tiles, device=DEV)
-                pi = torch.empty(B * rows, tiles, device=DEV, dtype=torch.int32)
-                bv = torch.empty(B, rows, device=DEV)
-                bi = torch.empty(B, rows, device=DEV, dtype=torch.int32)
-                _lib.call("opp_sim_conf", _lib.ptr(x), _lib.ptr(y), _lib.ptr(own), _lib.ptr(other),
-                          own_is_pt, _lib.ptr(conf_out), _lib.ptr(pv), _lib.ptr(pi), B, rows, cols, K,
-                          scale, split, _lib.stream())
-                _lib.call("opp_best_finalize", _lib.ptr(pv), _lib.ptr(pi), _lib.ptr(bv), _lib.ptr(bi),
-                          B * rows, tiles, _lib.stream())
-                return bv, bi
-
-            pt_val, pt_idx = best(a, b, lse_pt, lse_px, 1, L, S, ts, conf)
-            px_val, px_idx = best(b, a, lse_px, lse_pt, 0, S, L, tl, None)
-            torch.cuda.synchronize()
-            conf_ref = (torch.softmax(sim, 1) * torch.softmax(sim, 2)).float()
-            _close("sim conf", conf, conf_ref, 5e-4, 1e-7)
-            # maxima must agree with the conf matrix the kernel itself wrote (index-exact)
-            v, i = conf.max(2)
-            assert torch.equal(pt_idx.long(), i), "row argmax mismatch"
-            assert torch.equal(pt_val, v), "row max mismatch"
-            v, i = conf.max(1)
-            _close("sim col max", px_val, v, 1e-5, 1e-9)
-            agree = (px_idx.long() == i).float().mean().item()
-            print(f"  col argmax agreement {agree:.6f}")
-            assert agree > 0.999
-
-
 # ------------------------------------------------------------------------------------------ SIMT
 def _conv1_gemm_case(split, B, H, W, C, u8):
     """conv1 as im2col + one 64-wide wgmma K chunk (bias in K column 49), fp32 and uint8 images"""
@@ -861,21 +802,23 @@ def check_kpt_encode():
 
 
 def check_kv_state():
+    """single-plane K'/V rows (what the forward writes in both operand modes) -> KV state, with the
+    mt output in both plane modes"""
     for split in (0, 1):
         B, S, d = 2, 1000, 256
         kvf = torch.cat([_rand(B, S, d, seed=1).abs() + 0.1, _rand(B, S, d, seed=2)], 2)
-        kv = _planes(kvf, split)
+        kv = _planes(kvf, 0)
         mw = _rand(d, d, scale=0.06, seed=3)
         chunks = _lib.load().opp_kv_chunks_b(S, B)
         pl = 2 if split else 1
         part = torch.empty(B, chunks, 8, 33, 32, device=DEV)
         mt = torch.empty(B, d, pl * d, device=DEV, dtype=torch.half)
         ksum = torch.empty(B, d, device=DEV)
-        _lib.call("opp_kv_partial", _lib.ptr(kv), _lib.ptr(part), B, S, d, split, _lib.stream())
+        _lib.call("opp_kv_partial", _lib.ptr(kv), _lib.ptr(part), B, S, d, _lib.stream())
         _lib.call("opp_kv_finalize", _lib.ptr(part), _lib.ptr(mw), _lib.ptr(mt), _lib.ptr(ksum), B,
                   chunks, d, float(S), split, _lib.stream())
         torch.cuda.synchronize()
-        kvq = _q(kvf, split).double()
+        kvq = _q(kvf, 0).double()
         K = kvq[..., :d].view(B, S, 8, 32)
         V = kvq[..., d:].view(B, S, 8, 32)
         KV = torch.einsum("bshd,bshv->bhdv", K, V) / S
@@ -884,54 +827,6 @@ def check_kv_state():
         ref_mt = torch.einsum("chv,bhdv->bchd", mw.double().view(d, 8, 32), KV).reshape(B, d, d).float()
         _close(f"kv ksum split={split}", ksum, ref_ksum, 1e-5, 1e-3)
         _close("kv mt", _unplanes(mt, split), ref_mt, *_tol(split, (2e-3, 1e-4), (2e-5, 1e-6)))
-
-
-def check_match_select():
-    B, L, hc, wc = 3, 2500, 20, 24
-    S = hc * wc
-    g = torch.Generator().manual_seed(0)
-    conf = torch.rand(B, L, S, generator=g).to(DEV) * 0.3
-    # plant mutual maxima
-    for b in range(B):
-        perm = torch.randperm(S, generator=g)[:200]
-        rows = torch.randperm(L, generator=g)[:200]
-        conf[b, rows, perm] = 0.5 + 0.5 * torch.rand(200, generator=g).to(DEV)
-    pt_val, pt_idx = conf.max(2)
-    px_idx = conf.max(1).indices
-    kpts = torch.rand(B, L, 3, device=DEV)
-    scale = torch.rand(B, 2, device=DEV) + 0.5
-    cap = B * min(L, S)
-    scratch = torch.empty((B * L + 1023) // 1024 + 2, device=DEV, dtype=torch.int32)
-    b_ids = torch.empty(cap, device=DEV, dtype=torch.int64)
-    i_ids, j_ids = torch.empty_like(b_ids), torch.empty_like(b_ids)
-    mconf = torch.empty(cap, device=DEV)
-    mk3 = torch.empty(cap, 3, device=DEV)
-    mkc = torch.empty(cap, 2, device=DEV)
-    cnt = torch.zeros(1, device=DEV, dtype=torch.int32)
-    pt_idx32, px_idx32 = pt_idx.int(), px_idx.int()
-    _lib.call("opp_match_select", _lib.ptr(pt_val), _lib.ptr(pt_idx32), _lib.ptr(px_idx32),
-              _lib.ptr(kpts), _lib.ptr(scale), B, L, hc, wc, 0.4, 2, 8.0, _lib.ptr(scratch),
-              _lib.ptr(b_ids), _lib.ptr(i_ids), _lib.ptr(j_ids), _lib.ptr(mconf), _lib.ptr(mk3),
-              _lib.ptr(mkc), _lib.ptr(cnt), 0, _lib.stream())
-    torch.cuda.synchronize()
-    M = int(cnt.item())
-    # reference semantics (coarse_matching.py:142-172)
-    mask = conf > 0.4
-    mask = mask.view(B, L, hc, wc)
-    mask[:, :, :2] = False
-    mask[:, :, :, :2] = False
-    mask = mask.view(B, L, S)
-    mask = mask * (conf == conf.max(2, keepdim=True)[0]) * (conf == conf.max(1, keepdim=True)[0])
-    mv, aj = mask.max(2)
-    rb, ri = torch.where(mv)
-    rj = aj[rb, ri]
-    print(f"  match_select: M={M} ref={len(rb)}")
-    assert M == len(rb) and M > 100
-    assert torch.equal(b_ids[:M], rb) and torch.equal(i_ids[:M], ri) and torch.equal(j_ids[:M], rj)
-    assert torch.equal(mconf[:M], conf[rb, ri, rj])
-    assert torch.equal(mk3[:M], kpts[rb, ri])
-    ref_c = torch.stack([rj % wc, rj // wc], 1) * (8.0 * scale[rb][:, [1, 0]])
-    _close("match_select mkpts_c", mkc[:M], ref_c, 1e-6, 1e-5)
 
 
 def check_fine():
@@ -1133,13 +1028,11 @@ def check_sim_colmax():
             a, b = _planes(af, split), _planes(bf, split)
             scale = 1.0 / (256 * 0.0801)
             sim = (torch.einsum("blk,bsk->bls", _q(af, split).double(), _q(bf, split).double()) * scale)
-            lib = _lib.load()
-            ts, tl = lib.opp_sim_tiles(S), lib.opp_sim_tiles(L)
+            ts, groups = _lib.load().opp_sim_tiles(S), (L + 31) // 32
             lse_pt, lse_px = torch.empty(B, L, device=DEV), torch.empty(B, S, device=DEV)
-            ops.sim_lse(a, b, B, L, S, K, scale, torch.empty(B * L, ts, device=DEV),
-                        torch.empty(B * L, ts, device=DEV), lse_pt, split)
-            ops.sim_lse(b, a, B, S, L, K, scale, torch.empty(B * S, tl, device=DEV),
-                        torch.empty(B * S, tl, device=DEV), lse_px, split)
+            ops.sim_lse_cols(a, b, B, L, S, K, scale, torch.empty(B * L, ts, device=DEV),
+                             torch.empty(B * L, ts, device=DEV), lse_pt, torch.empty(B, groups, S, device=DEV),
+                             torch.empty(B, groups, S, device=DEV), lse_px, split)
             conf = torch.full((B, L, S), float("nan"), device=DEV)
             pv = torch.empty(B * L, ts, device=DEV)
             pi = torch.empty(B * L, ts, device=DEV, dtype=torch.int32)
@@ -1202,7 +1095,7 @@ def check_kv_single_plane():
     part = torch.empty(B, chunks, 8, 33, 32, device=DEV)
     mt = torch.empty(B, d, 2 * d, device=DEV, dtype=torch.half)
     ksum = torch.empty(B, d, device=DEV)
-    ops.kv_state(kv, part, mw, mt, ksum, B, S, d, float(S), True, kv_split=False)
+    ops.kv_state(kv, part, mw, mt, ksum, B, S, d, float(S), True)
     torch.cuda.synchronize()
     kvq = kv.double().view(B, S, 2 * d)
     K, V = kvq[..., :d].view(B, S, 8, 32), kvq[..., d:].view(B, S, 8, 32)
@@ -1729,11 +1622,9 @@ CHECKS = {
     "conv_layers": check_conv_layers,
     "conv_launch_invariance": check_conv_launch_invariance,
     "conv_win_production": check_conv_win_production,
-    "sim": check_sim,
     "conv1_gemm": check_conv1_gemm,
     "kpt_encode": check_kpt_encode,
     "kv_state": check_kv_state,
-    "match_select": check_match_select,
     "fine": check_fine,
     "full_attention": check_full_attention,
     "loftr_kernels": check_loftr_kernels,

@@ -352,21 +352,3 @@ def test_shared_bank_views_match_materialised_bank():
     for k in ("b_ids", "i_ids", "j_ids", "mconf", "expec_f", "mkpts_query_f", "conf_matrix"):
         assert torch.equal(a[k], shared[k]), k
 
-
-def test_four_pass_dual_softmax_flow_matches():
-    """The older flow (two lse + two conf GEMM passes, index-based mutual test) stays selectable
-    (model.coarse_colmax / coarse_lse_cols = False): same matches as the one-pass default."""
-    m = parity.cuda_model()
-    case = golden_io.cases()[0]
-    data, z = golden_io.load(case)
-    a = parity.run_cuda(data)
-    try:
-        m.coarse_colmax = m.coarse_lse_cols = False
-        b = parity.run_cuda(data)
-        parity.compare(b, {k: z[k] for k in z.files}, max_borderline=0)
-    finally:
-        m.coarse_colmax = m.coarse_lse_cols = True
-    for k in ("b_ids", "i_ids", "j_ids"):
-        assert torch.equal(a[k], b[k])
-    # the column statistics are merged in a different order (32-row groups vs 256-column tiles)
-    assert torch.allclose(a["mconf"], b["mconf"], atol=1e-4) and torch.allclose(a["conf_matrix"], b["conf_matrix"], atol=1e-4)

@@ -32,7 +32,7 @@ def _run(argv, timeout=1500, **env):
 # count on the host and on the device) against fp64 with its pinned tile, the device-count edges,
 # row masks, N-tile-width invariance, and the dual-softmax passes (column masks, row counts)
 ROW_CHECKS = ["row_gemms_split1", "row_gemms_split0", "row_dyn", "row_masks", "row_launch_invariance",
-              "linear_act", "linear_ln", "linear_q", "linear_act_shared", "sim", "sim_colmax", "sim_lse_cols",
+              "linear_act", "linear_ln", "linear_q", "linear_act_shared", "sim_colmax", "sim_lse_cols",
               "sim_col_mask"]
 FORCED = [(c, "32") for c in ROW_CHECKS] + [("row_gemms_split1", "64"), ("sim_lse_cols", "64")]
 
