@@ -705,6 +705,42 @@ int opp_kpt_train_fwd(const float* kpts, const float* stats, const float* desc, 
 int opp_kpt_train_bwd(const float* kpts, const float* stats, const float* dout, const float* pack, int batch, int n,
                       int row0, int nrows, float* part, float* dparams, int accumulate, opp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Training batch (opp_train_batch.cu): the homography augmentation of the query images and the
+ * ground-truth correspondences projected from the pose (OnePosePlusDataset.read_anno,
+ * src/datasets/OnePosePlus_dataset.py:341-444), fp32 with one rounding per operation.  pack fp32
+ * [B][opp_train_batch_pack_size()] holds each item's R, t, K, the point warp, the pixel
+ * normalisation, the image warp and the warp flag (layout in opp_train_batch.cu).
+ * ---------------------------------------------------------------------------------------- */
+
+int opp_train_batch_pack_size(void);
+
+/* out fp32 [B][h][w]: kornia homography_warp of img fp32 [B][h][w] for the items whose warp flag is
+ * set (bilinear, zero padding, align_corners=False), a copy of img for the others. */
+int opp_homography_warp_f32(const float* img, const float* pack, int batches, int h, int w, float* out,
+                            opp_stream_t stream);
+
+/* The correspondences of B items, flattened: assign int64 [2][n] (2D keypoint, 3D point), item b
+ * owns [offsets[b], offsets[b + 1]) and the 2D keypoints [kp_offsets[b], kp_offsets[b + 1]) of
+ * n_kp; kp3d fp32 [B][rows][3]; img_scale fp32 [B][2] (query_image_scale).  Projects, warps,
+ * rounds to the 8-px grid, keeps the first correspondence per cell and the last writer per 2D
+ * keypoint and writes key int64 [n] = ((b rows + i) cols + j) R + rank (INT64_MAX when dropped,
+ * R = ((w - 1) / 8 + 1) ((h - 1) / 8 + 1)) with its fine location key_xy fp32 [n][2].  Scratch:
+ * cell_owner int32 [B][R], kp_owner int32 [n_kp], rank_of int32 [n], fine fp32 [n][2].
+ * status int32 [2]: [0] error bits (1 cell index == cols or < 0, 2 assign[0] outside the item's
+ * keypoints, 4 assign[1] outside [0, rows)), [1] set by opp_train_gt_compact. */
+int opp_train_gt_build(const float* kp3d, const long long* assign, long long n, const long long* offsets,
+                       const long long* kp_offsets, long long n_kp, const float* pack, const float* img_scale,
+                       int batches, int rows, int h, int w, int w_c, int cols, int* cell_owner, int* kp_owner,
+                       int* rank_of, float* fine, long long* key, float* key_xy, int* status, opp_stream_t stream);
+
+/* From the keys sorted ascending (perm = their positions in key_xy): the last entry of each
+ * (b, i, j) = key / ranks, in order, into b_ids / i_ids / j_ids int64 [n] and fine_xy fp32 [n][2];
+ * status[1] = the number written.  One CTA. */
+int opp_train_gt_compact(const long long* sorted_key, const long long* perm, long long n, const float* key_xy,
+                         int rows, int cols, long long ranks, long long* b_ids, long long* i_ids, long long* j_ids,
+                         float* fine_xy, int* status, opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -788,3 +788,56 @@ def kpt_train_bwd(kpts, stats, dout, pack, row0, nrows, part, dparams, accumulat
         raise ValueError("wgrad partial buffer too small")
     call("opp_kpt_train_bwd", ptr(kpts), ptr(stats), ptr(dout), ptr(pack), B, N, int(row0), int(nrows), ptr(part),
          ptr(dparams), int(accumulate), stream())
+
+
+def homography_warp(image, pack):
+    """query_image fp32 [B, 1, h, w] -> a new tensor: kornia homography_warp (bilinear, zeros,
+    align_corners=False) of the items whose pack warp flag is set, a copy of the others.
+    pack fp32 [B, opp_train_batch_pack_size()] (train_batch._pack)."""
+    _chk(image, torch.float32, "query_image")
+    _chk(pack, torch.float32, "pack")
+    B, C, h, w = image.shape
+    if C != 1 or tuple(pack.shape) != (B, _lib.load().opp_train_batch_pack_size()):
+        raise ValueError(f"homography_warp: image {tuple(image.shape)} / pack {tuple(pack.shape)}")
+    out = torch.empty_like(image)
+    call("opp_homography_warp_f32", ptr(image), ptr(pack), B, h, w, ptr(out), stream())
+    return out
+
+
+def train_gt(kp3d, assign, offsets, kp_offsets, n_kp, pack, img_scale, hw, w_c, S):
+    """The ground-truth list of a training batch from the pose: (b_ids, i_ids, j_ids int64 [n],
+    fine_xy fp32 [n, 2], status int32 [2]) — the first status[1] entries are the list, status[0]
+    holds the error bits of opp_train_gt_build.  Nothing is synchronised here.
+    kp3d fp32 [B, L, 3]; assign int64 [2, n]; offsets / kp_offsets int64 [B + 1] (device);
+    n_kp = kp_offsets[-1] as a host int; img_scale fp32 [B, 2]; hw = (h, w) of the query image."""
+    _chk(kp3d, torch.float32, "keypoints3d")
+    _chk(assign, torch.int64, "assign")
+    _chk(offsets, torch.int64, "offsets")
+    _chk(kp_offsets, torch.int64, "kp_offsets")
+    _chk(pack, torch.float32, "pack")
+    _chk(img_scale, torch.float32, "query_image_scale")
+    B, L, _ = kp3d.shape
+    h, w = hw
+    n = assign.shape[1]
+    if assign.dim() != 2 or assign.shape[0] != 2 or offsets.numel() != B + 1 or kp_offsets.numel() != B + 1:
+        raise ValueError("train_gt: assign must be [2, n] and offsets [B + 1]")
+    if tuple(img_scale.shape) != (B, 2):
+        raise ValueError(f"query_image_scale has shape {tuple(img_scale.shape)}, expected {(B, 2)}")
+    dev, i32 = kp3d.device, torch.int32
+    ranks = ((w - 1) // 8 + 1) * ((h - 1) // 8 + 1)
+    cell_owner = torch.empty(B * ranks, dtype=i32, device=dev)
+    kp_owner = torch.empty(max(int(n_kp), 1), dtype=i32, device=dev)
+    rank_of = torch.empty(n, dtype=i32, device=dev)
+    fine = torch.empty(n, 2, dtype=torch.float32, device=dev)
+    key = torch.empty(n, dtype=torch.int64, device=dev)
+    key_xy = torch.empty(n, 2, dtype=torch.float32, device=dev)
+    status = torch.empty(2, dtype=i32, device=dev)
+    call("opp_train_gt_build", ptr(kp3d), ptr(assign), n, ptr(offsets), ptr(kp_offsets), int(n_kp), ptr(pack),
+         ptr(img_scale), B, L, h, w, int(w_c), int(S), ptr(cell_owner), ptr(kp_owner), ptr(rank_of), ptr(fine),
+         ptr(key), ptr(key_xy), ptr(status), stream())
+    sorted_key, perm = torch.sort(key)          # the one library step: order by (b, i, j, rank)
+    b_ids, i_ids, j_ids = (torch.empty(n, dtype=torch.int64, device=dev) for _ in range(3))
+    fine_xy = torch.empty(n, 2, dtype=torch.float32, device=dev)
+    call("opp_train_gt_compact", ptr(sorted_key), ptr(perm), n, ptr(key_xy), L, int(S), ranks, ptr(b_ids),
+         ptr(i_ids), ptr(j_ids), ptr(fine_xy), ptr(status), stream())
+    return b_ids, i_ids, j_ids, fine_xy, status
