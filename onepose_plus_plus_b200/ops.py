@@ -823,6 +823,8 @@ def train_gt(kp3d, assign, offsets, kp_offsets, n_kp, pack, img_scale, hw, w_c, 
         raise ValueError("train_gt: assign must be [2, n] and offsets [B + 1]")
     if tuple(img_scale.shape) != (B, 2):
         raise ValueError(f"query_image_scale has shape {tuple(img_scale.shape)}, expected {(B, 2)}")
+    if tuple(pack.shape) != (B, _lib.load().opp_train_batch_pack_size()):
+        raise ValueError(f"train_gt: pack has shape {tuple(pack.shape)}")
     dev, i32 = kp3d.device, torch.int32
     ranks = ((w - 1) // 8 + 1) * ((h - 1) // 8 + 1)
     cell_owner = torch.empty(B * ranks, dtype=i32, device=dev)

@@ -233,6 +233,8 @@ def prepare_batch(batch):
     L = kp3d.shape[1]
     h_c, w_c = int(h / COARSE_STRIDE), int(w / COARSE_STRIDE)
     S = h_c * w_c
+    if S == 0:
+        raise ValueError(f"prepare_batch: a {h}x{w} query image has no {COARSE_STRIDE}-px coarse cell")
     pack, hk = _pack(src, h, w)
     dev = img.device
     scale = batch["query_image_scale"].to(torch.float32)

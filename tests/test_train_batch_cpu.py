@@ -113,8 +113,8 @@ def test_prepare_batch_gives_the_reference_list(built, name):
 @needs_ref
 @pytest.mark.parametrize("name", list(CASES))
 def test_cpu_path_equals_the_restatement(built, name):
-    """The torch CPU path of prepare_batch and the NumPy restatement: the same list bit for bit and the
-    same warped images."""
+    """The torch CPU path of prepare_batch and the NumPy restatement: the same list and the same warped
+    images bit for bit."""
     case, ds, refs, items, _ = built[name]
     batch = train_batch.collate(items)
     src = batch["gt_source"]
@@ -128,7 +128,35 @@ def test_cpu_path_equals_the_restatement(built, name):
     for g, wnt in zip((got.b_ids, got.i_ids, got.j_ids, got.fine_xy), want):
         assert np.array_equal(g.numpy(), wnt)
     for b in range(len(src)):
-        assert np.abs(batch["query_image"][b, 0].numpy() - otb.warp_image(img[b, 0].numpy(), packs[b])).max() <= 2e-6
+        assert np.array_equal(batch["query_image"][b, 0].numpy(), otb.warp_image(img[b, 0].numpy(), packs[b]))
+
+
+@pytest.mark.parametrize("name", list(otb.EDGE_CASES))
+def test_cpu_path_on_edge_batches(name):
+    """The torch CPU path and the NumPy restatement on the edge batches of otb.EDGE_CASES: the same
+    list and images bit for bit, or the same ValueError."""
+    batch, expect = otb.edge_batch(name)
+    src = batch["gt_source"]
+    img = batch["query_image"].clone()
+    h, w = img.shape[-2:]
+    packs = [otb.pack_item(src.pose_gt[b], src.K_crop[b], src.homography[b], h, w) for b in range(len(src))]
+    assigns = [src.assign[:, src.offsets[b]:src.offsets[b + 1]].numpy() for b in range(len(src))]
+    args = (batch["keypoints3d"].numpy(), assigns, packs, batch["query_image_scale"].numpy(), (h, w))
+    if expect == "grid size":
+        with pytest.raises(ValueError, match="cell index == S"):
+            otb.batch_list(*args)
+    elif expect is None:
+        want = otb.batch_list(*args)
+    if expect is not None:
+        with pytest.raises(ValueError, match=expect):
+            train_batch.prepare_batch(batch)
+        return
+    train_batch.prepare_batch(batch)
+    got = batch["gt_sparse"].check()
+    for g, wnt in zip((got.b_ids, got.i_ids, got.j_ids, got.fine_xy), want):
+        assert np.array_equal(g.numpy(), wnt)
+    for b in range(len(src)):
+        assert np.array_equal(batch["query_image"][b, 0].numpy(), otb.warp_image(img[b, 0].numpy(), packs[b]))
 
 
 @needs_ref

@@ -40,32 +40,55 @@ def to_cuda(batch):
 
 
 def restated(batch):
-    """(list, images) of the NumPy restatement on a host batch"""
+    """(list, images) of the NumPy restatement on a host batch; the list is the ValueError it raises
+    instead, if it does"""
     src = batch["gt_source"]
     img = batch["query_image"]
     h, w = img.shape[-2:]
     packs = [otb.pack_item(src.pose_gt[b], src.K_crop[b], src.homography[b], h, w) for b in range(len(src))]
     assigns = [src.assign[:, src.offsets[b]:src.offsets[b + 1]].numpy() for b in range(len(src))]
-    lst = otb.batch_list(batch["keypoints3d"].numpy(), assigns, packs, batch["query_image_scale"].numpy(), (h, w))
+    try:
+        lst = otb.batch_list(batch["keypoints3d"].numpy(), assigns, packs, batch["query_image_scale"].numpy(),
+                             (h, w))
+    except ValueError as e:
+        lst = e
     return lst, [otb.warp_image(img[b, 0].numpy(), packs[b]) for b in range(len(src))]
 
 
-def check_against_restatement(batch):
-    (lb, li, lj, lxy), imgs = restated(batch)
+def check_against_restatement(batch, expect=None):
+    """The device path and the restatement: ids equal, fine_xy and the images bit-equal; or, with
+    expect, the ValueError expect names (S = 0: prepare_batch refuses the image up front)."""
+    (lst, imgs) = restated(batch)
+    if expect == "grid size":
+        assert isinstance(lst, ValueError), "the restatement has no cell index at the grid size"
+    elif expect is None:
+        assert not isinstance(lst, ValueError), lst
+    if expect is not None:
+        with pytest.raises(ValueError, match=expect):
+            train_batch.prepare_batch(to_cuda(batch))
+        return None
+    lb, li, lj, lxy = lst
     out = train_batch.prepare_batch(to_cuda(batch))
     got = out["gt_sparse"].check()
     assert np.array_equal(got.b_ids.cpu().numpy(), lb) and np.array_equal(got.i_ids.cpu().numpy(), li)
     assert np.array_equal(got.j_ids.cpu().numpy(), lj)
     assert np.array_equal(got.fine_xy.cpu().numpy(), lxy), "fine_xy differs from the restatement"
     for b, want in enumerate(imgs):
-        assert np.abs(out["query_image"][b, 0].cpu().numpy() - want).max() <= 2e-6, f"image {b}"
+        assert np.array_equal(out["query_image"][b, 0].cpu().numpy(), want), f"image {b}"
     return got
 
 
 @pytest.mark.parametrize("name", ["golden_warp", "golden_exact", "training_shape", "training_shape_scaled",
-                                  "no_correspondence"])
+                                  "no_correspondence", *otb.EDGE_CASES])
 def test_kernels_equal_the_restatement(name):
-    """Contract 1: ids equal, fine_xy bit-equal, warped images within 2e-6."""
+    """Contract 1: ids equal, fine_xy and the images bit-equal; on the edge batches of
+    otb.EDGE_CASES (odd sizes, j == S, scales, contention, rounding edges, sign flips, empty items)
+    the same list or the same ValueError."""
+    if name in otb.EDGE_CASES:
+        batch, expect = otb.edge_batch(name)
+        got = check_against_restatement(batch, expect)
+        print(f"{name}: {'ValueError' if got is None else len(got)}")
+        return
     if name.startswith("golden"):
         batch = batch_from(golden(name.split("_")[1]))
     elif name == "no_correspondence":
