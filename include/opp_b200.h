@@ -741,6 +741,50 @@ int opp_train_gt_compact(const long long* sorted_key, const long long* perm, lon
                          int rows, int cols, long long ranks, long long* b_ids, long long* i_ids, long long* j_ids,
                          float* fine_xy, int* status, opp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Keypoint-free SfM coarse matching (opp_sfm_points.cu): the 2D keypoint merge of
+ * points2D_worker / update_matches / transform_points2D (coarse_match_worker.py:81-175).  The raw
+ * matches of P pairs are fp32 [M][5] (x0, y0, x1, y1, mconf); pair p owns [offsets[p],
+ * offsets[p + 1]) and names the images pair_img int32 [P][2].  Keys are int64 image << 42 | x << 21 | y
+ * of the truncated coordinates: the caller guarantees 0 <= x, y < 2^21, images <= 2^20, mconf >= 0.
+ * ---------------------------------------------------------------------------------------- */
+
+/* key int64 [2M], conf fp32 [2M]: both endpoints of every match at their appearance index
+ * 2 offsets[p] + side * (offsets[p + 1] - offsets[p]) + m. */
+int opp_sfm_points_emit(const float* matches, long long m, const long long* offsets, const int* pair_img,
+                        int pairs, long long* key, float* conf, opp_stream_t stream);
+
+/* Entries of block_scratch (int32) that opp_sfm_points_segments needs for n sorted keys. */
+int opp_sfm_points_segments_scratch(long long n);
+
+/* From the n keys sorted ascending: start int32 [groups + 1] = the first position of each run of
+ * equal keys and n; *groups int32 = the number of runs. */
+int opp_sfm_points_segments(const long long* sorted_key, long long n, int* block_scratch, int* start, int* groups,
+                            opp_stream_t stream);
+
+/* One thread per group: ukey int64 [G] its key, sum fp64 [G] the sequential sum of conf[perm[j]] over
+ * its run, rank_key int64 [G] = -bits(sum), img_off int64 [images + 1] the first group of each image. */
+int opp_sfm_points_sums(const long long* sorted_key, const long long* perm, const float* conf, const int* start,
+                        int groups, int images, long long* ukey, double* sum, long long* rank_key,
+                        long long* img_off, opp_stream_t stream);
+
+/* img_key int64 [G] = the image of group perm1[q] (perm1: the stable sort of rank_key). */
+int opp_sfm_points_image_key(const long long* ukey, const long long* perm1, int groups, long long* img_key,
+                             opp_stream_t stream);
+
+/* q-th keypoint in (image, descending sum, ascending (x, y)) order, g = perm1[perm2[q]]:
+ * kpts fp32 [G][2] = (x, y), scores fp32 [G] = sum rounded to fp32, id_of int64 [G]: id_of[g] =
+ * q - img_off[image]. */
+int opp_sfm_points_rank(const long long* ukey, const double* sum, const long long* img_off, const long long* perm1,
+                        const long long* perm2, int groups, float* kpts, float* scores, long long* id_of,
+                        opp_stream_t stream);
+
+/* idx int64 [M][2] = the keypoint ids of each match's two endpoints; status int32 [1] = 1 when an
+ * endpoint is missing from its image's keys (written -1). */
+int opp_sfm_points_remap(const float* matches, long long m, const long long* offsets, const int* pair_img,
+                         int pairs, const long long* ukey, const long long* img_off, const long long* id_of,
+                         long long* idx, int* status, opp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -99,6 +99,12 @@ SIGNATURES = {
     "opp_homography_warp_f32": [P, P, I, I, I, P, P],
     "opp_train_gt_build": [P, P, L, P, P, L, P, P, I, I, I, I, I, I, P, P, P, P, P, P, P, P],
     "opp_train_gt_compact": [P, P, L, P, I, I, L, P, P, P, P, P, P],
+    "opp_sfm_points_emit": [P, L, P, P, I, P, P, P],
+    "opp_sfm_points_segments": [P, L, P, P, P, P],
+    "opp_sfm_points_sums": [P, P, P, P, I, I, P, P, P, P, P],
+    "opp_sfm_points_image_key": [P, P, I, P, P],
+    "opp_sfm_points_rank": [P, P, P, P, P, I, P, P, P, P],
+    "opp_sfm_points_remap": [P, L, P, P, I, P, P, P, P, P, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),
@@ -113,6 +119,7 @@ PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles"
          "opp_kpt_train_params": ([], c_int),
          "opp_kpt_train_pack_size": ([], c_int),
          "opp_train_batch_pack_size": ([], c_int),
+         "opp_sfm_points_segments_scratch": ([L], c_int),
          "opp_pose_metrics_scratch_bytes": ([I, I], c_longlong),
          "opp_last_error": ([], ctypes.c_char_p)}
 
@@ -158,7 +165,7 @@ KERNELS_PER_CALL = {"opp_match_select_colmax": 3, "opp_match_select_colmax_set":
                     "opp_backbone_train_conv_wgrad": 2, "opp_backbone_train_conv_wgrad_tf32x3": 2,
                     "opp_backbone_train_bn_stats": 2,
                     "opp_backbone_train_bn_act_bwd": 3, "opp_kpt_train_bwd": 2,
-                    "opp_train_gt_build": 3}
+                    "opp_train_gt_build": 3, "opp_sfm_points_segments": 3}
 LAUNCHES = 0
 _PROFILE = None
 

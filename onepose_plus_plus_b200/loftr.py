@@ -115,6 +115,39 @@ class LoFTR_for_OnePose_Plus(_Engine):
             cur0, cur1 = n0, n1
         return cur0, cur1
 
+    def _coarse_select(self, t0, t1, B, hc, wc, H, s0, s1, conf=None):
+        """LoFTR utils/coarse_matching.py:74-107, 133-259 on B pairs of final coarse tokens: the
+        one-pass dual softmax and the mutual-nearest selection (threshold, border on all sides,
+        coordinates times the scales).  conf fp32 [B, S, S] receives the matrix; None skips it.
+        Returns (M, b_ids, i_ids, j_ids, mconf, mkpts0_c, mkpts1_c) trimmed to the M matches (one host
+        sync, for the count)."""
+        dev = t0.device
+        f32, i32 = torch.float32, torch.int32
+        split = self.split
+        S = hc * wc
+        mc = self.config["match_coarse"]
+        scale = 1.0 / (256.0 * mc["dsmax_temperature"])
+        ts = ops.sim_tiles(S)
+        pm, ps = self._buf("pm_pt", (B * S, ts), f32, dev), self._buf("ps_pt", (B * S, ts), f32, dev)
+        lse0, lse1 = self._buf("lse_pt", (B, S), f32, dev), self._buf("lse_px", (B, S), f32, dev)
+        groups = (S + 31) // 32
+        ops.sim_lse_cols(t0, t1, B, S, S, 256, scale, pm, ps, lse0, self._buf("lse_col_m", (B, groups, S), f32, dev),
+                         self._buf("lse_col_s", (B, groups, S), f32, dev), lse1, split)
+        pt_val, pt_idx = self._buf("pt_val", (B, S), f32, dev), self._buf("pt_idx", (B, S), i32, dev)
+        colmax = self._buf("colmax", (B, S), i32, dev)
+        ops.sim_conf_colmax(t0, t1, lse0, lse1, conf, B, S, S, 256, scale, pm, self._buf("pi_pt", (B * S, ts), i32, dev),
+                            pt_val, pt_idx, colmax, split)
+        cap = B * S
+        count = self._buf("match_count", (1,), i32, dev)
+        b_ids, i_ids, j_ids = (torch.empty(cap, dtype=torch.int64, device=dev) for _ in range(3))
+        mconf = torch.empty(cap, dtype=f32, device=dev)
+        mk0, mk1 = torch.empty((cap, 2), dtype=f32, device=dev), torch.empty((cap, 2), dtype=f32, device=dev)
+        ops.match_select_2d(pt_val, pt_idx, colmax, s0, s1, B, hc, wc, hc, wc, mc["thr"], mc["border_rm"],
+                            float(H / hc), self._buf("match_scratch", ((cap + 1023) // 1024 + 2,), i32, dev),
+                            b_ids, i_ids, j_ids, mconf, mk0, mk1, count)
+        M = int(count.item())   # the one host sync (the reference syncs in torch.where)
+        return M, b_ids[:M], i_ids[:M], j_ids[:M], mconf[:M], mk0[:M], mk1[:M]
+
     def _fine_layer(self, L, x, src, G, T, out16, out32=None):
         """LoFTREncoderLayer.forward (d_model 128) on G groups of T tokens: x, src [G*T, pl*128]."""
         dev = x.device
@@ -163,7 +196,7 @@ class LoFTR_for_OnePose_Plus(_Engine):
             self._ensure_plan(dev)
             split = self.split
             pl = 2 if split else 1
-            f16, f32, i32 = torch.float16, torch.float32, torch.int32
+            f16, f32 = torch.float16, torch.float32
             img = torch.cat([im0, im1], 0)
             if img.dtype not in (torch.uint8, torch.float32):
                 img = img.float()
@@ -174,35 +207,13 @@ class LoFTR_for_OnePose_Plus(_Engine):
                          "hw0_c": torch.Size((hc, wc)), "hw1_c": torch.Size((hc, wc)),
                          "hw0_f": torch.Size((hf, wf)), "hw1_f": torch.Size((hf, wf))})
             t0, t1 = self._coarse(tok[:B], tok[B:], B, S, S)
-            # ---- coarse matching (LoFTR utils/coarse_matching.py:74-107, 133-259)
-            mc = self.config["match_coarse"]
-            scale = 1.0 / (256.0 * mc["dsmax_temperature"])
-            ts = ops.sim_tiles(S)
-            pm, ps = self._buf("pm_pt", (B * S, ts), f32, dev), self._buf("ps_pt", (B * S, ts), f32, dev)
-            lse0, lse1 = self._buf("lse_pt", (B, S), f32, dev), self._buf("lse_px", (B, S), f32, dev)
-            groups = (S + 31) // 32
-            ops.sim_lse_cols(t0, t1, B, S, S, 256, scale, pm, ps, lse0, self._buf("lse_col_m", (B, groups, S), f32, dev),
-                             self._buf("lse_col_s", (B, groups, S), f32, dev), lse1, split)
             conf = torch.empty((B, S, S), dtype=f32, device=dev)
-            pt_val, pt_idx = self._buf("pt_val", (B, S), f32, dev), self._buf("pt_idx", (B, S), i32, dev)
-            colmax = self._buf("colmax", (B, S), i32, dev)
-            ops.sim_conf_colmax(t0, t1, lse0, lse1, conf, B, S, S, 256, scale, pm, self._buf("pi_pt", (B * S, ts), i32, dev),
-                                pt_val, pt_idx, colmax, split)
-            cap = B * S
-            count = self._buf("match_count", (1,), i32, dev)
-            b_ids, i_ids, j_ids = (torch.empty(cap, dtype=torch.int64, device=dev) for _ in range(3))
-            mconf = torch.empty(cap, dtype=f32, device=dev)
-            mk0, mk1 = torch.empty((cap, 2), dtype=f32, device=dev), torch.empty((cap, 2), dtype=f32, device=dev)
             s0 = data["scale0"].to(device=dev, dtype=f32).contiguous() if "scale0" in data else None
             s1 = data["scale1"].to(device=dev, dtype=f32).contiguous() if "scale1" in data else None
-            ops.match_select_2d(pt_val, pt_idx, colmax, s0, s1, B, hc, wc, hc, wc, mc["thr"], mc["border_rm"],
-                                float(H / hc), self._buf("match_scratch", ((cap + 1023) // 1024 + 2,), i32, dev),
-                                b_ids, i_ids, j_ids, mconf, mk0, mk1, count)
-            M = int(count.item())   # the one host sync (the reference syncs in torch.where)
-            b_ids, i_ids, j_ids = b_ids[:M], i_ids[:M], j_ids[:M]
+            M, b_ids, i_ids, j_ids, mconf, mk0, mk1 = self._coarse_select(t0, t1, B, hc, wc, H, s0, s1, conf)
             data.update({"conf_matrix": conf, "b_ids": b_ids, "i_ids": i_ids, "j_ids": j_ids,
                          "gt_mask": torch.zeros(M, dtype=torch.bool, device=dev), "m_bids": b_ids,
-                         "mkpts0_c": mk0[:M], "mkpts1_c": mk1[:M], "mconf": mconf[:M]})
+                         "mkpts0_c": mk0, "mkpts1_c": mk1, "mconf": mconf})
             if not self.enable_fine_matching:
                 data.update({"mkpts0_f": data["mkpts0_c"], "mkpts1_f": data["mkpts1_c"]})
                 return
@@ -237,3 +248,73 @@ class LoFTR_for_OnePose_Plus(_Engine):
             mk1f = torch.empty((M, 2), dtype=f32, device=dev)
             ops.fine_match_2d(x32, data["mkpts1_c"], b_ids, s1, expec_f, mk1f, M, self.W, float(H / hf))
             data.update({"expec_f": expec_f, "mkpts0_f": data["mkpts0_c"], "mkpts1_f": mk1f})
+
+    # ------------------------------------------------------------------ SfM coarse matching
+    def image_tokens(self, images_u8, image_chunk=16):
+        """The coarse tokens of N images, each image once: conv1 .. layer3 and layer3_outconv with the
+        position-encoding epilogue, bit-equal to the tokens forward() computes for the same image.
+        The FPN branches that only the fine level reads are skipped.  images_u8 uint8 [N, 1, H, W] on
+        the device; the backbone runs on `image_chunk` images at a time, so its workspace stays that
+        of one chunk.  Returns (fp16 planes [N, S, pl*256], (hc, wc))."""
+        N, _, H, W = images_u8.shape
+        dev = images_u8.device
+        self._ensure_plan(dev)
+        hc, wc = H // 8, W // 8
+        store = torch.empty((N, hc * wc, (2 if self.split else 1) * 256), dtype=torch.float16, device=dev)
+        for c0 in range(0, N, image_chunk):
+            tok, _, _ = self._backbone(images_u8[c0:c0 + image_chunk].contiguous(), coarse_only=True)
+            store[c0:c0 + image_chunk].copy_(tok)
+        return store, (hc, wc)
+
+    @torch.no_grad()
+    def coarse_matches_for_pairs(self, images_u8, scales, pair_idx, pair_batch=32, image_chunk=16):
+        """Coarse-only matching of many pairs over one image set (the keypoint-free SfM coarse match,
+        coarse_match_worker.py:44-76): the backbone once per image (image_tokens), then the coarse
+        transformer, the dual softmax and the selection on `pair_batch` pairs at a time, without the
+        confidence matrix.  One host sync per pair batch, for its match count.
+        images_u8 uint8 [N, 1, H, W] (CUDA), scales fp32 [N, 2] (the per-image scale0 / scale1),
+        pair_idx int64 [P, 2] (image indices).  Returns a dict of device tensors over all pairs, in
+        pair order and within a pair in (i) order as forward() gives them: b_ids (the pair index),
+        i_ids, j_ids, mkpts0_c, mkpts1_c, mconf, and offsets int64 [P + 1] (host) delimiting the
+        pairs."""
+        if self.training:
+            raise NotImplementedError("LoFTR_for_OnePose_Plus is the inference matcher: call .eval()")
+        if not (torch.is_tensor(images_u8) and images_u8.is_cuda and images_u8.dtype == torch.uint8):
+            raise TypeError("images_u8 must be a uint8 CUDA tensor [N, 1, H, W]")
+        N, C, H, W = images_u8.shape
+        if C != 1 or H % 8 or W % 8 or H < 48 or W < 48:
+            raise ValueError(f"images must be [N, 1, H, W] with H, W multiples of 8 (>= 48), got {tuple(images_u8.shape)}")
+        pair_idx = torch.as_tensor(pair_idx, dtype=torch.int64).reshape(-1, 2)
+        if tuple(scales.shape) != (N, 2):
+            raise ValueError(f"scales must be [N, 2] = [{N}, 2], got {tuple(scales.shape)}")
+        if pair_idx.numel() and (int(pair_idx.min()) < 0 or int(pair_idx.max()) >= N):
+            raise ValueError("pair_idx names an image outside [0, N)")
+        if pair_batch < 1:
+            raise ValueError("pair_batch must be >= 1")
+        with torch.cuda.device(images_u8.device):
+            dev = images_u8.device
+            store, (hc, wc) = self.image_tokens(images_u8, image_chunk)
+            S = hc * wc
+            scales = scales.to(device=dev, dtype=torch.float32)
+            pidx = pair_idx.to(dev)
+            P = pair_idx.shape[0]
+            out = {k: [] for k in ("b_ids", "i_ids", "j_ids", "mkpts0_c", "mkpts1_c", "mconf")}
+            counts = []
+            for p0 in range(0, P, pair_batch):
+                idx = pidx[p0:p0 + pair_batch]
+                B = idx.shape[0]
+                t0, t1 = self._coarse(store[idx[:, 0]], store[idx[:, 1]], B, S, S)
+                s0, s1 = scales[idx[:, 0]].contiguous(), scales[idx[:, 1]].contiguous()
+                M, b_ids, i_ids, j_ids, mconf, mk0, mk1 = self._coarse_select(t0, t1, B, hc, wc, H, s0, s1)
+                for k, v in zip(out, (b_ids + p0, i_ids, j_ids, mk0, mk1, mconf)):
+                    out[k].append(v)
+                counts.append(torch.bincount(b_ids, minlength=B).cpu() if M else torch.zeros(B, dtype=torch.int64))
+            res = {k: torch.cat(v) if v else torch.empty((0, 2) if k.startswith("mkpts") else (0,),
+                                                          dtype=torch.float32 if k[0] == "m" else torch.int64,
+                                                          device=dev)
+                   for k, v in out.items()}
+            offsets = torch.zeros(P + 1, dtype=torch.int64)
+            if P:
+                torch.cumsum(torch.cat(counts), 0, out=offsets[1:])
+            res["offsets"] = offsets
+            return res

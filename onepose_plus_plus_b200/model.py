@@ -432,13 +432,14 @@ class _Engine(nn.Module):
         return sum(e[0].numel() for e in self._ws.values())
 
     # ------------------------------------------------------------------ stages
-    def _backbone(self, img, defer_fine=False, fpn_stream=None):
+    def _backbone(self, img, defer_fine=False, fpn_stream=None, coarse_only=False):
         """ResNetFPN_8_2.forward (backbone/resnet.py:141-164) -> coarse tokens (+pe), fine map.
         defer_fine: stop before layer1_outconv2 and return its input (the merged 1/2-resolution
         map) instead of the fine map; the caller finishes with _fine_head_dense or, when the
         matches are few, _fine_head_windows.  fpn_stream (latency mode): the top-down path below
         the coarse output — which nothing needs before the fine stage — is enqueued on that stream
-        so that it runs beside the coarse transformer; the caller joins it before the fine head."""
+        so that it runs beside the coarse transformer; the caller joins it before the fine head.
+        coarse_only: stop after the coarse tokens (the fine map is None)."""
         P = self._plan
         dev = img.device
         B, _, H, W = img.shape
@@ -468,6 +469,9 @@ class _Engine(nn.Module):
         S = hc * wc
         tok = self._buf("q2_0", (B, S, pl * 256), f16, dev)
         x3_out = cv("layer3_outconv", x3, "x3_out", 1, 1, tok=tok, pe=self._pe_tokens(hc, wc, dev))
+        if coarse_only:
+            return tok, None, (hc, wc)
+
         def top_down():
             # FPN top-down merge fused into the lateral 1x1 conv epilogue (resnet.py:149-157)
             x2_lat = cv("layer2_outconv", x2, "x2_lat", 1, 1, up=x3_out)

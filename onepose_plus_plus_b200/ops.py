@@ -843,3 +843,69 @@ def train_gt(kp3d, assign, offsets, kp_offsets, n_kp, pack, img_scale, hw, w_c, 
     call("opp_train_gt_compact", ptr(sorted_key), ptr(perm), n, ptr(key_xy), L, int(S), ranks, ptr(b_ids),
          ptr(i_ids), ptr(j_ids), ptr(fine_xy), ptr(status), stream())
     return b_ids, i_ids, j_ids, fine_xy, status
+
+
+SFM_XY_LIMIT = 1 << 21      # the key packs x and y in 21 bits each and the image id in 20
+SFM_MAX_IMAGES = 1 << 20
+
+
+def sfm_points(matches, offsets, pair_img, images):
+    """The 2D keypoint merge of the SfM coarse matching (opp_sfm_points.cu) over all pairs at once.
+    matches fp32 [M, 5] (x0, y0, x1, y1, mconf) of P pairs in order; offsets int64 [P + 1] and
+    pair_img int32 [P, 2] (image ids < images) on the device.  Returns (kpts fp32 [G, 2], scores
+    fp32 [G], img_off int64 [images + 1], idx int64 [M, 2], status int32 [1]): image i's keypoints
+    are kpts[img_off[i]:img_off[i + 1]] in id order, idx holds each match's two ids and status is
+    non-zero when an endpoint was not found (it cannot be, for valid input).  Raises ValueError, before
+    any launch, for coordinates the key cannot pack (outside [0, 2^21) or not finite), a negative or
+    non-finite mconf, an image id outside [0, images) or offsets that do not partition the matches."""
+    _chk(matches, torch.float32, "matches")
+    _chk(offsets, torch.int64, "offsets")
+    _chk(pair_img, torch.int32, "pair_img")
+    P = pair_img.shape[0]
+    M = matches.shape[0]
+    if matches.dim() != 2 or matches.shape[1] != 5 or pair_img.dim() != 2 or pair_img.shape[1] != 2 \
+            or tuple(offsets.shape) != (P + 1,):
+        raise ValueError(f"sfm_points: matches {tuple(matches.shape)}, offsets {tuple(offsets.shape)}, "
+                         f"pair_img {tuple(pair_img.shape)}")
+    if P == 0 or M == 0 or not 0 < images <= SFM_MAX_IMAGES or 2 * M >= 2 ** 31:
+        raise ValueError(f"sfm_points: P={P}, M={M}, images={images} outside the built range")
+    xy, conf = matches[:, :4], matches[:, 4]
+    ok = torch.stack([(xy >= 0).all(), (xy < SFM_XY_LIMIT).all(), (conf >= 0).all(), torch.isfinite(conf).all(),
+                      (pair_img >= 0).all(), (pair_img < images).all(), offsets[0] == 0, offsets[-1] == M,
+                      (offsets[1:] >= offsets[:-1]).all()])
+    if not bool(ok.all()):
+        names = ("x, y >= 0", f"x, y < {SFM_XY_LIMIT}", "mconf >= 0", "mconf finite", "image ids >= 0",
+                 f"image ids < {images}", "offsets[0] == 0", f"offsets[-1] == {M}", "offsets ascending")
+        bad = [n for n, v in zip(names, ok.tolist()) if not v]
+        raise ValueError(f"sfm_points: input violates {', '.join(bad)}")
+    dev, i32, i64 = matches.device, torch.int32, torch.int64
+    n = 2 * M
+    key = torch.empty(n, dtype=i64, device=dev)
+    conf2 = torch.empty(n, dtype=torch.float32, device=dev)
+    call("opp_sfm_points_emit", ptr(matches), M, ptr(offsets), ptr(pair_img), P, ptr(key), ptr(conf2), stream())
+    sorted_key, perm = torch.sort(key, stable=True)     # library step: groups keep their appearance order
+    scratch = torch.empty(_lib.load().opp_sfm_points_segments_scratch(n), dtype=i32, device=dev)
+    start = torch.empty(n + 1, dtype=i32, device=dev)
+    groups = torch.empty(1, dtype=i32, device=dev)
+    call("opp_sfm_points_segments", ptr(sorted_key), n, ptr(scratch), ptr(start), ptr(groups), stream())
+    G = int(groups.item())
+    ukey, rank_key = torch.empty(G, dtype=i64, device=dev), torch.empty(G, dtype=i64, device=dev)
+    sums = torch.empty(G, dtype=torch.float64, device=dev)
+    img_off = torch.empty(images + 1, dtype=i64, device=dev)
+    call("opp_sfm_points_sums", ptr(sorted_key), ptr(perm), ptr(conf2), ptr(start), G, int(images), ptr(ukey),
+         ptr(sums), ptr(rank_key), ptr(img_off), stream())
+    del key, sorted_key, perm, conf2, start, scratch
+    _, perm1 = torch.sort(rank_key, stable=True)        # descending sum; ties keep ascending (x, y)
+    img_key = torch.empty(G, dtype=i64, device=dev)
+    call("opp_sfm_points_image_key", ptr(ukey), ptr(perm1), G, ptr(img_key), stream())
+    _, perm2 = torch.sort(img_key, stable=True)         # then by image, keeping that order
+    kpts = torch.empty(G, 2, dtype=torch.float32, device=dev)
+    scores = torch.empty(G, dtype=torch.float32, device=dev)
+    id_of = torch.empty(G, dtype=i64, device=dev)
+    call("opp_sfm_points_rank", ptr(ukey), ptr(sums), ptr(img_off), ptr(perm1), ptr(perm2), G, ptr(kpts),
+         ptr(scores), ptr(id_of), stream())
+    idx = torch.empty(M, 2, dtype=i64, device=dev)
+    status = torch.empty(1, dtype=i32, device=dev)
+    call("opp_sfm_points_remap", ptr(matches), M, ptr(offsets), ptr(pair_img), P, ptr(ukey), ptr(img_off), ptr(id_of),
+         ptr(idx), ptr(status), stream())
+    return kpts, scores, img_off, idx, status
