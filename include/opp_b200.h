@@ -337,6 +337,12 @@ int opp_fine_gather_2d(const void* fine0, const void* fine1, const long long* b_
                        const long long* j_ids, void* x16, int m, int hf0, int wf0, int wc0, int hf1, int wf1,
                        int wc1, int stride, int window, int split, opp_stream_t stream);
 
+/* opp_fine_gather_2d over one store of many images' fine maps, fine NHWC fp16 [N][hf][wf][planes*128]:
+ * match m reads image img0[m]'s map for seq 0 and image img1[m]'s for seq 1 (both sides one size). */
+int opp_fine_gather_2d_images(const void* fine, const long long* img0, const long long* img1, const long long* i_ids,
+                              const long long* j_ids, void* x16, int m, int hf, int wf, int wc, int stride,
+                              int window, int split, opp_stream_t stream);
+
 /* LinearAttention.forward (linear_attention.py:29-61) between small token groups, 8 heads x 16:
  * group g: q fp16 [g][l][planes*128] = elu(q_proj x)+1, kv fp16 [g][s][planes*256] =
  * (elu(k_proj src)+1 | v_proj src); out like q. */
@@ -784,6 +790,33 @@ int opp_sfm_points_rank(const long long* ukey, const double* sum, const long lon
 int opp_sfm_points_remap(const float* matches, long long m, const long long* offsets, const int* pair_img,
                          int pairs, const long long* ukey, const long long* img_off, const long long* id_of,
                          long long* idx, int* status, opp_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Keypoint-free SfM refinement (opp_sfm_refine.cu): feature sampling at keypoints and the track
+ * feature aggregation of feature_aggregation_and_update (post_optimization/feature_aggregation.py).
+ * ---------------------------------------------------------------------------------------- */
+
+/* sample_feature_from_featuremap (loftr_for_sfm/utils/sample_feature_from_featuremap.py) at n
+ * keypoints kpts [n][2] (x, y; fp64 when kpts_f64, else fp32) of images img int64 [n] (NULL: image 0)
+ * in map NHWC fp16 [N][hm][wm][planes*channels] (hi plane, then lo plane when split).  imghw fp32
+ * [N][2] = (h, w) of each image in pixels times its scale.  grid_sample(align_corners=True, zeros
+ * padding), nearest (round half to even) when `nearest`, else bilinear.  out fp32 [n][channels]. */
+int opp_sample_feature(const void* map, const long long* img, const void* kpts, int kpts_f64, long long n, int hm,
+                       int wm, int channels, int split, const float* imghw, int nearest, float* out,
+                       opp_stream_t stream);
+
+/* row int64 [q]: for each query key, perm[j] where sorted_key[j] is its only occurrence among the n
+ * sorted keys; -1 when the key is absent, -2 when it occurs more than once. */
+int opp_sfm_refine_lookup(const long long* sorted_key, const long long* perm, long long n, const long long* query,
+                          long long q, long long* row, opp_stream_t stream);
+
+/* Track t owns members [track_off[t], track_off[t + 1]) (at least one), member k reads row[k]:
+ * mean_c fp32 [T][dc] = the fp32 sum of c0[row[k]] in member order divided by the count (np.mean
+ * of the stacked rows), mean_f [T][df] the same over f0; ref_c fp32 [K][dc] = c1[row[k]], ref_f
+ * [K][df] = f1[row[k]]. */
+int opp_sfm_refine_aggregate(const float* c0, const float* c1, const float* f0, const float* f1, int dc, int df,
+                             const long long* row, const long long* track_off, int tracks, float* mean_c,
+                             float* mean_f, float* ref_c, float* ref_f, opp_stream_t stream);
 
 #ifdef __cplusplus
 }

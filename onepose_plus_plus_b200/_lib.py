@@ -105,6 +105,10 @@ SIGNATURES = {
     "opp_sfm_points_image_key": [P, P, I, P, P],
     "opp_sfm_points_rank": [P, P, P, P, P, I, P, P, P, P],
     "opp_sfm_points_remap": [P, L, P, P, I, P, P, P, P, P, P],
+    "opp_fine_gather_2d_images": [P, P, P, P, P, P, I, I, I, I, I, I, I, P],
+    "opp_sample_feature": [P, P, P, I, L, I, I, I, I, P, I, P, P],
+    "opp_sfm_refine_lookup": [P, P, L, P, L, P, P],
+    "opp_sfm_refine_aggregate": [P, P, P, P, I, I, P, P, I, P, P, P, P, P],
 }
 PLAIN = {"opp_version": ([], c_int), "opp_num_sms": ([], c_int), "opp_sim_tiles": ([I], c_int),
          "opp_kv_chunks": ([I], c_int),

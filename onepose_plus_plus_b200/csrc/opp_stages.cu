@@ -1010,11 +1010,12 @@ match_scatter_2d_kernel(const float* pt_val, const int* pt_idx, const unsigned* 
 // row (seq * M + m) * WW + ww;  seq 0 = image 0's window centred on cell i, seq 1 = image 1's on j.
 __global__ void __launch_bounds__(128) fine_gather_2d_kernel(
     const __half* __restrict__ f0, const __half* __restrict__ f1, const long long* __restrict__ b_ids,
-    const long long* __restrict__ i_ids, const long long* __restrict__ j_ids, __half* __restrict__ x16,
-    int M, int hf0, int wf0, int wc0, int hf1, int wf1, int wc1, int stride, int W, int lo_off) {
+    const long long* __restrict__ b1_ids, const long long* __restrict__ i_ids, const long long* __restrict__ j_ids,
+    __half* __restrict__ x16, int M, int hf0, int wf0, int wc0, int hf1, int wf1, int wc1, int stride, int W,
+    int lo_off) {
   pdl_sync();
   const int m = blockIdx.x, seq = blockIdx.y, c = threadIdx.x;
-  const long long b = b_ids[m];
+  const long long b = seq ? b1_ids[m] : b_ids[m];   // map index of this side's image
   const long long cell = seq ? j_ids[m] : i_ids[m];
   const int wc = seq ? wc1 : wc0, hf = seq ? hf1 : hf0, wf = seq ? wf1 : wf0;
   const int cy = (int)(cell / wc), cx = (int)(cell - (long long)cy * wc);
@@ -1457,8 +1458,21 @@ int opp_fine_gather_2d(const void* fine0, const void* fine1, const long long* b_
   OPP_REQUIRE(fine0 && fine1 && b_ids && i_ids && j_ids && x16, "null pointer");
   OPP_REQUIRE(window % 2 == 1 && window >= 1 && window <= 9, "window %d unsupported (odd, <= 9)", window);
   OPP_CHECK_CUDA(opp::launch_pdl(fine_gather_2d_kernel, dim3(dim3(m, 2)), dim3(128), 0, (cudaStream_t)stream, 
-      (const __half*)fine0, (const __half*)fine1, b_ids, i_ids, j_ids, (__half*)x16, m, hf0, wf0, wc0, hf1, wf1,
-      wc1, stride, window, split ? 128 : 0));
+      (const __half*)fine0, (const __half*)fine1, b_ids, b_ids, i_ids, j_ids, (__half*)x16, m, hf0, wf0, wc0, hf1,
+      wf1, wc1, stride, window, split ? 128 : 0));
+  OPP_CHECK_CUDA(cudaGetLastError());
+  return OPP_OK;
+}
+
+int opp_fine_gather_2d_images(const void* fine, const long long* img0, const long long* img1, const long long* i_ids,
+                              const long long* j_ids, void* x16, int m, int hf, int wf, int wc, int stride,
+                              int window, int split, opp_stream_t stream) {
+  if (m == 0) return OPP_OK;
+  OPP_REQUIRE(fine && img0 && img1 && i_ids && j_ids && x16, "null pointer");
+  OPP_REQUIRE(window % 2 == 1 && window >= 1 && window <= 9, "window %d unsupported (odd, <= 9)", window);
+  OPP_CHECK_CUDA(opp::launch_pdl(fine_gather_2d_kernel, dim3(dim3(m, 2)), dim3(128), 0, (cudaStream_t)stream,
+      (const __half*)fine, (const __half*)fine, img0, img1, i_ids, j_ids, (__half*)x16, m, hf, wf, wc, hf, wf, wc,
+      stride, window, split ? 128 : 0));
   OPP_CHECK_CUDA(cudaGetLastError());
   return OPP_OK;
 }

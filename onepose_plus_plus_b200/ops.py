@@ -909,3 +909,67 @@ def sfm_points(matches, offsets, pair_img, images):
     call("opp_sfm_points_remap", ptr(matches), M, ptr(offsets), ptr(pair_img), P, ptr(ukey), ptr(img_off), ptr(id_of),
          ptr(idx), ptr(status), stream())
     return kpts, scores, img_off, idx, status
+
+
+# ---- keypoint-free SfM refinement (opp_sfm_refine.cu; used by loftr.py and sfm_refine.py) ---------
+
+def fine_gather_2d_images(fine, img0, img1, i_ids, j_ids, x16, m, hf, wf, wc, stride, window, split):
+    """fine_gather_2d over a store of many images' fine maps: match m reads image img0[m] / img1[m]."""
+    _chk(fine, torch.float16, "fine")
+    for name, t in (("img0", img0), ("img1", img1), ("i_ids", i_ids), ("j_ids", j_ids)):
+        _chk(t, torch.int64, name)
+    call("opp_fine_gather_2d_images", ptr(fine), ptr(img0), ptr(img1), ptr(i_ids), ptr(j_ids), ptr(x16), m, hf, wf,
+         wc, stride, window, int(split), stream())
+
+
+def sample_feature(fmap, channels, split, kpts, imghw, nearest, img=None, out=None):
+    """sample_feature_from_featuremap at kpts [n, 2] (fp32 or fp64, on the device) from the engine's
+    NHWC fp16 map store [N, h, w, planes*channels]; img int64 [n] names each point's image (None:
+    image 0), imghw fp32 [N, 2] = (h, w) * scale per image.  Returns fp32 [n, channels]."""
+    _chk(fmap, torch.float16, "map")
+    if kpts.dtype not in (torch.float32, torch.float64) or not kpts.is_cuda or not kpts.is_contiguous():
+        raise TypeError("kpts must be a contiguous fp32 or fp64 CUDA tensor")
+    _chk(imghw, torch.float32, "imghw")
+    _chk(img, torch.int64, "img")
+    N, hm, wm, C = fmap.shape
+    if C != (2 if split else 1) * channels or kpts.dim() != 2 or kpts.shape[1] != 2 or tuple(imghw.shape) != (N, 2):
+        raise ValueError(f"sample_feature: map {tuple(fmap.shape)}, kpts {tuple(kpts.shape)}, imghw {tuple(imghw.shape)}")
+    n = kpts.shape[0]
+    if out is None:
+        out = torch.empty((n, channels), dtype=torch.float32, device=kpts.device)
+    call("opp_sample_feature", ptr(fmap), ptr(img), ptr(kpts), int(kpts.dtype == torch.float64), n, hm, wm, channels,
+         int(split), ptr(imghw), int(bool(nearest)), ptr(out), stream())
+    return out
+
+
+def sfm_refine_lookup(row_key, query):
+    """row int64 [q]: the position in row_key (int64 [n]) of each query key, -1 when absent, -2 when the
+    key occurs more than once."""
+    _chk(row_key, torch.int64, "row_key")
+    _chk(query, torch.int64, "query")
+    row = torch.empty(query.shape[0], dtype=torch.int64, device=query.device)
+    if query.shape[0] == 0:
+        return row
+    if row_key.shape[0] == 0:
+        return row.fill_(-1)
+    sorted_key, perm = torch.sort(row_key)     # library step, as in sfm_points
+    call("opp_sfm_refine_lookup", ptr(sorted_key), ptr(perm), row_key.shape[0], ptr(query), query.shape[0], ptr(row),
+         stream())
+    return row
+
+
+def sfm_refine_aggregate(c0, c1, f0, f1, row, track_off):
+    """Track means and reference-side gathers of feature_aggregation_and_update: c0, c1 fp32 [R, dc],
+    f0, f1 fp32 [R, df]; row int64 [K] (member -> row), track_off int64 [T + 1].  Returns (mean_c
+    [T, dc], mean_f [T, df], ref_c [K, dc], ref_f [K, df])."""
+    for name, t in (("c0", c0), ("c1", c1), ("f0", f0), ("f1", f1)):
+        _chk(t, torch.float32, name)
+    _chk(row, torch.int64, "row")
+    _chk(track_off, torch.int64, "track_off")
+    T, K, dc, df = track_off.shape[0] - 1, row.shape[0], c0.shape[1], f0.shape[1]
+    dev = row.device
+    mean_c, mean_f = torch.empty((T, dc), device=dev), torch.empty((T, df), device=dev)
+    ref_c, ref_f = torch.empty((K, dc), device=dev), torch.empty((K, df), device=dev)
+    call("opp_sfm_refine_aggregate", ptr(c0), ptr(c1), ptr(f0), ptr(f1), dc, df, ptr(row), ptr(track_off), T,
+         ptr(mean_c), ptr(mean_f), ptr(ref_c), ptr(ref_f), stream())
+    return mean_c, mean_f, ref_c, ref_f
