@@ -632,10 +632,13 @@ int opp_coarse_tf_ln_bwd(const float* x, int ldx, const float* gamma, const floa
 
 /* ------------------------------------------------------------------------------------------
  * Training, backbone (opp_train_backbone.cu): the ResNet-FPN's convolutions, batch-statistics
- * BatchNorm + activation (+ residual) and the FPN's bilinear x2 upsample-add, forward and backward,
- * fp32 on the CUDA cores.  Maps are NCHW fp32; weights [c_out][c_in][k][k]; k in {1, 3, 7},
- * stride in {1, 2}, pad = k / 2; (h, w) is the convolution's input size.  Every sum runs in a fixed
- * order without floating-point atomics: results are bit-reproducible.
+ * BatchNorm + activation (+ residual) and the FPN's bilinear x2 upsample-add, forward and backward.
+ * The convolutions run on the tensor cores in 3xTF32: each operand is split into tf32 hi + lo and
+ * every k8 step sums lo·hi, hi·lo and hi·hi in fp32, so each product is within 3.01·2^-22 |a b| of
+ * a·b before the fp32 accumulation (DESIGN §7 f4).  The rest is fp32.  Maps are NCHW fp32; weights
+ * [c_out][c_in][k][k]; k in {1, 3, 7}, stride in {1, 2}, pad = k / 2; (h, w) is the convolution's
+ * input size.  Every sum runs in a fixed order without floating-point atomics: results are
+ * bit-reproducible.
  * ---------------------------------------------------------------------------------------- */
 
 /* Output pixels per weight-gradient partial; BatchNorm partials of a [batches][c][hw] map per channel. */
@@ -653,17 +656,6 @@ int opp_backbone_train_conv_dgrad(const float* dy, const float* w, int batches, 
 int opp_backbone_train_conv_wgrad(const float* x, const float* dy, int batches, int c_in, int h, int wd, int c_out,
                                   int ksize, int stride, int pix0, int npix, float* part, float* dw, int accumulate,
                                   opp_stream_t stream);
-/* The same three passes on the tensor cores in 3xTF32 (opp_train_backbone_tc.cu): each operand is split
- * into tf32 hi + lo and every k8 step sums lo·hi, hi·lo and hi·hi in fp32.  Arguments as above; the
- * weight gradient uses the same group (opp_backbone_train_wgrad_group) and partial buffer. */
-int opp_backbone_train_conv_tf32x3(const float* x, const float* w, int batches, int c_in, int h, int wd, int c_out,
-                                   int ksize, int stride, float* y, opp_stream_t stream);
-int opp_backbone_train_conv_dgrad_tf32x3(const float* dy, const float* w, int batches, int c_in, int h, int wd,
-                                         int c_out, int ksize, int stride, float* dx, int accumulate,
-                                         opp_stream_t stream);
-int opp_backbone_train_conv_wgrad_tf32x3(const float* x, const float* dy, int batches, int c_in, int h, int wd,
-                                         int c_out, int ksize, int stride, int pix0, int npix, float* part,
-                                         float* dw, int accumulate, opp_stream_t stream);
 /* mean / invstd [c] of x [batches][c][hw] over batches * hw values (biased variance); when
  * running_mean / running_var are given they are updated as F.batch_norm does (unbiased variance).
  * part fp64 [c][parts][2]. */

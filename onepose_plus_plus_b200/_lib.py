@@ -86,9 +86,6 @@ SIGNATURES = {
     "opp_backbone_train_conv": [P, P, I, I, I, I, I, I, I, P, P],
     "opp_backbone_train_conv_dgrad": [P, P, I, I, I, I, I, I, I, P, I, P],
     "opp_backbone_train_conv_wgrad": [P, P, I, I, I, I, I, I, I, I, I, P, P, I, P],
-    "opp_backbone_train_conv_tf32x3": [P, P, I, I, I, I, I, I, I, P, P],
-    "opp_backbone_train_conv_dgrad_tf32x3": [P, P, I, I, I, I, I, I, I, P, I, P],
-    "opp_backbone_train_conv_wgrad_tf32x3": [P, P, I, I, I, I, I, I, I, I, I, P, P, I, P],
     "opp_backbone_train_bn_stats": [P, I, I, I, F, P, P, P, P, P, F, P],
     "opp_backbone_train_bn_act": [P, I, I, I, P, P, P, P, P, I, P, P],
     "opp_backbone_train_bn_act_bwd": [P, P, P, I, I, I, P, P, P, I, I, P, P, P, P, P],
@@ -166,7 +163,7 @@ KERNELS_PER_CALL = {"opp_match_select_colmax": 3, "opp_match_select_colmax_set":
                     "opp_gt_index": 5, "opp_coarse_focal_fwd_sparse": 3, "opp_coarse_focal_bwd_sparse": 2,
                     "opp_fine_train_wgrad": 2, "opp_fine_train_ln_bwd": 2,
                     "opp_coarse_tf_kv": 2, "opp_coarse_tf_attn_bwd_q": 2, "opp_coarse_tf_ln_bwd": 2,
-                    "opp_backbone_train_conv_wgrad": 2, "opp_backbone_train_conv_wgrad_tf32x3": 2,
+                    "opp_backbone_train_conv_wgrad": 2,
                     "opp_backbone_train_bn_stats": 2,
                     "opp_backbone_train_bn_act_bwd": 3, "opp_kpt_train_bwd": 2,
                     "opp_train_gt_build": 3, "opp_sfm_points_segments": 3}

@@ -1,15 +1,25 @@
 // opp_train_backbone.cu — the ResNet-FPN backbone of training on the device: convolution forward,
-// data gradient and weight gradient, batch-statistics BatchNorm with its activation and residual, and
-// the FPN's bilinear x2 upsample-add, forward and backward, fp32 on the CUDA cores (DESIGN §7 f4).
+// data gradient and weight gradient on the tensor cores in 3xTF32, batch-statistics BatchNorm with its
+// activation and residual, and the FPN's bilinear x2 upsample-add, forward and backward (DESIGN §7 f4).
 //
 // Activations are NCHW fp32.  Weights are [C_out][C_in][k][k] (nn.Conv2d's layout), pad = k / 2.
 // The three convolution passes are one implicit GEMM with operands gathered straight from the maps:
-//   forward  out[p][co]    = sum_{ci,tap} x(p, ci, tap)       W[co][ci][tap]      (p: output pixel)
-//   dgrad    dx[q][ci]     = sum_{co,tap} dy(q, co, tap)      W[co][ci][tap]      (q: input pixel)
-//   wgrad    dW[co][ci,tap] = sum_p       dy[p][co]           x(p, ci, tap)
+//   forward  out[p][co]     = sum_{ci,tap} x(p, ci, tap)  W[co][ci][tap]     M = output pixels, N = c_out
+//   dgrad    dx[q][ci]      = sum_{co,tap} dy(q, co, tap) W[co][ci][tap]     M = input pixels,  N = c_in
+//   wgrad    dW[co][ci,tap] = sum_p        dy[p][co]      x(p, ci, tap)      M = c_out, N = c_in·k², K = pixels
 // where x(p, ci, tap) is the input the tap reads for output pixel p (0 outside the map) and
 // dy(q, co, tap) the output-gradient pixel whose tap reads input pixel q: for stride 2 a tap
 // contributes only where (i + pad - k_y) is even and (i + pad - k_y) / 2 is in range.
+//
+// Each gathered value v is split into tf32 hi = rna(v) and lo = rna(v - hi), and every k8 step issues
+// three wgmma m64n64k8 tf32 MMAs into one fp32 accumulator, always in the order lo·hi, hi·lo, hi·hi
+// (the lo·lo term, |lo·lo| <= 2^-22 |a·b|, is dropped).  The accumulator restarts at every 32-wide K
+// chunk and its sum is added to an fp32 register total, in chunk order.
+//
+// CTA: 256 threads = two warpgroups, a 128 x 64 tile of C (each warpgroup 64 rows), K in chunks of 32.
+// Every thread gathers: a chunk's A (128 rows) and B (64 rows) go to registers, are split, and are
+// stored as four K-major planes (A hi, A lo, B hi, B lo; rows of 32 tf32 = 128 B, 128-byte swizzle)
+// into one of two ring stages.  The gather of chunk k + 1 runs while the MMAs of chunk k are in flight.
 //
 // Every reduction runs in a fixed order and no kernel uses floating-point atomics, so two calls give
 // the same bits:
@@ -27,10 +37,12 @@
 namespace opp {
 namespace {
 
-constexpr int kBM = 128, kBN = 64, kBK = 16, kThreads = 256;
-constexpr int kPadA = kBM + 4, kPadB = kBN + 4;     // shared rows padded against bank conflicts
-constexpr int kWgradGroup = 2048;                   // output pixels per wgrad partial
-constexpr int kBnChunk = 4096;                      // pixels per BatchNorm partial
+constexpr int kBM = 128, kBN = 64, kBK = 32, kThreads = 256;
+constexpr int kWgradGroup = 2048;                          // output pixels per wgrad partial
+constexpr int kPlaneA = kBM * kBK * 4, kPlaneB = kBN * kBK * 4;
+constexpr int kStage = 2 * kPlaneA + 2 * kPlaneB;          // A hi, A lo, B hi, B lo: 48 KiB
+constexpr int kSmem = 2 * kStage + 1024;                   // two stages + 1024-byte alignment slack
+constexpr int kBnChunk = 4096;                             // pixels per BatchNorm partial
 constexpr float kLeakySlope = 0.01f;
 
 enum { kFwd = 0, kDgrad = 1, kWgrad = 2 };
@@ -40,18 +52,63 @@ struct ConvGeo {
   int batches, c_in, h, w, c_out, ho, wo, stride, pad;
 };
 
-// One implicit-GEMM CTA: a kBM x kBN tile of C = A B^T, K in chunks of kBK, 8 x 4 per thread,
-// shared operands double-buffered, the next chunk prefetched into registers.
-//   kFwd:   M = output pixels, N = c_out, K = c_in·KS², C -> y (NCHW)
-//   kDgrad: M = input pixels,  N = c_in,  K = c_out·KS², C -> dx (NCHW, += when accumulate)
-//   kWgrad: M = c_out, N = c_in·KS², K = the output pixels of group blockIdx.z, C -> part[z]
+
+__device__ __forceinline__ uint32_t tf32_rna(float v) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+  return r;
+}
+
+// byte offset of (row, 16-byte column chunk) in a K-major plane of 128-byte rows, 128-byte swizzle
+__device__ __forceinline__ uint32_t swz(int row, int chunk) {
+  return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4));
+}
+
+// four consecutive K values of one row, split into hi and lo, into the hi plane and the lo plane
+__device__ __forceinline__ void store_split4(uint32_t hi_plane, uint32_t lo_plane, uint32_t off, const float* v) {
+  uint4 h, l;
+  h.x = tf32_rna(v[0]), h.y = tf32_rna(v[1]), h.z = tf32_rna(v[2]), h.w = tf32_rna(v[3]);
+  l.x = tf32_rna(v[0] - __uint_as_float(h.x)), l.y = tf32_rna(v[1] - __uint_as_float(h.y));
+  l.z = tf32_rna(v[2] - __uint_as_float(h.z)), l.w = tf32_rna(v[3] - __uint_as_float(h.w));
+  sts128(hi_plane + off, h);
+  sts128(lo_plane + off, l);
+}
+
+#define OPP_WG_ACC8(i)                                                                              \
+  "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]),    \
+      "+f"(d[i + 6]), "+f"(d[i + 7])
+// d = A B^T (+ d when accumulate) for one m64n64k8 tf32 step, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], uint64_t a_desc, uint64_t b_desc,
+                                                    int accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1;\n\t"
+      "}\n"
+      : OPP_WG_ACC8(0), OPP_WG_ACC8(8), OPP_WG_ACC8(16), OPP_WG_ACC8(24)
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
+#undef OPP_WG_ACC8
+
+// One CTA: a kBM x kBN tile of C = A B^T over K [k_begin, k_end).
+//   kFwd:   C -> y (NCHW);  kDgrad: C -> dx (NCHW, += when accumulate);  kWgrad: C -> part[blockIdx.z]
+// Gather mapping per chunk:
+//   kFwd / kDgrad A: row m = tid % 128 (consecutive pixels across a warp), K quads tid / 128 + 2 i;
+//   B (all modes) and kWgrad A: K quad tid % 8, rows tid / 8 + 32 i (128 contiguous bytes per row).
 template <int MODE, int KS>
-__global__ void __launch_bounds__(kThreads) bb_conv_kernel(const float* __restrict__ x, const float* __restrict__ wt,
-                                                           const float* __restrict__ dy, ConvGeo g, int pix0,
-                                                           int npix, int accumulate, float* __restrict__ out) {
+__global__ void __launch_bounds__(kThreads, 2) bb_conv_kernel(const float* __restrict__ x,
+                                                                 const float* __restrict__ wt,
+                                                                 const float* __restrict__ dy, ConvGeo g, int pix0,
+                                                                 int npix, int accumulate, float* __restrict__ out) {
   constexpr int KK = KS * KS;
-  __shared__ __align__(16) float As[2][kBK][kPadA];
-  __shared__ __align__(16) float Bs[2][kBK][kPadB];
+  constexpr int kAQ = 4, kBQ = 2;                          // quads of 4 values per thread: A, B
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int tid = threadIdx.x;
   const int hw = g.h * g.w, howo = g.ho * g.wo;
   int M, N, k_begin, k_end;
@@ -65,10 +122,9 @@ __global__ void __launch_bounds__(kThreads) bb_conv_kernel(const float* __restri
     k_end = min(k_begin + kWgradGroup, pix0 + npix);
   }
   const int m0 = blockIdx.y * kBM, n0 = blockIdx.x * kBN;
+  const int q = tid & 7;                                   // K quad of the row-per-8-threads loads
 
-  // loader state --------------------------------------------------------------------------------
-  // kFwd / kDgrad A: one pixel per thread (m = tid % 128), k rows tid / 128 + 2j.
-  // B (all modes) and kWgrad A: k = tid % 16, rows tid / 16 + 16j.
+  // loader state ----------------------------------------------------------------------------------
   int a_b = 0, a_y = 0, a_x = 0;
   bool a_ok = false;
   if constexpr (MODE != kWgrad) {
@@ -81,152 +137,170 @@ __global__ void __launch_bounds__(kThreads) bb_conv_kernel(const float* __restri
     a_y = p / pw;
     a_x = p - a_y * pw;
   }
-  int bw_ci[4], bw_ky[4], bw_kx[4];     // kWgrad B rows: (ci, tap) of n
+  int bw_ci[kBQ], bw_ky[kBQ], bw_kx[kBQ];                  // kWgrad B rows: (ci, tap) of n
   if constexpr (MODE == kWgrad) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int n = n0 + (tid >> 4) + 16 * j;
+    for (int i = 0; i < kBQ; ++i) {
+      const int n = n0 + (tid >> 3) + 32 * i;
       const int ci = n / KK, tap = n - ci * KK;
-      bw_ci[j] = n < N ? ci : -1;
-      bw_ky[j] = tap / KS;
-      bw_kx[j] = tap - (tap / KS) * KS;
+      bw_ci[i] = n < N ? ci : -1;
+      bw_ky[i] = tap / KS;
+      bw_kx[i] = tap - (tap / KS) * KS;
     }
   }
 
-  float ra[8], rb[4];
+  float ra[kAQ][4], rb[kBQ][4];
   auto load = [&](int kc) {
-    if constexpr (MODE == kFwd) {
+    if constexpr (MODE == kFwd || MODE == kDgrad) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int k = kc + (tid >> 7) + 2 * j;
-        float v = 0.f;
-        if (a_ok && k < k_end) {
-          const int ci = k / KK, tap = k - ci * KK, ky = tap / KS, kx = tap - ky * KS;
-          const int iy = a_y * g.stride - g.pad + ky, ix = a_x * g.stride - g.pad + kx;
-          if (iy >= 0 && iy < g.h && ix >= 0 && ix < g.w) v = x[((size_t)a_b * g.c_in + ci) * hw + iy * g.w + ix];
-        }
-        ra[j] = v;
-      }
+      for (int i = 0; i < kAQ; ++i)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int k = kc + (tid & 15), n = n0 + (tid >> 4) + 16 * j;
-        rb[j] = (n < N && k < k_end) ? wt[(size_t)n * k_end + k] : 0.f;
-      }
-    } else if constexpr (MODE == kDgrad) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int k = kc + (tid >> 7) + 2 * j;
-        float v = 0.f;
-        if (a_ok && k < k_end) {
-          const int co = k / KK, tap = k - co * KK, ky = tap / KS, kx = tap - ky * KS;
-          const int ty = a_y + g.pad - ky, tx = a_x + g.pad - kx;
-          if (ty >= 0 && tx >= 0 && ty % g.stride == 0 && tx % g.stride == 0) {
-            const int oy = ty / g.stride, ox = tx / g.stride;
-            if (oy < g.ho && ox < g.wo) v = dy[((size_t)a_b * g.c_out + co) * howo + oy * g.wo + ox];
+        for (int e = 0; e < 4; ++e) {
+          const int k = kc + 4 * ((tid >> 7) + 2 * i) + e;
+          float v = 0.f;
+          if (a_ok && k < k_end) {
+            const int c = k / KK, tap = k - c * KK, ky = tap / KS, kx = tap - ky * KS;
+            if constexpr (MODE == kFwd) {
+              const int iy = a_y * g.stride - g.pad + ky, ix = a_x * g.stride - g.pad + kx;
+              if (iy >= 0 && iy < g.h && ix >= 0 && ix < g.w) v = x[((size_t)a_b * g.c_in + c) * hw + iy * g.w + ix];
+            } else {
+              const int ty = a_y + g.pad - ky, tx = a_x + g.pad - kx;
+              if (ty >= 0 && tx >= 0 && ty % g.stride == 0 && tx % g.stride == 0) {
+                const int oy = ty / g.stride, ox = tx / g.stride;
+                if (oy < g.ho && ox < g.wo) v = dy[((size_t)a_b * g.c_out + c) * howo + oy * g.wo + ox];
+              }
+            }
           }
+          ra[i][e] = v;
         }
-        ra[j] = v;
-      }
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int k = kc + (tid & 15), n = n0 + (tid >> 4) + 16 * j;
-        float v = 0.f;
-        if (n < N && k < k_end) {
-          const int co = k / KK, tap = k - co * KK;
-          v = wt[((size_t)co * g.c_in + n) * KK + tap];
+      for (int i = 0; i < kBQ; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int k = kc + 4 * q + e, n = n0 + (tid >> 3) + 32 * i;
+          float v = 0.f;
+          if (n < N && k < k_end) {
+            if constexpr (MODE == kFwd) {
+              v = wt[n * k_end + k];                      // < 2^31 (conv_geo)
+            } else {
+              const int co = k / KK, tap = k - co * KK;
+              v = wt[((size_t)co * g.c_in + n) * KK + tap];
+            }
+          }
+          rb[i][e] = v;
         }
-        rb[j] = v;
-      }
     } else {
-      const int k = kc + (tid & 15);
-      const bool kok = k < k_end;
-      const int b = kok ? k / howo : 0;
-      const int p = kok ? k - b * howo : 0;
-      const int oy = p / g.wo, ox = p - oy * g.wo;
+      // the four output pixels of this thread's quad, shared by its A and B rows
+      int pb[4], pp[4], py[4], px[4];
+      bool pok[4];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int m = m0 + (tid >> 4) + 16 * j;
-        ra[j] = (kok && m < M) ? dy[((size_t)b * g.c_out + m) * howo + p] : 0.f;
+      for (int e = 0; e < 4; ++e) {
+        const int k = kc + 4 * q + e;
+        pok[e] = k < k_end;
+        pb[e] = pok[e] ? k / howo : 0;
+        pp[e] = pok[e] ? k - pb[e] * howo : 0;
+        py[e] = pp[e] / g.wo;
+        px[e] = pp[e] - py[e] * g.wo;
       }
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float v = 0.f;
-        if (kok && bw_ci[j] >= 0) {
-          const int iy = oy * g.stride - g.pad + bw_ky[j], ix = ox * g.stride - g.pad + bw_kx[j];
-          if (iy >= 0 && iy < g.h && ix >= 0 && ix < g.w)
-            v = x[((size_t)b * g.c_in + bw_ci[j]) * hw + iy * g.w + ix];
+      for (int i = 0; i < kAQ; ++i) {
+        const int m = m0 + (tid >> 3) + 32 * i;
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          ra[i][e] = (pok[e] && m < M) ? dy[((size_t)pb[e] * g.c_out + m) * howo + pp[e]] : 0.f;
+      }
+#pragma unroll
+      for (int i = 0; i < kBQ; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float v = 0.f;
+          if (pok[e] && bw_ci[i] >= 0) {
+            const int iy = py[e] * g.stride - g.pad + bw_ky[i], ix = px[e] * g.stride - g.pad + bw_kx[i];
+            if (iy >= 0 && iy < g.h && ix >= 0 && ix < g.w)
+              v = x[((size_t)pb[e] * g.c_in + bw_ci[i]) * hw + iy * g.w + ix];
+          }
+          rb[i][e] = v;
         }
-        rb[j] = v;
-      }
     }
   };
   auto store = [&](int s) {
-    if constexpr (MODE == kWgrad) {
+    const uint32_t a_hi = base + s * kStage, a_lo = a_hi + kPlaneA;
+    const uint32_t b_hi = a_lo + kPlaneA, b_lo = b_hi + kPlaneB;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) As[s][tid & 15][(tid >> 4) + 16 * j] = ra[j];
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) As[s][(tid >> 7) + 2 * j][tid & (kBM - 1)] = ra[j];
+    for (int i = 0; i < kAQ; ++i) {
+      const uint32_t off = MODE == kWgrad ? swz((tid >> 3) + 32 * i, q) : swz(tid & (kBM - 1), (tid >> 7) + 2 * i);
+      store_split4(a_hi, a_lo, off, ra[i]);
     }
 #pragma unroll
-    for (int j = 0; j < 4; ++j) Bs[s][tid & 15][(tid >> 4) + 16 * j] = rb[j];
+    for (int i = 0; i < kBQ; ++i) store_split4(b_hi, b_lo, swz((tid >> 3) + 32 * i, q), rb[i]);
+    fence_proxy_async_smem();                            // generic stores -> the MMAs' async-proxy reads
   };
 
   // main loop -------------------------------------------------------------------------------------
-  const int tm = tid >> 4, tn = tid & 15;
-  float acc[8][4];
+  // The wgmma accumulator rounds toward zero once per instruction (DESIGN §3), a bias that grows with
+  // the number of accumulating MMAs.  So each chunk's 12 MMAs start from zero in acc, and the chunk sum
+  // is added to tot with an IEEE fp32 add: one round-to-nearest add per 32 K values.
+  const int wg = tid >> 7;
+  float acc[32], tot[32];
 #pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+  for (int i = 0; i < 32; ++i) tot[i] = 0.f;
   int s = 0;
   load(k_begin);
   store(0);
   __syncthreads();
   for (int kc = k_begin; kc < k_end; kc += kBK) {
     const bool more = kc + kBK < k_end;
-    if (more) load(kc + kBK);
+    const uint32_t a_hi = base + s * kStage + wg * (kPlaneA / 2), a_lo = a_hi + kPlaneA;
+    const uint32_t b_hi = base + s * kStage + 2 * kPlaneA, b_lo = b_hi + kPlaneB;
+    wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < kBK; ++kk) {
-      const float4 a0 = *reinterpret_cast<const float4*>(&As[s][kk][tm * 4]);
-      const float4 a1 = *reinterpret_cast<const float4*>(&As[s][kk][64 + tm * 4]);
-      const float4 b0 = *reinterpret_cast<const float4*>(&Bs[s][kk][tn * 4]);
-      const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-      const float bv[4] = {b0.x, b0.y, b0.z, b0.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+    for (int kk = 0; kk < kBK / 8; ++kk) {
+      const uint32_t o = kk * 32;                        // one k8 step: 32 bytes along the row
+      wgmma_m64n64k8_tf32(acc, make_kmajor_sw128_desc(a_lo + o), make_kmajor_sw128_desc(b_hi + o), kk);
+      wgmma_m64n64k8_tf32(acc, make_kmajor_sw128_desc(a_hi + o), make_kmajor_sw128_desc(b_lo + o), 1);
+      wgmma_m64n64k8_tf32(acc, make_kmajor_sw128_desc(a_hi + o), make_kmajor_sw128_desc(b_hi + o), 1);
     }
+    wgmma_commit();
     if (more) {
+      load(kc + kBK);                                    // the other stage was released by the last wait
       store(s ^ 1);
-      __syncthreads();
-      s ^= 1;
     }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) tot[i] += acc[i];
+    __syncthreads();
+    s ^= 1;
   }
 
-  // epilogue --------------------------------------------------------------------------------------
+  // epilogue: accumulator element 4 j + 2 h + c is row r0 + 8 h, column 8 j + c0 + c --------------------
+  const int warp = (tid >> 5) & 3, lane = tid & 31;
+  const int r0 = m0 + 64 * wg + 16 * warp + (lane >> 2), c0 = n0 + 2 * (lane & 3);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int m = m0 + (i < 4 ? tm * 4 + i : 64 + tm * 4 + i - 4);
+  for (int h = 0; h < 2; ++h) {
+    const int m = r0 + 8 * h;
     if (m >= M) continue;
     if constexpr (MODE == kWgrad) {
       float* o = out + (size_t)blockIdx.z * M * N + (size_t)m * N;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int n = n0 + tn * 4 + j;
-        if (n < N) o[n] = acc[i][j];
-      }
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int n = c0 + 8 * j + c;
+          if (n < N) o[n] = tot[4 * j + 2 * h + c];
+        }
     } else {
       const int plane = MODE == kFwd ? howo : hw;
       const int b = m / plane, p = m - b * plane;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int n = n0 + tn * 4 + j;
-        if (n >= N) continue;
-        float* o = out + ((size_t)b * N + n) * plane + p;
-        *o = (MODE == kDgrad && accumulate) ? *o + acc[i][j] : acc[i][j];
-      }
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int n = c0 + 8 * j + c;
+          if (n >= N) continue;
+          float* o = out + ((size_t)b * N + n) * plane + p;
+          const float v = tot[4 * j + 2 * h + c];
+          *o = (MODE == kDgrad && accumulate) ? *o + v : v;
+        }
     }
   }
 }
@@ -237,7 +311,7 @@ __global__ void bb_reduce_kernel(const float* __restrict__ part, int parts, int 
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float s = accumulate ? dw[i] : 0.f;
-  for (int q = 0; q < parts; ++q) s += part[(size_t)q * n + i];
+  for (int p = 0; p < parts; ++p) s += part[(size_t)p * n + i];
   dw[i] = s;
 }
 
@@ -450,13 +524,22 @@ int conv_geo(int batches, int c_in, int h, int w, int c_out, int ksize, int stri
   return OPP_OK;
 }
 
+template <int MODE, int KS>
+cudaError_t launch_ks(dim3 grid, cudaStream_t st, const float* x, const float* w, const float* dy, const ConvGeo& g,
+                      int pix0, int npix, int accumulate, float* out) {
+  static const cudaError_t attr =
+      cudaFuncSetAttribute(bb_conv_kernel<MODE, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+  if (attr != cudaSuccess) return attr;
+  bb_conv_kernel<MODE, KS><<<grid, kThreads, kSmem, st>>>(x, w, dy, g, pix0, npix, accumulate, out);
+  return cudaGetLastError();
+}
+
 template <int MODE>
 cudaError_t launch_conv(int ksize, dim3 grid, cudaStream_t st, const float* x, const float* w, const float* dy,
                         const ConvGeo& g, int pix0, int npix, int accumulate, float* out) {
-  if (ksize == 1) bb_conv_kernel<MODE, 1><<<grid, kThreads, 0, st>>>(x, w, dy, g, pix0, npix, accumulate, out);
-  if (ksize == 3) bb_conv_kernel<MODE, 3><<<grid, kThreads, 0, st>>>(x, w, dy, g, pix0, npix, accumulate, out);
-  if (ksize == 7) bb_conv_kernel<MODE, 7><<<grid, kThreads, 0, st>>>(x, w, dy, g, pix0, npix, accumulate, out);
-  return cudaGetLastError();
+  if (ksize == 1) return launch_ks<MODE, 1>(grid, st, x, w, dy, g, pix0, npix, accumulate, out);
+  if (ksize == 3) return launch_ks<MODE, 3>(grid, st, x, w, dy, g, pix0, npix, accumulate, out);
+  return launch_ks<MODE, 7>(grid, st, x, w, dy, g, pix0, npix, accumulate, out);
 }
 
 int bn_parts(int batches, int hw) { return batches * ((hw + kBnChunk - 1) / kBnChunk); }

@@ -662,8 +662,8 @@ class OnePosePlus_model(_Engine):
         # opp_coarse_tf_* kernels forward and backward, recomputing one layer at a time (train_coarse_tf.py)
         self.coarse_transformer_train_mode = os.environ.get("OPP_B200_COARSE_TF_TRAIN", "autograd")
         # backbone of .train() on CUDA: "autograd" = train_path.backbone (cuDNN), "kernels" = the
-        # opp_backbone_train_* kernels forward and backward, recomputing one segment at a time (train_backbone.py),
-        # "tf32x3" = the same with the convolutions on the tensor cores in 3xTF32
+        # opp_backbone_train_* kernels forward and backward (convolutions on the tensor cores in 3xTF32),
+        # recomputing one segment at a time (train_backbone.py)
         self.backbone_train_mode = os.environ.get("OPP_B200_BACKBONE_TRAIN", "autograd")
         # keypoint encoder of .train() on CUDA: "autograd" = train_path.keypoint_encoding, "kernels" = the
         # opp_kpt_train_* kernels forward and backward, recomputing each point's MLP (train_kpt.py)

@@ -630,33 +630,28 @@ def conv_out_hw(h, w, k, stride):
     return (h + 2 * pad - k) // stride + 1, (w + 2 * pad - k) // stride + 1
 
 
-def _tc(name, tf32x3):
-    """The fp32 CUDA-core entry point, or its 3xTF32 tensor-core twin (opp_train_backbone_tc.cu)."""
-    return name + "_tf32x3" if tf32x3 else name
-
-
-def backbone_conv(x, w, stride, y, tf32x3=False):
-    """y [B, c_out, ho, wo] = conv2d(x, w, stride, padding=k // 2); tf32x3: on the tensor cores."""
+def backbone_conv(x, w, stride, y):
+    """y [B, c_out, ho, wo] = conv2d(x, w, stride, padding=k // 2)."""
     B, C, H, W, co, k, s = _conv_args(x, w, stride)
     _chk(y, torch.float32, "y")
     if tuple(y.shape) != (B, co, *conv_out_hw(H, W, k, s)):
         raise ValueError(f"y has shape {tuple(y.shape)}")
-    call(_tc("opp_backbone_train_conv", tf32x3), ptr(x), ptr(w), B, C, H, W, co, k, s, ptr(y), stream())
+    call("opp_backbone_train_conv", ptr(x), ptr(w), B, C, H, W, co, k, s, ptr(y), stream())
 
 
-def backbone_conv_dgrad(dy, w, stride, dx, accumulate, tf32x3=False):
+def backbone_conv_dgrad(dy, w, stride, dx, accumulate):
     """dx [B, c_in, h, w] (+)= the input gradient of conv2d(., w, stride) for the output gradient dy."""
     B, C, H, W, co, k, s = _conv_args(dx, w, stride)
     _chk(dy, torch.float32, "dy")
     if tuple(dy.shape) != (B, co, *conv_out_hw(H, W, k, s)):
         raise ValueError(f"dy has shape {tuple(dy.shape)}")
-    call(_tc("opp_backbone_train_conv_dgrad", tf32x3), ptr(dy), ptr(w), B, C, H, W, co, k, s, ptr(dx),
+    call("opp_backbone_train_conv_dgrad", ptr(dy), ptr(w), B, C, H, W, co, k, s, ptr(dx),
          int(accumulate), stream())
 
 
-def backbone_conv_wgrad(x, dy, stride, dw, part, pix0, npix, accumulate, tf32x3=False):
+def backbone_conv_wgrad(x, dy, stride, dw, part, pix0, npix, accumulate):
     """dw (+)= the weight gradient over output pixels [pix0, pix0 + npix) of the flat (b, oy, ox) index;
-    part fp32 with at least ceil(npix / group) * dw.numel() entries (the same group in both forms)."""
+    part fp32 with at least ceil(npix / group) * dw.numel() entries."""
     B, C, H, W, co, k, s = _conv_args(x, dw, stride)
     _chk(dy, torch.float32, "dy")
     _chk(part, torch.float32, "part")
@@ -665,7 +660,7 @@ def backbone_conv_wgrad(x, dy, stride, dw, part, pix0, npix, accumulate, tf32x3=
     group = backbone_wgrad_group()
     if part.numel() < -(-npix // group) * dw.numel():
         raise ValueError("wgrad partial buffer too small")
-    call(_tc("opp_backbone_train_conv_wgrad", tf32x3), ptr(x), ptr(dy), B, C, H, W, co, k, s, int(pix0), int(npix),
+    call("opp_backbone_train_conv_wgrad", ptr(x), ptr(dy), B, C, H, W, co, k, s, int(pix0), int(npix),
          ptr(part), ptr(dw), int(accumulate), stream())
 
 

@@ -1,12 +1,11 @@
-"""ResNet-FPN backbone of the training forward on the device (model.backbone_train_mode "kernels" or
-"tf32x3", CUDA, train mode).
+"""ResNet-FPN backbone of the training forward on the device (model.backbone_train_mode "kernels",
+CUDA, train mode).
 
 One autograd Function replaces train_path.backbone(model.backbone, img): the 22 convolutions, the 17
 BatchNorms with their ReLU / LeakyReLU and residual adds, and the two bilinear x2 upsample-adds of the
-FPN, forward and backward in fp32 on the CUDA cores (csrc/opp_train_backbone.cu).  In mode "tf32x3" the
-convolutions' forward, data gradient and weight gradient run on the tensor cores instead, in 3xTF32
-(each operand split into tf32 hi + lo, three MMAs per k8 step: csrc/opp_train_backbone_tc.cu); the
-rest, the segment walk and the memory plan are the same in both modes.
+FPN, forward and backward (csrc/opp_train_backbone.cu).  The convolutions' forward, data gradient and
+weight gradient run on the tensor cores in 3xTF32 (each operand split into tf32 hi + lo, three MMAs
+per k8 step); the rest runs in fp32.
 
 BatchNorm follows each module's own .training: batch statistics over N·H·W (biased variance, the
 module's eps), with running_mean / running_var / num_batches_tracked updated in place once per forward
@@ -25,8 +24,7 @@ import torch
 
 from . import ops
 
-MODES = ("autograd", "kernels", "tf32x3")
-DEVICE_MODES = ("kernels", "tf32x3")
+MODES = ("autograd", "kernels")
 WGRAD_SLICE_GROUPS = 32      # partials of one opp_backbone_train_conv_wgrad call (44 MiB at 196 x 196 x 3 x 3)
 
 BLOCKS = ("layer1.0", "layer1.1", "layer2.0", "layer2.1", "layer3.0", "layer3.1")
@@ -74,7 +72,7 @@ def use_kernels(model, data):
     mode = model.backbone_train_mode
     if mode not in MODES:
         raise ValueError(f"backbone_train_mode must be one of {MODES}, not {mode!r}")
-    if mode not in DEVICE_MODES or not model.training or not data["query_image"].is_cuda:
+    if mode != "kernels" or not model.training or not data["query_image"].is_cuda:
         return False
     check(model, data)
     return True
@@ -94,9 +92,8 @@ def _empty(shape, dev):
 class _Net:
     """The parameters by name, the BN statistics and the kernel calls of one forward / backward."""
 
-    def __init__(self, bb, tensors, dev, mode="kernels"):
+    def __init__(self, bb, tensors, dev):
         self.dev = dev
-        self.tf32x3 = mode == "tf32x3"       # the convolutions on the tensor cores (3xTF32)
         self.w = {n: t.detach().contiguous() for n, t in zip(CONVS, tensors[:len(CONVS)])}
         gb = tensors[len(CONVS):]
         self.gamma = {n: gb[2 * i].detach().contiguous() for i, n in enumerate(BNS)}
@@ -113,7 +110,7 @@ class _Net:
         w = self.w[name]
         ho, wo = ops.conv_out_hw(H, W, w.shape[2], self.stride[name])
         y = _empty((B, w.shape[0], ho, wo), self.dev)
-        ops.backbone_conv(x, w, self.stride[name], y, tf32x3=self.tf32x3)
+        ops.backbone_conv(x, w, self.stride[name], y)
         return y
 
     def _stats(self, name, h):
@@ -183,13 +180,12 @@ class _Net:
         step = WGRAD_SLICE_GROUPS * group
         part = _empty(min(pixels, step) // group * w.numel() + w.numel(), self.dev)
         for p0 in range(0, pixels, step):
-            ops.backbone_conv_wgrad(x, dy, self.stride[name], dw, part, p0, min(step, pixels - p0), True,
-                                    tf32x3=self.tf32x3)
+            ops.backbone_conv_wgrad(x, dy, self.stride[name], dw, part, p0, min(step, pixels - p0), True)
         self.grads[name] = dw
 
     def dgrad(self, name, dy, x_shape, out=None, accumulate=False):
         dx = _empty(x_shape, self.dev) if out is None else out
-        ops.backbone_conv_dgrad(dy, self.w[name], self.stride[name], dx, accumulate, tf32x3=self.tf32x3)
+        ops.backbone_conv_dgrad(dy, self.w[name], self.stride[name], dx, accumulate)
         return dx
 
     def bn_bwd(self, name, h, y, dy, act, dres=None):
@@ -255,13 +251,13 @@ _SEGMENTS = (
 
 class BackboneStage(torch.autograd.Function):
     """(x3_out [B, 256, H/8, W/8], x1_out [B, 128, H/2, W/2]) = train_path.backbone(bb, img) on the
-    kernels.  Inputs: the backbone module (structure, BN modes and running statistics), the device mode
-    ("kernels" or "tf32x3"), the image [B, 1, H, W], then params(bb)."""
+    kernels.  Inputs: the backbone module (structure, BN modes and running statistics), the image
+    [B, 1, H, W], then params(bb)."""
 
     @staticmethod
-    def forward(ctx, bb, mode, img, *tensors):
+    def forward(ctx, bb, img, *tensors):
         dev = img.device
-        net = _Net(bb, tensors, dev, mode)
+        net = _Net(bb, tensors, dev)
         net.record = True
         img = img.detach().contiguous()
         x0 = net.bn("bn1", net.conv("conv1", img), "relu")
@@ -276,14 +272,13 @@ class BackboneStage(torch.autograd.Function):
         ctx.batch = tuple(net.stats[n][2] for n in BNS)
         ctx.save_for_backward(img, *segs, x3_out, x2_out, *stats, *tensors)
         ctx.bb = bb
-        ctx.mode = mode
         ctx.set_materialize_grads(False)
         return x3_out, x1_out
 
     @staticmethod
     def backward(ctx, d_x3_out, d_x1_out):
-        need = ctx.needs_input_grad[3:]
-        nothing = (None, None, None) + (None,) * len(need)
+        need = ctx.needs_input_grad[2:]
+        nothing = (None, None) + (None,) * len(need)
         if not any(need) or (d_x3_out is None and d_x1_out is None):
             return nothing
         saved = ctx.saved_tensors
@@ -291,7 +286,7 @@ class BackboneStage(torch.autograd.Function):
         stats = saved[10:10 + 2 * len(BNS)]
         tensors = saved[10 + 2 * len(BNS):]
         dev = img.device
-        net = _Net(ctx.bb, tensors, dev, ctx.mode)
+        net = _Net(ctx.bb, tensors, dev)
         net.stats = {n: (stats[2 * i], stats[2 * i + 1], ctx.batch[i]) for i, n in enumerate(BNS)}
         net.grads = {}
         need_conv = dict(zip(CONVS, need[:len(CONVS)]))
@@ -347,12 +342,9 @@ class BackboneStage(torch.autograd.Function):
             dgb = net.grads.get(n)
             grads += [dgb[0] if dgb is not None and need[len(CONVS) + 2 * i] else None,
                       dgb[1] if dgb is not None and need[len(CONVS) + 2 * i + 1] else None]
-        return (None, None, None, *grads)
+        return (None, None, *grads)
 
 
-def backbone(bb, img, mode="kernels"):
-    """train_path.backbone(bb, img) on the kernels of a device mode ("kernels": fp32 CUDA cores, "tf32x3":
-    3xTF32 tensor cores): (feat_c [B, 256, H/8, W/8], feat_f [B, 128, H/2, W/2])."""
-    if mode not in DEVICE_MODES:
-        raise ValueError(f"backbone device mode must be one of {DEVICE_MODES}, not {mode!r}")
-    return BackboneStage.apply(bb, mode, img, *params(bb))
+def backbone(bb, img):
+    """train_path.backbone(bb, img) on the kernels: (feat_c [B, 256, H/8, W/8], feat_f [B, 128, H/2, W/2])."""
+    return BackboneStage.apply(bb, img, *params(bb))

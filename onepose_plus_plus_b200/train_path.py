@@ -19,10 +19,9 @@ tensors the fine level (fine_preprocess -> loftr_fine -> fine_matching) runs on 
 opp_fine_train_* kernels instead (train_fine.py), and with model.coarse_transformer_train_mode ==
 "kernels" the coarse transformer runs on the opp_coarse_tf_* kernels (train_coarse_tf.py).  With
 model.backbone_train_mode == "kernels" the ResNet-FPN backbone runs on the opp_backbone_train_*
-kernels, BatchNorm following each module's .training (train_backbone.py); "tf32x3" runs its
-convolutions on the tensor cores in 3xTF32 (opp_backbone_train_conv*_tf32x3) and the rest the same way.  With
-model.kpt_encoder_train_mode == "kernels" the keypoint-encoder MLP runs on the opp_kpt_train_* kernels
-(train_kpt.py).  The ground truth the padding draws from is data["conf_matrix_gt"] or, in its place, the
+kernels, its convolutions on the tensor cores in 3xTF32, BatchNorm following each module's .training
+(train_backbone.py).  With model.kpt_encoder_train_mode == "kernels" the keypoint-encoder MLP runs on
+the opp_kpt_train_* kernels (train_kpt.py).  The ground truth the padding draws from is data["conf_matrix_gt"] or, in its place, the
 correspondence list data["gt_sparse"] (train_gt.py).
 
 Every function cites the reference lines it follows.
@@ -330,7 +329,7 @@ def forward_train(model, data):
     kpt_kernels = train_kpt.use_kernels(model, data)
     data.update({"bs": img.size(0), "q_hw_i": img.shape[2:]})
     if backbone_kernels:
-        feat_c, feat_f = train_backbone.backbone(model.backbone, img, model.backbone_train_mode)
+        feat_c, feat_f = train_backbone.backbone(model.backbone, img)
     else:
         feat_c, feat_f = backbone(model.backbone, img)
     data.update({"q_hw_c": feat_c.shape[2:], "q_hw_f": feat_f.shape[2:]})

@@ -1,16 +1,18 @@
 """Time and memory of the backbone of a training step, forward + backward, at the reference training
 shape (B = 4, 512 x 512), alternating in one process: train_path.backbone by autograd with PyTorch's
 default cudnn TF32, the same with TF32 off, and train_backbone.BackboneStage (the opp_backbone_train_*
-kernels).  A torch.profiler run times the dominant convolution (layer1_outconv2.0, 196 -> 196 3 x 3 at
-256 x 256) forward, dgrad and wgrad on the kernels.  A second JSON line times one whole model.train()
-forward + Loss + backward (B = 4, 512 x 512, N = 7000, planted) with every device mode on and with all
-of them off.  Card name, power limit and SM clock are read in the same call.
+kernels, convolutions in 3xTF32 on the tensor cores).  Two torch.profiler runs time the convolutions:
+the stage's launches summed per pass kind (forward / dgrad / wgrad, k), and the dominant convolution
+(layer1_outconv2.0, 196 -> 196 3 x 3 at 256 x 256) on its own.  A second JSON line times one whole
+model.train() forward + Loss + backward (B = 4, 512 x 512, N = 7000, planted) with every device mode on
+and with all of them off.  Card name, power limit and SM clock are read in the same call.
 
     python scripts/train_backbone_probe.py [--reps 10]
 """
 import argparse
 import json
 import os
+import re
 import subprocess
 import sys
 
@@ -25,7 +27,7 @@ from oracle import workload  # noqa: E402
 from onepose_plus_plus_b200 import OnePosePlus_model, losses, ops, train_backbone, train_gt, train_path  # noqa: E402
 from tests.test_train_gt_gpu import planted_gt  # noqa: E402
 
-FP32_PEAK = 67e12       # H100 SXM data sheet, dense FP32
+PASS = {"0": "fwd", "1": "dgrad", "2": "wgrad"}
 
 
 def _smi():
@@ -53,6 +55,22 @@ def _peak(fn):
     fn()
     torch.cuda.synchronize()
     return round((torch.cuda.max_memory_allocated() - base) / 2 ** 20, 1)
+
+
+def _by_pass(prof, n):
+    """{pass_k: ms per run} from bb_conv_kernel<MODE, KS>, and the wgrad's bb_reduce_kernel."""
+    out = {}
+    for ev in prof.key_averages():
+        m = re.search(r"bb_conv_kernel<(\d), (\d)>", ev.key)
+        if m:
+            key = f"{PASS[m.group(1)]}_k{m.group(2)}"
+        elif "bb_reduce" in ev.key:
+            key = "wgrad_reduce"
+        else:
+            continue
+        t = ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
+        out[key] = round(out.get(key, 0.0) + t / 1e3 / n, 3)
+    return out
 
 
 def stage(reps):
@@ -86,6 +104,14 @@ def stage(reps):
         t = sorted(times[name])
         out[name] = {"median_ms": round(t[len(t) // 2], 2), "min_ms": round(t[0], 2), "max_ms": round(t[-1], 2),
                      "peak_mib": peaks[name]}
+    # every convolution launch of the stage, per pass kind, under the profiler
+    runs["kernels"]()
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for _ in range(3):
+            runs["kernels"]()
+        torch.cuda.synchronize()
+    out["stage_conv_ms_by_pass"] = _by_pass(prof, 3)
     # the dominant convolution on its own, under the profiler
     x = torch.randn(4, 196, 256, 256, device="cuda")
     w = bb.layer1_outconv2[0].weight.detach().contiguous()
@@ -109,16 +135,12 @@ def stage(reps):
         torch.cuda.synchronize()
     smi_conv = _smi()
     flop = 2.0 * pixels * 196 * 196 * 9
-    kt = {}
-    for ev in prof.key_averages():
-        name = ev.key
-        if "bb_conv_kernel" in name or "bb_reduce" in name:
-            mode = "fwd" if "<0, 3>" in name else "dgrad" if "<1, 3>" in name else "wgrad"
-            t_ms = ev.device_time_total / 1e3 / 5 if hasattr(ev, "device_time_total") else ev.cuda_time_total / 1e3 / 5
-            kt[mode] = kt.get(mode, 0.0) + t_ms
-    out["layer1_outconv2.0"] = {"device": smi_conv, **{
-        m: {"ms": round(t, 3), "tflops": round(flop / (t * 1e-3) / 1e12, 2),
-            "share_of_67_tflops": round(flop / (t * 1e-3) / FP32_PEAK, 3)} for m, t in kt.items()}}
+    d = _by_pass(prof, 5)
+    kt = {"fwd": d.get("fwd_k3", 0.0), "dgrad": d.get("dgrad_k3", 0.0),
+          "wgrad": d.get("wgrad_k3", 0.0) + d.get("wgrad_reduce", 0.0)}
+    # fp32-equivalent algorithmic FLOPs (the 3xTF32 MMAs issue three times as many)
+    out["layer1_outconv2.0"] = {"device": smi_conv, "flop_per_pass": flop, **{
+        m: {"ms": round(t, 3), "tflops_fp32_equiv": round(flop / (t * 1e-3) / 1e12, 2)} for m, t in kt.items()}}
     return out
 
 
@@ -127,7 +149,8 @@ def _step(sd, gt, on):
     m.load_state_dict(sd, strict=True)
     m = m.cuda().train()
     m.conf_matrix_mode = "lazy" if on else "eager"
-    m.fine_train_mode = m.coarse_transformer_train_mode = m.backbone_train_mode = "kernels" if on else "autograd"
+    m.fine_train_mode = m.coarse_transformer_train_mode = m.backbone_train_mode = m.kpt_encoder_train_mode = \
+        "kernels" if on else "autograd"
     return m
 
 

@@ -28,9 +28,13 @@ def test_switch_defaults_and_errors(monkeypatch):
     monkeypatch.setenv("OPP_B200_BACKBONE_TRAIN", "kernels")
     assert _model().backbone_train_mode == "kernels"
     img = torch.zeros(1, 1, 64, 64)
-    m.backbone_train_mode = "cudnn"
+    for bad in ("cudnn", "tf32x3", "TF32x3", "tf32", ""):
+        m.backbone_train_mode = bad
+        with pytest.raises(ValueError, match="backbone_train_mode"):
+            train_backbone.use_kernels(m, {"query_image": img})
+    monkeypatch.setenv("OPP_B200_BACKBONE_TRAIN", "tf32x3")
     with pytest.raises(ValueError, match="backbone_train_mode"):
-        train_backbone.use_kernels(m, {"query_image": img})
+        train_backbone.use_kernels(_model(), {"query_image": img})
     m.backbone_train_mode = "kernels"
     assert not train_backbone.use_kernels(m, {"query_image": img})               # CPU tensors: unchanged path
     assert not train_backbone.use_kernels(m.eval(), {"query_image": img})
